@@ -1,4 +1,4 @@
-# B200 image for the framework (reference Dockerfile:1-17 rebuilt; its CMD had invalid JSON and
+# H100 image for the framework (reference Dockerfile:1-17 rebuilt; its CMD had invalid JSON and
 # a wrong relative path — both fixed here).
 FROM nvidia/cuda:12.9.0-devel-ubuntu24.04
 
@@ -10,7 +10,7 @@ RUN pip3 install --break-system-packages -r /app/requirements.txt
 
 COPY . /app/
 WORKDIR /app
-# compile the sm_100a libraries in-tree (nvcc cross-compiles; no GPU needed at build time)
+# compile the sm_90a libraries in-tree (nvcc cross-compiles; no GPU needed at build time)
 RUN python3 -c "import __graft_entry__ as g; g.build()"
 
 CMD ["bin/horovodrun", "-np", "4", "-H", "localhost:4", "python3", "app/torch_train.py"]

@@ -7,7 +7,7 @@ printed lines as the reference script (reference app/torch_train.py:208-312):
 With no arguments it trains the reference workload: LSTM(23 -> 256) regressor on the
 ES-futures window data, fp32, Adam lr=1e-6, per-rank batch 32, ceil(100 / world) epochs,
 gradient averaging through ``hvd.DistributedOptimizer`` and an initial
-``hvd.broadcast_parameters`` — but on the B200-native runtime instead of Horovod.
+``hvd.broadcast_parameters`` — but on the H100-native runtime instead of Horovod.
 
 Optional flags / environment variables (all default to the reference behaviour) select the
 [DRIVER] benchmark variants from BASELINE.json (``--model resnet18|resnet50|resnet152|
@@ -60,7 +60,7 @@ def parse_args(argv=None):
     p.add_argument("--cuda-graph", action="store_true",
                    default=env("B200DP_CUDA_GRAPH", "0") == "1",
                    help="capture the whole training step (fwd+bwd+fused allreduce/update) in one "
-                        "CUDA graph; B200-first answer for the launch-bound LSTM config")
+                        "CUDA graph; H100-first answer for the launch-bound LSTM config")
     p.add_argument("--data", default=env("B200DP_DATA", "data_es.csv"))
     return p.parse_args(argv)
 
@@ -114,7 +114,7 @@ if __name__ == "__main__":
         if loader_kind == "auto":
             loader_kind = "device" if use_cuda else "dataloader"
         if loader_kind == "device":
-            # B200-first: the whole (small) dataset is device resident; same sharded permutation
+            # H100-first: the whole (small) dataset is device resident; same sharded permutation
             # as DistributedSampler(seed=0) and, like the reference, set_epoch is never called.
             train_loader = DeviceBatchLoader(x_train, y_train, args.batch_size,
                                              num_replicas=hvd.size(), rank=hvd.rank(),

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Headline benchmark (BASELINE.json): images/sec for ResNet-50 synthetic-ImageNet bf16
-data-parallel training through ``hvd.DistributedOptimizer`` on N B200s of one node.
+data-parallel training through ``hvd.DistributedOptimizer`` on N H100s of one node.
 
     python bench.py --gpus 1 --steps 20 --warmup 5
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 \
@@ -13,15 +13,22 @@ full training steps (forward, backward, gradient allreduce, optimizer update).  
 the same metric through the public API with the per-step H2D copy of the inputs from pinned
 host memory and a D2H read of the loss inside the timed region.
 
-Baselines.  ``--impl reference`` would run the unmodified reference from ``baseline/_ref``; the
-reference is a single script that needs the ``horovod`` and ``GPUtil`` packages and a network
-download — none are installable offline (DESIGN.md §0) — so that arm prints
+``--dump-outputs DIR`` writes what the timed path computed in its last timed step, as float32 ``.npy``
+files: ``loss.npy`` (the step's loss) and ``params_sample.npy`` (the updated parameters, flattened in
+``model.parameters()`` order; a fixed seeded sample of 8M elements when the model is larger).  Inputs
+and initial weights are seeded, so two builds run with the same arguments can be compared output for
+output.  For ResNet training the step is bit-reproducible: every cross-CTA reduction on that path
+(BatchNorm statistics, split-K weight and bias gradients) sums in a fixed order.
+
+Baselines.  ``--impl reference`` would run the unmodified reference application; it is a single
+script that needs the ``horovod`` and ``GPUtil`` packages and a network download — none are
+installable offline (DESIGN.md §0) — so that arm prints
 ``{"impl": "reference", "unavailable": ...}``.  Because of that, the default (``ours``) run ALSO
 measures, in the same invocation on the same GPUs, the labelled **NCCL stand-in** (same model on
 library cuDNN/cuBLAS ops + NCCL DistributedDataParallel + the stock torch optimizer — NOT
 Horovod, NOT the reference) for a few steps and reports ``vs_baseline = value / stand-in`` with
 ``baseline_kind`` saying so; ``--impl nccl_standin`` runs only that arm.  At N > 1 the ``ours``
-run additionally executes a self-check: one step through the fused sm_100a engine vs the same
+run additionally executes a self-check: one step through the fused sm_90a engine vs the same
 step with ``torch.distributed.all_reduce`` + the torch optimizer on a cloned model, and a
 cross-rank bit-equality check of the updated parameters.
 """
@@ -54,21 +61,32 @@ def parse():
                    help="capture the whole training step (fwd+bwd+fused allreduce/update) in one CUDA "
                         "graph (ours only; 'auto' falls back to eager if capture fails)")
     p.add_argument("--lr", type=float, default=None)
+    p.add_argument("--dump-outputs", default=None, metavar="DIR",
+                   help="write the last timed step's loss and (sampled) updated parameters as .npy files")
     return p.parse_args()
 
 
+DUMP_MAX_ELEMS = 8 << 20          # 32 MB of float32 parameters
+
+
+def dump_outputs(out_dir, loss, model):
+    """Loss and updated parameters of the last timed step -> DIR/loss.npy, DIR/params_sample.npy."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), np.asarray([float(loss)], dtype=np.float32))
+    flat = torch.cat([p.detach().reshape(-1).float() for p in model.parameters()])
+    if flat.numel() > DUMP_MAX_ELEMS:
+        g = torch.Generator().manual_seed(0)
+        idx = torch.randperm(flat.numel(), generator=g)[:DUMP_MAX_ELEMS].sort().values
+        flat = flat[idx.to(flat.device)]
+    np.save(os.path.join(out_dir, "params_sample.npy"), flat.cpu().numpy())
+
+
 def reference_arm(args):
-    """Try to run the UNMODIFIED reference (baseline/_ref); report why it cannot run."""
+    """Report why the unmodified reference application cannot run here."""
     why = None
-    ref_dir = os.path.join(ROOT, "baseline", "_ref")
-    script = os.path.join(ref_dir, "app", "torch_train.py")
     try:
-        if not os.path.exists(script):
-            src = "/root/reference/app/torch_train.py"
-            if os.path.exists(src):
-                os.makedirs(os.path.dirname(script), exist_ok=True)
-                import shutil
-                shutil.copyfile(src, script)      # byte-identical copy, git-ignored
         missing = []
         for mod in ("horovod.torch", "GPUtil"):
             try:
@@ -76,11 +94,8 @@ def reference_arm(args):
             except Exception as e:  # noqa: BLE001
                 missing.append(f"{mod} ({type(e).__name__})")
         if missing:
-            why = ("reference is one script (no setup.py/pyproject: pip install of /root/reference "
-                   "fails) that imports " + ", ".join(missing) + " — not installable offline "
-                   "(not in /opt/wheelhouse); it also downloads its dataset at import time")
-        elif not os.path.exists(script):
-            why = "baseline/_ref/app/torch_train.py missing and /root/reference not mounted"
+            why = ("reference is one script (no setup.py/pyproject) that imports " + ", ".join(missing) +
+                   " — not installable offline; it also downloads its dataset at import time")
         else:
             why = ("reference script has no benchmark mode for BASELINE.json's metric "
                    "(ResNet-50 images/s); it only trains its LSTM on a downloaded CSV")
@@ -162,7 +177,7 @@ class SyntheticSeqBatches:
         return x.to(self.device, non_blocking=True), y.to(self.device, non_blocking=True)
 
 
-def run_arm(impl, wl, hvd, world, rank, steps, warmup, graph_mode, want_e2e, want_clocks):
+def run_arm(impl, wl, hvd, world, rank, steps, warmup, graph_mode, want_e2e, want_clocks, dump_dir=None):
     """Build the workload for ``impl`` and time ``steps`` training steps.  Returns a dict."""
     import torch
     from distributed_torch_horovod_gcp_b200.ops import functional as F2, counters
@@ -249,6 +264,8 @@ def run_arm(impl, wl, hvd, world, rank, steps, warmup, graph_mode, want_e2e, wan
     if graphed:
         launches = gs.kernels_per_replay * steps          # replayed graph nodes, counted at capture
     final_loss = float(loss)
+    if dump_dir is not None and rank == 0:
+        dump_outputs(dump_dir, loss, model)
 
     e2e = None
     if want_e2e:
@@ -293,7 +310,7 @@ def selfcheck(wl, hvd, world, rank):
     """Reduction + update check at N > 1, with IDENTICAL local gradients on both arms: one backward on
     a plain clone produces per-rank gradients; (a) ``dist.all_reduce`` (NCCL) average + the stock torch
     optimizer update the clone, (b) the same local gradients are placed in the fused engine's gradient
-    buckets and ONE fused sm_100a launch per bucket reduces them over NVLink and updates the model.
+    buckets and ONE fused sm_90a launch per bucket reduces them over NVLink and updates the model.
     Also checks that the updated replicas are bit-identical across ranks."""
     import copy
     import hashlib
@@ -334,7 +351,7 @@ def selfcheck(wl, hvd, world, rank):
     return {"max_rel_err": worst, "replicas_bit_identical": len(set(digests)) == 1,
             "expected": ("a few bf16 ulps (2^-8 = 0.0039 each): the NCCL arm rounds the reduced gradient to bf16 "
                          "and torch updates bf16 parameters in bf16; the fused engine sums in fp32 (another "
-                         "order) and rounds the fp32 master once — measured 0.008-0.009 at 2 and 8 GPUs"
+                         "order) and rounds the fp32 master once"
                          if wl.dtype_name == "bf16" else "fp32 rounding (~1e-6)"),
             "what": "fused NVLink allreduce+update vs NCCL all_reduce + torch optimizer on identical "
                     "local gradients; per-tensor max|a-b| / max|b|, worst tensor"}
@@ -360,7 +377,7 @@ def main():
     wl = Workload(args, dev, rank)
 
     main_res = run_arm(args.impl, wl, hvd, world, rank, args.steps, args.warmup, args.graph,
-                       want_e2e=not args.no_e2e, want_clocks=True)
+                       want_e2e=not args.no_e2e, want_clocks=True, dump_dir=args.dump_outputs)
     main_res.pop("model")
     opt = main_res.pop("opt")
     if hasattr(opt, "remove_hooks"):
@@ -418,11 +435,11 @@ def main():
                        "cuda_graph": main_res["graphed"],
                        "l2": ("launch/latency-bound config: working set (2 MB) lives in L2 by design"
                               if wl.is_lstm else
-                              "no explicit flush: per-step working set (activations, several GB) >> 126 MB L2"),
+                              "no explicit flush: per-step working set (activations, several GB) >> 50 MB L2"),
                        "comm": main_res["comm"]},
             "clocks": main_res["clocks"], "e2e": e2e,
             "gpu_launches": main_res["launches"],
-            "gpu_launches_note": "hand-written sm_100a kernels of this repo inside the timed region "
+            "gpu_launches_note": "hand-written sm_90a kernels of this repo inside the timed region "
                                  "(ATen glue such as loss / pooling kernels is not counted)",
             "selfcheck": check,
             "final_loss": round(main_res["final_loss"], 6),

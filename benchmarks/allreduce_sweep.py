@@ -1,17 +1,17 @@
 #!/usr/bin/env python
 """Gradient all-reduce bandwidth sweep, 1 KB – 1 GB ([DRIVER] BASELINE.json config 5):
-the framework's sm_100a kernels (one-shot / two-shot / NVLS, and the auto choice) against
+the framework's sm_90a kernels (one-shot / two-shot / NVLS, and the auto choice) against
 ``torch.distributed`` NCCL on the same buffers.
 
     python -m torch.distributed.run --nproc-per-node 8 --master-addr 127.0.0.1 --master-port 29533 \
-        benchmarks/allreduce_sweep.py --out gpurun_out/allreduce_sweep_8.json
+        benchmarks/allreduce_sweep.py --out allreduce_sweep_8.json
 
 Every number is device-timed (CUDA events around ``iters`` back-to-back collectives on the
 launching stream, barrier + synchronize on both sides) and is the MAX over ranks.
-bus GB/s = 2 (N-1)/N * bytes / t   (NCCL-tests convention); roofline = NVLink 5 per-direction
-bandwidth (900 GB/s nominal, 770 GB/s measured peer copy — profiling recipe).
+bus GB/s = 2 (N-1)/N * bytes / t   (NCCL-tests convention); roofline = NVLink per-direction
+bandwidth (H100 SXM, NVLink 4: 450 GB/s nominal).
 Buffers live in symmetric memory (zero-copy, in place), like NCCL's in-place all-reduce.
-Small sizes are L2-resident by nature (latency regime); sizes >= 256 MB exceed the 126 MB L2.
+Small sizes are L2-resident by nature (latency regime); sizes >= 256 MB exceed the 50 MB L2.
 """
 import argparse
 import json
@@ -106,8 +106,7 @@ def main():
         os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
         with open(args.out, "w") as f:
             json.dump({"world": world, "dtype": args.dtype, "multicast": bool(symm.multicast),
-                       "roofline_GBs": {"nvlink_nominal_per_dir": 900, "peer_copy_measured": 770,
-                                        "nccl_8rank_1GiB_measured": 725},
+                       "roofline_GBs": {"nvlink_nominal_per_dir_h100_sxm_datasheet": 450},
                        "rows": rows}, f, indent=1)
     if rank == 0 and args.write_tuning:
         from distributed_torch_horovod_gcp_b200.runtime import tuning

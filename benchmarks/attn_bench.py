@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""tcgen05 flash attention (csrc/attn_sm100.cu) vs F.scaled_dot_product_attention on the ViT-B/16 shape
+"""wgmma flash attention (csrc/attn_sm90.cu) vs F.scaled_dot_product_attention on the ViT-B/16 shape
 (batch 128, 12 heads, 197 tokens, d 64) and a long-sequence shape; forward and forward+backward.
 CUDA events, 3 warm-ups, L2 flush before each timed call, median of --iters."""
 import argparse, json, os, sys
@@ -26,7 +26,7 @@ def timeit(fn, iters, flush):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=10)
-    ap.add_argument("--out", default="gpurun_out/attn_bench.json")
+    ap.add_argument("--out", default=None, help="also write the rows to this JSON file")
     args = ap.parse_args()
     from distributed_torch_horovod_gcp_b200.ops import kernels
     assert kernels.has("attention_fused")
@@ -52,8 +52,9 @@ def main():
                            "ours_tflops": round(3.5 * flops_f / t_ob / 1e6, 1), "speedup": round(t_lb / t_ob, 2)}}
         rows.append(row)
         print(json.dumps(row), flush=True)
-    os.makedirs(os.path.dirname(args.out) or ".", exist_ok=True)
-    json.dump(rows, open(args.out, "w"), indent=1)
+    if args.out:
+        os.makedirs(os.path.dirname(args.out) or ".", exist_ok=True)
+        json.dump(rows, open(args.out, "w"), indent=1)
 
 
 if __name__ == "__main__":

@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""Per-layer timing of the implicit-GEMM convolution (csrc/conv_sm100.cu) against cuDNN on the
+"""Per-layer timing of the implicit-GEMM convolution (csrc/conv_sm90.cu) against cuDNN on the
 ResNet-50 shapes at batch 256 (the headline config): forward, dgrad, wgrad.
 
-    python benchmarks/conv_bench.py [--batch 256] [--iters 10] [--out gpurun_out/conv_bench.json]
+    python benchmarks/conv_bench.py [--batch 256] [--iters 10] [--out conv_bench.json]
 
 Timing: CUDA events on the launching stream, 3 warm-up calls, an L2 flush (256 MiB memset) before
 every timed call.  TFLOP/s = 2*N*OH*OW*Cout*Cin*R*S / t; fraction is against
@@ -53,13 +53,13 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, default=256)
     ap.add_argument("--iters", type=int, default=10)
-    ap.add_argument("--out", default="gpurun_out/conv_bench.json")
+    ap.add_argument("--out", default=None, help="also write the rows to this JSON file")
     ap.add_argument("--only", type=int, default=-1, help="run a single shape index")
     ap.add_argument("--ours-only", action="store_true", help="skip the cuDNN arm (for ncu captures)")
     args = ap.parse_args()
     from distributed_torch_horovod_gcp_b200.ops import kernels, conv as C
     assert kernels.has("conv_implicit_gemm")
-    peak = 1683.7
+    peak = 989.0      # H100 SXM data sheet, dense bf16 (not measured); MEASURED_PEAKS.json overrides
     try:
         peak = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))),
                                            "MEASURED_PEAKS.json")))["bf16_tflops"]
@@ -109,8 +109,9 @@ def main():
     tot_c = sum(r[k]["cudnn_us"] for r in rows for k in ("fprop", "dgrad", "wgrad"))
     summary = {"total_ours_us": round(tot_o, 1), "total_cudnn_us": round(tot_c, 1), "peak_tflops": peak}
     print(json.dumps(summary), flush=True)
-    os.makedirs(os.path.dirname(args.out) or ".", exist_ok=True)
-    json.dump({"rows": rows, "summary": summary}, open(args.out, "w"), indent=1)
+    if args.out:
+        os.makedirs(os.path.dirname(args.out) or ".", exist_ok=True)
+        json.dump({"rows": rows, "summary": summary}, open(args.out, "w"), indent=1)
 
 
 if __name__ == "__main__":

@@ -1,7 +1,7 @@
 """Process-wide runtime state: rank/size/topology, control-plane process group, backends.
 
 Replaces Horovod's C++ global state + controller (SURVEY.md §2.2 N1/N2; reached from
-reference app/torch_train.py:210,217,227,232).  Design differences, B200-first:
+reference app/torch_train.py:210,217,227,232).  Design differences, H100-first:
 
 * No background polling thread and no per-tensor negotiation: the data-parallel bucket
   plan is static and identical on all ranks, so ordering is by bucket index and
@@ -9,7 +9,7 @@ reference app/torch_train.py:210,217,227,232).  Design differences, B200-first:
 * The control plane (rendezvous, handle exchange, plan-hash check) is a Gloo CPU group
   from ``torch.distributed``; it is used at init / setup time only.
 * The data plane for CUDA tensors is the symmetric-memory runtime in
-  ``runtime/`` (cuMem VMM peer mappings + NVLS multicast) driven by the sm_100a
+  ``runtime/`` (cuMem VMM peer mappings + NVLS multicast) driven by the sm_90a
   kernels in ``csrc/comm_kernels.cu``.  NCCL is only a loud fallback.
 """
 from __future__ import annotations

@@ -2,9 +2,9 @@
 
     python -m distributed_torch_horovod_gcp_b200.build [--force] [--verbose]
 
-Produces ``distributed_torch_horovod_gcp_b200/lib/*.so`` for sm_100a:
+Produces ``distributed_torch_horovod_gcp_b200/lib/*.so`` for sm_90a (H100):
   libb200dp_comm.so     csrc/runtime.cpp + csrc/comm_kernels.cu
-  libb200dp_kernels.so  csrc/gemm_sm100.cu, conv_sm100.cu, elementwise.cu, lstm_kernels.cu, lstm_rec_sm100.cu ...
+  libb200dp_kernels.so  csrc/gemm_sm90.cu, conv_sm90.cu, elementwise.cu, lstm_kernels.cu, lstm_rec_sm90.cu ...
 nvcc cross-compiles without a GPU, so this also runs on the CPU dev box.
 """
 from __future__ import annotations
@@ -21,15 +21,15 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "lib")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-Wall", "-Xcompiler", "-Wno-unused-function",
     "--expt-relaxed-constexpr",
 ]
 
 TARGETS = {
     "libb200dp_comm.so": ["runtime.cpp", "comm_kernels.cu"],
-    "libb200dp_kernels.so": ["gemm_sm100.cu", "conv_sm100.cu", "elementwise.cu", "lstm_kernels.cu",
-                             "lstm_rec_sm100.cu", "attn_sm100.cu"],
+    "libb200dp_kernels.so": ["gemm_sm90.cu", "conv_sm90.cu", "elementwise.cu", "lstm_kernels.cu",
+                             "lstm_rec_sm90.cu", "attn_sm90.cu"],
 }
 
 

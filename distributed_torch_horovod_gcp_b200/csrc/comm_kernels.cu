@@ -1,4 +1,4 @@
-// sm_100a communication kernels over NVLink 5 / NVSwitch peer memory.
+// sm_90a communication kernels over NVLink / NVSwitch peer memory.
 //
 // K1 one-shot allreduce  : every rank loads the same 16-byte chunk from all peers (P2P ld over
 //                          NVLink), sums in fp32 in fixed rank order (bit-identical on all

@@ -1,4 +1,4 @@
-// Fused NHWC bf16 batch-norm kernels for sm_100a (memory-bound; 128-bit vector access).
+// Fused NHWC bf16 batch-norm kernels for sm_90a (memory-bound; 128-bit vector access).
 //
 // A channels-last activation is a row-major [M = N*H*W, C] matrix, so per-channel statistics are
 // column reductions and normalisation is a per-column affine.  Fusions (vs the eager
@@ -45,12 +45,23 @@ __device__ __forceinline__ uint4 ldg_stream(const uint4* p) {
 // Column reduction scaffold: the flattened vector index i (8 channels per vector) maps to channel
 // group i % V.  The total thread count is a multiple of V, so a thread always owns ONE channel
 // group and accumulates NACC x 8 partial sums in registers; threads of a block that share a group
-// are combined through shared memory and the block issues one atomicAdd per (channel, quantity).
+// are combined through shared memory and the block writes its partial sums to its own slot.  The
+// last block to finish adds the slots of all blocks in block order to `outs`: the result does not
+// depend on which block finished when, so a training step computes the same bits every run
+// (fp32 atomics would sum in arrival order).
+constexpr int RED_MAX_BLOCKS = 256;
+constexpr int RED_MAX_COLS = 2 * 2048;                  // NACC x channels
+__device__ float g_red_slots[RED_MAX_BLOCKS * RED_MAX_COLS];
+__device__ unsigned int g_red_done;
+
 template <int NACC, int NT>
 __device__ __forceinline__ void block_reduce_to_global(float (&acc)[NACC][8], int V, float* const* outs) {
   __shared__ float sm[NT][8 + 1];
+  __shared__ bool last;
   const int tid = threadIdx.x;
   const int groups = NT / V;      // threads per channel group inside this block (>=1)
+  const int C = V * 8;
+  float* slot = g_red_slots + (size_t)blockIdx.x * (NACC * C);
 #pragma unroll
   for (int q = 0; q < NACC; ++q) {
     __syncthreads();
@@ -58,21 +69,33 @@ __device__ __forceinline__ void block_reduce_to_global(float (&acc)[NACC][8], in
     for (int j = 0; j < 8; ++j) sm[tid][j] = acc[q][j];
     __syncthreads();
     // V*8 channel sums, each over `groups` partials: spread over all threads (8 per group)
-    for (int item = tid; item < V * 8; item += NT) {
+    for (int item = tid; item < C; item += NT) {
       const int g0 = item >> 3, j = item & 7;
       float s = 0.f;
       for (int g = 0; g < groups; ++g) s += sm[g0 + g * V][j];
-      atomicAdd(outs[q] + g0 * 8 + j, s);
+      slot[q * C + item] = s;
     }
   }
+  __threadfence();
+  __syncthreads();
+  if (tid == 0) last = atomicAdd(&g_red_done, 1u) == gridDim.x - 1;
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  for (int item = tid; item < NACC * C; item += NT) {
+    float s = 0.f;
+    for (unsigned b = 0; b < gridDim.x; ++b) s += __ldcg(g_red_slots + (size_t)b * (NACC * C) + item);
+    outs[item / C][item % C] += s;
+  }
+  if (tid == 0) g_red_done = 0u;
 }
 
 // Reduction kernels run ONE 1024-thread block per SM: same-address fp32 atomics serialise in L2
 // (~40 ns each), so the number of blocks — not the data size — set the tail of the first version
-// (888 blocks -> ~45 us per launch; 148 blocks -> ~7 us).
+// (one block per SM instead of several per SM shortens that tail several-fold).
 constexpr int RTHREADS = 1024;
 
-// B200 needs >= ~64 KB in flight per SM to saturate HBM3e (6.5 TB/s x ~1 us): every kernel below
+// HBM3 needs >= ~32 KB in flight per SM to saturate (3.35 TB/s x ~1 us over 132 SMs): every kernel below
 // issues UNROLL independent 128-bit loads per thread per input before consuming any of them.
 __device__ __forceinline__ uint4 ld_or_zero(const uint4* p, long long i, long long n) {
   return i < n ? ldg_stream(p + i) : make_uint4(0, 0, 0, 0);
@@ -586,7 +609,7 @@ __global__ void __launch_bounds__(THREADS) maxpool_bwd_patch_kernel(const uint4*
 }
 
 // ---- stem im2col: 7x7 / stride 2 / pad 3 over NHWC bf16 with C = 3 ------------------------------------
-// Turns the ResNet stem into a plain GEMM for the tcgen05 kernel: A[m][k], m = (n, oh, ow),
+// Turns the ResNet stem into a plain GEMM for the wgmma kernel: A[m][k], m = (n, oh, ow),
 // k = kh*24 + j, j = kw*3 + c for j < 21 and three more elements (the next pixel) for j = 21..23 that
 // the packed weights multiply by zero — row pitch KP = 7*24 = 168.  With that K order every (pixel, kh)
 // segment is a straight 48-byte copy of the (zero-padded) input row starting at byte 12*ow, i.e. 4-byte
@@ -732,7 +755,8 @@ int reduce_grid() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (g_sms <= 0) g_sms = 148;
+    if (g_sms <= 0) g_sms = 132;
+    if (g_sms > RED_MAX_BLOCKS) g_sms = RED_MAX_BLOCKS;   // one reduction slot per block
   }
   return g_sms;
 }
@@ -793,7 +817,7 @@ int b200dp_cast_acc_zero(void* src, void* dst, long long n, int out_bf16, int ac
   }
   const long long n4 = n / 4;
   int grid = (int)((n4 + 255) / 256);
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > reduce_grid() * 8) grid = reduce_grid() * 8;
   if (grid < 1) grid = 1;
   cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
   if (out_bf16) cast_acc_zero_kernel<true><<<grid, 256, 0, st>>>((float*)src, dst, n4, accumulate, zero_src);
@@ -945,7 +969,7 @@ int b200dp_maxpool_fwd(const void* x, void* y, void* idx, int N, int H, int W, i
   const int OH = (H + 2 - 3) / 2 + 1, OW = (W + 2 - 3) / 2 + 1, V = C / 8;
   const long long total = (long long)N * OH * OW * V;
   int grid = (int)((total + THREADS - 1) / THREADS);
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > reduce_grid() * 16) grid = reduce_grid() * 16;
   maxpool_fwd_kernel<<<grid, THREADS, 0, (cudaStream_t)(uintptr_t)stream>>>((const uint4*)x, (uint4*)y,
                                                                              (uint2*)idx, N, H, W, OH, OW, V);
   cudaError_t e = cudaGetLastError();
@@ -960,7 +984,7 @@ int b200dp_maxpool_bwd(const void* dy, const void* idx, void* dx, int N, int H, 
   if (H % 2 == 0 && W % 2 == 0) {
     const long long patches = (long long)N * (H / 2) * (W / 2) * V;
     int pgrid = (int)((patches + THREADS - 1) / THREADS);
-    if (pgrid > 148 * 16) pgrid = 148 * 16;
+    if (pgrid > reduce_grid() * 16) pgrid = reduce_grid() * 16;
     maxpool_bwd_patch_kernel<<<pgrid, THREADS, 0, (cudaStream_t)(uintptr_t)stream>>>(
         (const uint4*)dy, (const uint2*)idx, (uint4*)dx, N, H, W, OH, OW, V);
     cudaError_t pe = cudaGetLastError();
@@ -969,7 +993,7 @@ int b200dp_maxpool_bwd(const void* dy, const void* idx, void* dx, int N, int H, 
   }
   const long long total = (long long)N * H * W * V;
   int grid = (int)((total + THREADS - 1) / THREADS);
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > reduce_grid() * 16) grid = reduce_grid() * 16;
   maxpool_bwd_kernel<<<grid, THREADS, 0, (cudaStream_t)(uintptr_t)stream>>>((const uint4*)dy, (const uint2*)idx,
                                                                              (uint4*)dx, N, H, W, OH, OW, V);
   cudaError_t e = cudaGetLastError();

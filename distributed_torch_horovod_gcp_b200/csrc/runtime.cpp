@@ -4,11 +4,11 @@
 // Symmetric-memory runtime for one NVSwitch domain (<= 8 GPUs, one process per GPU).
 //
 // Replaces the Horovod C++ core pieces that own communication memory (fusion buffer
-// manager, NCCL communicator bootstrap; SURVEY.md §2.2 N1/N2/N5).  B200-first: memory that
+// manager, NCCL communicator bootstrap; SURVEY.md §2.2 N1/N2/N5).  H100-first: memory that
 // peers touch is allocated with the CUDA VMM API (cuMemCreate) as POSIX-fd shareable
 // handles, the fds are passed between the ranks' processes with SCM_RIGHTS over abstract
 // unix sockets, every rank maps every peer's allocation into its own VA space (P2P over
-// NVLink 5) and, when the fabric supports it, all ranks bind the same physical pages to one
+// NVLink) and, when the fabric supports it, all ranks bind the same physical pages to one
 // multicast object (NVLS: multimem.ld_reduce / multimem.st execute in the NVSwitch).
 //
 // Pure C ABI, called from Python through ctypes (runtime/symm.py).  No torch headers.

@@ -5,7 +5,7 @@ data of the benchmark's shape").
 device on a copy stream (double-buffered), so an end-to-end step really contains the H2D
 copy of that step's inputs — the e2e number in bench.py counts these bytes.
 
-``DeviceBatchLoader`` is the B200-first replacement for the reference's
+``DeviceBatchLoader`` is the H100-first replacement for the reference's
 DataLoader+DistributedSampler on tiny tensors (app/torch_train.py:248-251): the whole
 (small) training set lives on the device, the sharded permutation is computed once per
 epoch, and batches are gathered on-device — no worker processes, no per-batch H2D.

@@ -133,7 +133,7 @@ def _free_port() -> int:
 
 def make_parser() -> argparse.ArgumentParser:
     p = argparse.ArgumentParser(
-        prog="horovodrun", description="B200 data-parallel launcher (horovodrun-compatible CLI)")
+        prog="horovodrun", description="H100 data-parallel launcher (horovodrun-compatible CLI)")
     p.add_argument("-v", "--version", action="store_true")
     p.add_argument("-np", "--num-proc", dest="np", type=int)
     p.add_argument("-cb", "--check-build", action="store_true")
@@ -198,7 +198,7 @@ def _env_for(slot: Slot, master_addr: str, master_port: int, args) -> Dict[str, 
         e["HOROVOD_TIMELINE"] = args.timeline_filename
     if args.timeline_mark_cycles:
         e["HOROVOD_TIMELINE_MARK_CYCLES"] = "1"
-    # Horovod's stall inspector == the bounded spin-wait of the sm_100a kernels (runtime/symm.py reads these)
+    # Horovod's stall inspector == the bounded spin-wait of the sm_90a kernels (runtime/symm.py reads these)
     if args.no_stall_check:
         e["HOROVOD_STALL_CHECK_DISABLE"] = "1"
     if args.stall_check_warning_time_seconds is not None:
@@ -237,8 +237,8 @@ def check_build() -> str:
         ("Frameworks", [("PyTorch", True)]),
         ("Controllers", [("MPI", False), ("Gloo", True)]),
         ("Tensor Operations", [
-            ("sm_100a symmetric-memory kernels (P2P / NVLS)", lib.available("libb200dp_comm.so")),
-            ("sm_100a tcgen05 compute kernels", lib.available("libb200dp_kernels.so")),
+            ("sm_90a symmetric-memory kernels (P2P / NVLS)", lib.available("libb200dp_comm.so")),
+            ("sm_90a wgmma compute kernels", lib.available("libb200dp_kernels.so")),
             ("NCCL (fallback only)", bool(torch.distributed.is_nccl_available())),
             ("Gloo (CPU tensors)", True), ("MPI", False)]),
     ]

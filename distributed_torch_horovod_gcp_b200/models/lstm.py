@@ -8,12 +8,12 @@ every forward (app/torch_train.py:179-193); the last timestep is selected
 the reference's (``lstm.weight_ih_l0`` … ``linear3.bias``) so ``broadcast_parameters``
 moves the same 10 tensors / 1 480 196 bytes.
 
-B200-first changes (SURVEY.md §2.6 S2/S4, §7.3):
+H100-first changes (SURVEY.md §2.6 S2/S4, §7.3):
   * ``(h0, c0)`` come from the device generator (no CPU randn + pageable H2D + sync per
     step), the last-step gather is a slice (no host-built index tensor);
   * on CUDA (fp32, hidden size 256, one unidirectional layer — the reference configuration)
     forward/backward run on the persistent cluster LSTM kernels (K5: ``ops/lstm_rec.py``,
-    csrc/lstm_rec_sm100.cu — tf32 tcgen05, W_hh resident in shared memory, h exchanged through
+    csrc/lstm_rec_sm90.cu — tf32 wgmma, W_hh resident in shared memory, h exchanged through
     DSMEM) and the chained-GEMM head (K6: ``ops/lstm_fused.py``); other shapes (bidirectional,
     multi-layer, other hidden sizes) use cuDNN / cuBLAS, which is also the numerics oracle.
 """

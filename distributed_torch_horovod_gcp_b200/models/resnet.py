@@ -6,8 +6,8 @@ reference, whose only model is the LSTM — SURVEY.md §0 item 6).
 parameters **and** BN buffers (SURVEY.md §7.3).  ResNet-50 here has 25 557 032 parameters
 in 161 tensors, matching the survey's count.
 
-B200-first layout: activations are NHWC (``channels_last``) bf16, so every 1x1 convolution
-is a plain ``[N*H*W, Cin] x [Cin, Cout]`` GEMM for the tcgen05 kernel and BN/ReLU/residual
+H100-first layout: activations are NHWC (``channels_last``) bf16, so every 1x1 convolution
+is a plain ``[N*H*W, Cin] x [Cin, Cout]`` GEMM for the wgmma kernel and BN/ReLU/residual
 are fused row-wise epilogues/prologues (``ops.functional.conv_bn_act``).  Each
 conv+BN(+ReLU)(+residual) is ONE functional call so the fused kernels can replace it as a
 unit; the PyTorch composition is the fallback and the numerics oracle.

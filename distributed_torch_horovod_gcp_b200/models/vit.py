@@ -2,7 +2,7 @@
 the reference — SURVEY.md §0 item 6).  86 567 656 parameters in 152 tensors at 224x224 /
 1000 classes, matching the survey's count.
 
-Every matmul goes through ``ops.functional.linear`` (tcgen05 GEMM with fused bias / GELU /
+Every matmul goes through ``ops.functional.linear`` (wgmma GEMM with fused bias / GELU /
 residual epilogues when the in-tree kernels are built) and attention through
 ``ops.functional.attention``; the patch embedding is a stride-16 16x16 convolution, i.e. a
 pure ``[N*196, 768] x [768, 768]`` GEMM after an NHWC patch gather.

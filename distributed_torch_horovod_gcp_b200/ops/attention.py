@@ -1,4 +1,4 @@
-"""Flash attention binding (csrc/attn_sm100.cu): tcgen05 forward + backward, bf16, head dim 64,
+"""Flash attention binding (csrc/attn_sm90.cu): wgmma forward + backward, bf16, head dim 64,
 non-causal (the ViT-B/16 configuration).  ``attention_fused(q, k, v)`` takes ``[B, H, S, 64]``
 tensors with ANY batch/head/sequence strides (64 contiguous) — in the model they are the three dense
 ``[B*S, D]`` projection outputs viewed as ``[B, S, H, 64]`` and transposed, so no un-pack / re-pack

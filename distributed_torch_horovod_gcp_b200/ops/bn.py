@@ -1,8 +1,12 @@
 """Fused NHWC BatchNorm(+residual)(+ReLU) (csrc/elementwise.cu) and the conv+BN+act unit used by
-the ResNet blocks.  1x1 stride-1 convolutions run on the tcgen05 GEMM (an NHWC activation is a
+the ResNet blocks.  1x1 stride-1 convolutions run on the wgmma GEMM (an NHWC activation is a
 row-major [N*H*W, C] matrix), the 7x7 stem on im2col + that GEMM, and 3x3 / strided 1x1 convolutions
-on the implicit-GEMM kernel (ops/conv.py, csrc/conv_sm100.cu); cuDNN is only the fallback for shapes
-none of these cover (e.g. a 3-channel 3x3 stem)."""
+on the implicit-GEMM kernel (ops/conv.py, csrc/conv_sm90.cu); cuDNN is only the fallback for shapes
+none of these cover (e.g. a 3-channel 3x3 stem).
+
+The batch-statistics reductions (here and in the producing GEMM / convolution epilogue) sum per-CTA
+partials in a fixed order through one per-library set of slots, so they are bit-reproducible but must
+not run concurrently on different CUDA streams; the training step issues them on one stream."""
 from __future__ import annotations
 
 import ctypes
@@ -199,10 +203,10 @@ STEM_KP = 168          # k = kh*24 + kw*3 + c (21 real + 3 zero-weighted columns
 
 
 class _StemConvFn(torch.autograd.Function):
-    """ResNet stem (7x7, stride 2, pad 3, 3 input channels) as im2col + tcgen05 GEMM.  cuDNN runs
-    this layer on legacy sm80 kernels (1.5 ms fwd + 0.8 ms wgrad at batch 256); the im2col matrix
-    ([N*112*112, 168] bf16) is kept for the weight gradient — HBM capacity is not the constraint
-    on a 180 GB part, bandwidth is."""
+    """ResNet stem (7x7, stride 2, pad 3, 3 input channels) as im2col + wgmma GEMM.  The im2col
+    matrix ([N*112*112, 168] bf16, about 1 GB at batch 256) is kept for the weight gradient instead
+    of being rebuilt: it fits easily in an 80 GB H100, and HBM bandwidth, not capacity, bounds
+    the step."""
 
     @staticmethod
     def forward(ctx, x, weight, stats=None):
@@ -250,7 +254,7 @@ _FUSE_STATS = os.environ.get("B200DP_BN_STATS_IN_EPILOGUE", "1") == "1"
 
 
 def conv2d(x, conv: torch.nn.Conv2d, box=None, stats=None, park=None):
-    """Convolution of an NHWC bf16 activation; 1x1/stride-1 and the 7x7 stem -> tcgen05 GEMM, 3x3 and
+    """Convolution of an NHWC bf16 activation; 1x1/stride-1 and the 7x7 stem -> wgmma GEMM, 3x3 and
     strided 1x1 -> implicit-GEMM kernel.  Returns ``(y, stats_filled)``: when ``stats`` (fp32 [2*Cout]
     accumulator) is given and the kernel that ran supports it, its epilogue has added the output's
     per-channel sum / sum of squares."""

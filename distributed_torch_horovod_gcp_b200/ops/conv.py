@@ -1,6 +1,6 @@
-"""Implicit-GEMM convolution binding (csrc/conv_sm100.cu): 3x3 (stride 1/2, pad 1) and 1x1
+"""Implicit-GEMM convolution binding (csrc/conv_sm90.cu): 3x3 (stride 1/2, pad 1) and 1x1
 (stride 1/2) NHWC bf16 convolutions — forward, data gradient and weight gradient — on the
-tcgen05 mainloop, with the filter taps expressed as shifted 4D TMA boxes (zero padding = TMA
+wgmma mainloop, with the filter taps expressed as shifted 4D TMA boxes (zero padding = TMA
 out-of-bounds fill).  No cuDNN call and no im2col buffer on this path.
 
 Weights are consumed as ``[Cout][R][S][Cin]`` — PyTorch's ``channels_last`` layout of a
@@ -170,7 +170,7 @@ class _ConvFn(torch.autograd.Function):
 
 def conv2d(x: torch.Tensor, weight: torch.Tensor, stride: int = 1, padding: Optional[int] = None, stats=None,
            park=None):
-    """``F.conv2d`` for NHWC bf16 activations on the sm_100a implicit-GEMM kernel.  ``stats`` (fp32
+    """``F.conv2d`` for NHWC bf16 activations on the sm_90a implicit-GEMM kernel.  ``stats`` (fp32
     [2*Cout], zero on entry): the kernel's epilogue adds the per-channel sum / sum of squares of the
     output to it — the batch statistics of the BatchNorm that follows."""
     if padding is None:

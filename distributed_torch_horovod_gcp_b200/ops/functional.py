@@ -2,7 +2,7 @@
 
 Each function is ONE fusable unit.  ``*_reference`` are plain PyTorch compositions — the CPU
 path and the fp32 numerics oracle for the kernels' tests; the CUDA fast paths are the
-hand-written sm_100a kernels bound in ``ops.kernels``: tcgen05 GEMM with fused epilogues
+hand-written sm_90a kernels bound in ``ops.kernels``: wgmma GEMM with fused epilogues
 (ops/gemm.py), implicit-GEMM convolution (ops/conv.py), fused BN/ReLU/residual and max-pool
 (ops/bn.py), LayerNorm (ops/ln.py), flash attention forward/backward (ops/attention.py).
 """
@@ -19,7 +19,7 @@ _FORCE_REFERENCE = os.environ.get("B200DP_REFERENCE_OPS", "0") == "1"
 
 
 def _kernels(x: torch.Tensor):
-    """Return the kernels module when ``x`` can take the sm_100a path, else ``None``."""
+    """Return the kernels module when ``x`` can take the sm_90a path, else ``None``."""
     if _FORCE_REFERENCE or not x.is_cuda:
         return None
     from . import kernels
@@ -146,7 +146,7 @@ def qkv_attention(x, weight, bias, heads: int):
 def patch_embed(x, weight, bias, patch: int):
     """``[B,3,H,W]`` (NCHW logical, any memory format) -> ``[B, (H/p)*(W/p), D]``: gather
     non-overlapping patches to rows and run ONE GEMM against ``weight`` viewed as
-    ``[D, 3*p*p]`` (identical to the stride-p conv, but GEMM-shaped for tcgen05)."""
+    ``[D, 3*p*p]`` (identical to the stride-p conv, but GEMM-shaped for the wgmma GEMM)."""
     B, C, H, W = x.shape
     gh, gw = H // patch, W // patch
     cols = x.reshape(B, C, gh, patch, gw, patch).permute(0, 2, 4, 1, 3, 5) \

@@ -1,10 +1,10 @@
-"""tcgen05 GEMM binding (csrc/gemm_sm100.cu) and the autograd ``linear`` built on it.
+"""wgmma GEMM binding (csrc/gemm_sm90.cu) and the autograd ``linear`` built on it.
 
     y = act(x @ W^T + b) (+ residual)          forward : A = x (K-major),  B = W (K-major)
     dx = dy' @ W                                dgrad   : A = dy' (K-major), B = W (MN-major)
     dW = dy'^T @ x                              wgrad   : A = dy' (MN-major), B = x (MN-major),
                                                           split-K, fp32 atomics
-No transposes are materialised: the kernel takes MN-major operands through its UMMA
+No transposes are materialised: the kernel takes MN-major operands through its GMMA
 descriptors.  ``dy' = dy * act'(z)`` is fused into the dgrad of the *next* layer's epilogue
 where possible; here it is computed by the epilogue modes 3/4 of the kernel when the layer
 has an activation.
@@ -12,7 +12,6 @@ has an activation.
 from __future__ import annotations
 
 import ctypes
-import os
 from typing import Optional
 
 import torch
@@ -31,7 +30,7 @@ def register(lib, have):
     _lib = lib
     vp, i, f = ctypes.c_void_p, ctypes.c_int, ctypes.c_float
     lib.b200dp_gemm_bf16.argtypes = [vp, vp, vp, i, i, i, i, i, i, i, i, vp, vp, vp, vp, i, i, f, i,
-                                     i, i, i, vp, vp, ctypes.c_uint64]
+                                     i, i, vp, vp, ctypes.c_uint64]
     lib.b200dp_gemm_bf16.restype = i
     lib.b200dp_gemm_last_error.restype = ctypes.c_char_p
     if hasattr(lib, "b200dp_cast_acc_zero"):
@@ -46,10 +45,14 @@ def gemm(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor, M: int, N: int, K:
          a_mn: bool = False, b_mn: bool = False, bias: Optional[torch.Tensor] = None,
          residual: Optional[torch.Tensor] = None, preact: Optional[torch.Tensor] = None,
          act: int = 0, out_mode: int = 0, alpha: float = 1.0, splits: int = 1, block_n: int = 0,
-         max_ctas: int = 0, two_cta: Optional[bool] = None, stats: Optional[torch.Tensor] = None,
+         max_ctas: int = 0, stats: Optional[torch.Tensor] = None,
          res_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Raw kernel call.  ``a``: [M,K] (K-major) or [K,M] (MN-major) bf16 with contiguous rows;
-    ``b``: [N,K] or [K,N]; ``out``: [M,N] bf16 (out_mode 0) or fp32 (1: atomic add, 2: store)."""
+    ``b``: [N,K] or [K,N]; ``out``: [M,N] bf16 (out_mode 0) or fp32 (1: add, 2: store).
+    Split-K (out_mode 1, splits > 1) sums in split order through a workspace allocated per launch on the
+    current stream, so it may run on any stream.  ``stats`` accumulates through one per-library set of
+    per-CTA slots: calls with ``stats`` (and the BatchNorm reductions of ``ops.bn``) must not run
+    concurrently on different streams."""
     assert _lib is not None, "libb200dp_kernels.so not loaded"
     assert a.dtype == torch.bfloat16 and b.dtype == torch.bfloat16
     assert a.stride(-1) == 1 and b.stride(-1) == 1 and out.stride(-1) == 1
@@ -60,29 +63,14 @@ def gemm(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor, M: int, N: int, K:
         int(a_mn), int(b_mn), bias_bf, bias_f32,
         residual.data_ptr() if residual is not None else None,
         preact.data_ptr() if preact is not None else None,
-        act, out_mode, float(alpha), splits, block_n, max_ctas, int(_want_2cta(M, N, K, two_cta)),
+        act, out_mode, float(alpha), splits, block_n, max_ctas,
         stats.data_ptr() if stats is not None else None,
         res_mask.data_ptr() if res_mask is not None else None,
         torch.cuda.current_stream(a.device).cuda_stream)
     if rc != 0:
         raise RuntimeError("b200dp_gemm_bf16: " + (_lib.b200dp_gemm_last_error() or b"").decode())
-    counters.bump("gemm_sm100")
+    counters.bump("gemm_sm90")
     return out
-
-
-_TWO_CTA = os.environ.get("B200DP_GEMM_2CTA", "1")
-
-
-def _want_2cta(M: int, N: int, K: int, override: Optional[bool]) -> bool:
-    """cta_group::2 (256x256 tile per CTA pair) pays when the GEMM is operand-bandwidth bound:
-    wide N (the kernel instantiates BN=256 only) and enough rows/depth for the pair to amortise."""
-    if override is not None:
-        return bool(override)
-    if _TWO_CTA == "0":
-        return False
-    if _TWO_CTA == "force":
-        return N > 128
-    return N > 128 and M >= 512 and K >= 256
 
 
 def supported(x: torch.Tensor, weight: torch.Tensor) -> bool:
@@ -92,7 +80,7 @@ def supported(x: torch.Tensor, weight: torch.Tensor) -> bool:
     return N % 8 == 0 and K % 8 == 0 and x.shape[-1] == K and x.numel() // K >= 1
 
 
-def _splits_for(M_out: int, N_out: int, K_red: int, sms: int = 148) -> int:
+def _splits_for(M_out: int, N_out: int, K_red: int, sms: int = 132) -> int:
     tiles = ((M_out + 127) // 128) * ((N_out + 127) // 128)
     if tiles >= (2 * sms) // 3:
         return 1                       # enough tiles to fill the GPU: no split, direct bf16 store
@@ -168,7 +156,7 @@ def bias_grad(dz: torch.Tensor, N: int, M: int, dtype) -> torch.Tensor:
     acc = torch.zeros((N, 8), dtype=torch.float32, device=dz.device)
     kb = (M + 63) // 64
     gemm(dz, _ones(M, dz.device), acc, N, 8, M, a_mn=True, b_mn=True, out_mode=1,
-         splits=max(1, min(kb // 4, (2 * 148) // max((N + 127) // 128, 1))), block_n=64)
+         splits=max(1, min(kb // 4, (2 * 132) // max((N + 127) // 128, 1))), block_n=64)
     return acc[:, 0].to(dtype)
 
 
@@ -312,8 +300,8 @@ def mlp(x, w1, b1, w2, b2, residual=None):
 class _QKVFn(torch.autograd.Function):
     """Attention input projection producing q, k, v as three DENSE [M, D] matrices (three GEMMs on
     row-slices of the packed [3D, D] weight).  A packed [M, 3D] output forces PyTorch to un-pack
-    with strided views forward and to re-pack dq/dk/dv with a cat + copies backward — 5.5 ms of
-    a 31 ms ViT-B step (profiles/run_1gpu_vit_2cta_epilogue.log).  Here the backward consumes
+    with strided views forward and to re-pack dq/dk/dv with a cat + copies backward.  Here the
+    backward consumes
     dq, dk, dv where they are: dx is accumulated through the GEMM's residual input and the weight
     gradient is written slice by slice."""
 

@@ -2,8 +2,7 @@
 
 With the fused engine every ``param.grad`` is a view into a flat gradient bucket in symmetric
 memory.  Autograd's ``AccumulateGrad`` then costs one ``add`` kernel (and often one layout
-``copy``) per parameter per step — 160 + 142 launches for ResNet-50 (profiles/
-launches_resnet50_ours.csv).  A weight-gradient kernel that knows where the bucket slot is can
+``copy``) per parameter per step — about 300 launches for ResNet-50.  A weight-gradient kernel that knows where the bucket slot is can
 write there itself; this module is the handshake:
 
   forward  : ``note_forward(weight)``      (counts uses: shared weights keep the autograd path)

@@ -1,4 +1,4 @@
-"""Python bindings (ctypes) for the in-tree sm_100a compute kernels
+"""Python bindings (ctypes) for the in-tree sm_90a compute kernels
 (``csrc/*.cu`` -> ``lib/libb200dp_kernels.so``).  Loaded lazily; every op registers itself
 in ``_HAVE`` once its symbol resolves, so the functional layer can route per-op.
 """
@@ -32,7 +32,7 @@ def enabled_for(x: torch.Tensor) -> bool:
         return False
     if _load() is None:
         return False
-    return torch.cuda.get_device_capability(x.device)[0] == 10
+    return torch.cuda.get_device_capability(x.device)[0] == 9
 
 
 def has(op: str) -> bool:

@@ -1,7 +1,7 @@
 """K6 — fused linear head of the reference LSTM model (csrc/lstm_kernels.cu): the last-timestep
 gather (reference index_select, app/torch_train.py:196) + the three activation-free linears
 (app/torch_train.py:199-205) as ONE forward kernel and TWO backward kernels, fp32.  The recurrent
-part is the persistent cluster kernel K5 (ops/lstm_rec.py, csrc/lstm_rec_sm100.cu)."""
+part is the persistent cluster kernel K5 (ops/lstm_rec.py, csrc/lstm_rec_sm90.cu)."""
 from __future__ import annotations
 
 import ctypes

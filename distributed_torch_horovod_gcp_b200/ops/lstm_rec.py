@@ -1,8 +1,8 @@
-"""K5 — persistent LSTM recurrence binding (csrc/lstm_rec_sm100.cu).
+"""K5 — persistent LSTM recurrence binding (csrc/lstm_rec_sm90.cu).
 
 ``lstm_recurrent(x, h0, c0, w_ih, w_hh, b_ih, b_hh) -> (seq, (hT, cT))`` is a drop-in for a
 single-layer unidirectional ``nn.LSTM(batch_first=True)`` call with hidden size 256 (the reference
-model, /root/reference/app/torch_train.py:121-122,195) in fp32: forward = x-projection kernel + ONE
+model, reference app/torch_train.py:121-122,195) in fp32: forward = x-projection kernel + ONE
 cluster kernel for all timesteps, backward = ONE cluster kernel + ONE gradient kernel.  Weight
 gradients go straight into the gradient-bucket slots when the parameters carry a grad sink
 (ops/grad_sink.py).  cuDNN is not involved.

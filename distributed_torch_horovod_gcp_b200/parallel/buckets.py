@@ -7,7 +7,7 @@ list; its hash is cross-checked over the control plane at construction, which re
 Horovod's per-step negotiation check.  Gradients are *views* into the flat bucket, so the
 ``BatchedD2DMemcpy`` pack/unpack kernels of Horovod (N6) do not exist here.
 
-Layout rules (they matter to the sm_100a kernels in csrc/comm_kernels.cu):
+Layout rules (they matter to the sm_90a kernels in csrc/comm_kernels.cu):
   * a bucket never mixes dtypes, devices or optimizer param-groups (one hyper-parameter
     block per bucket);
   * every tensor starts on a 16-byte boundary inside the bucket (vectorised 128-bit

@@ -1,6 +1,6 @@
 """Fused gradient-allreduce + optimizer engine (the north-star hot path).
 
-One bucket == one launch of an sm_100a kernel from csrc/comm_kernels.cu that
+One bucket == one launch of an sm_90a kernel from csrc/comm_kernels.cu that
   (1) reduces the bucket's gradients across all ranks by reading peer memory over NVLink
       (one-shot), or by slice with P2P pushes (two-shot), or in the NVSwitch (NVLS);
   (2) scales by 1/N, (3) runs the SGD-momentum / Adam / AdamW update on fp32 master

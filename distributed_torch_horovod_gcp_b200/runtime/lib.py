@@ -1,8 +1,8 @@
 """Locate / load the in-tree native libraries.
 
   lib/libb200dp_comm.so     C++ runtime (csrc/runtime.cpp: symmetric heap, fd passing) +
-                            sm_100a comm kernels (csrc/comm_kernels.cu: allreduce/broadcast(+optimizer))
-  lib/libb200dp_kernels.so  sm_100a math  (csrc/gemm_sm100.cu …)  — tcgen05 GEMM, BN, LSTM …
+                            sm_90a comm kernels (csrc/comm_kernels.cu: allreduce/broadcast(+optimizer))
+  lib/libb200dp_kernels.so  sm_90a math  (csrc/gemm_sm90.cu …)  — wgmma GEMM, BN, LSTM …
 
 They are built IN-TREE by ``build.py`` (``__graft_entry__.build()``) so they travel with the
 repo snapshot to the GPU box, and loaded with ctypes (no torch headers => seconds to build).

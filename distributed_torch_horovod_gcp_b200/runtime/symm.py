@@ -1,4 +1,4 @@
-"""Python driver of the C++ symmetric-memory runtime (csrc/runtime.cpp) and of the sm_100a
+"""Python driver of the C++ symmetric-memory runtime (csrc/runtime.cpp) and of the sm_90a
 communication kernels (csrc/comm_kernels.cu).
 
 One ``SymmRuntime`` per process (= per GPU).  ``alloc`` is a *collective*: every rank creates
@@ -359,9 +359,8 @@ class SymmRuntime:
             return ALGO_TWOSHOT
         if o in ("nvls", "2") and self.multicast and need_mc:
             return ALGO_NVLS
-        # Measured table (runtime/tuning.py; profiles/allreduce_sweep_*.json): one-shot only wins
-        # in the pure-latency regime; above it the sliced kernels win at every size and the
-        # in-switch reduction (NVLS) beats P2P two-shot from ~64 KB up to 1 GB (838 vs 641 GB/s).
+        # Table (runtime/tuning.py): one-shot only wins in the pure-latency regime; above it the
+        # sliced kernels, and where the switch supports it the in-switch reduction (NVLS).
         from . import tuning
         return tuning.choose(self.world, nbytes, bool(self.multicast and need_mc))
 

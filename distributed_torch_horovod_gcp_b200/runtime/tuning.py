@@ -2,8 +2,8 @@
 (`HOROVOD_AUTOTUNE` / parameter_manager: Bayesian search over fusion threshold and cycle time;
 SURVEY.md §2.2 N11, §5.6).  There is nothing to search at run time here: the bucket plan is
 static and the only choice is WHICH kernel reduces a bucket of a given size on a given world
-size.  The default table below was measured on 8xB200 and 2xB200 (profiles/allreduce_sweep_*.json);
-`benchmarks/allreduce_sweep.py --write-tuning FILE` re-derives it on another machine and
+size.  The default table below is a starting point, not a measurement of any particular machine;
+`benchmarks/allreduce_sweep.py --write-tuning FILE` derives one for the machine it runs on and
 `B200DP_TUNING_FILE=FILE` makes every rank load it.
 
 Table format (JSON): {"<world>": {"oneshot_max_bytes": int, "prefer": "nvls" | "twoshot"}, ...}

@@ -2,7 +2,7 @@
 
 The reference uses exactly eight call sites of ``horovod.torch`` (app/torch_train.py:17,
 210,217,227,232,249,259,266,308; SURVEY.md §2.3 A1–A8).  All of them, plus the rest of the
-commonly used Horovod surface, are provided here on top of the B200 runtime.
+commonly used Horovod surface, are provided here on top of the H100 runtime.
 """
 from __future__ import annotations
 
@@ -55,7 +55,7 @@ def gloo_enabled() -> bool:
 
 
 def nccl_built() -> int:
-    """NCCL is present only as a fallback data plane; the product path is the sm_100a
+    """NCCL is present only as a fallback data plane; the product path is the sm_90a
     symmetric-memory kernels (see ``symm_built``)."""
     try:
         return int(_torch.distributed.is_nccl_available())
@@ -80,7 +80,7 @@ def ccl_built() -> bool:
 
 
 def symm_built() -> bool:
-    """True when the in-tree sm_100a runtime library has been built."""
+    """True when the in-tree sm_90a runtime library has been built."""
     from ..runtime import lib
     return lib.available()
 

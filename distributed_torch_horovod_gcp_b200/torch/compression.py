@@ -1,7 +1,7 @@
 """Gradient compression (wire dtype) — Horovod's ``hvd.Compression`` shape (SURVEY.md §2.3;
 default ``none`` at the reference's call site app/torch_train.py:259).
 
-On B200 the interesting setting is ``bf16``: gradients travel NVLink as bf16 and are
+On H100 the interesting setting is ``bf16``: gradients travel NVLink as bf16 and are
 accumulated in fp32 registers inside the fused allreduce kernel, which halves link bytes.
 """
 from __future__ import annotations

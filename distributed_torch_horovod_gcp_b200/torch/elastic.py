@@ -3,7 +3,7 @@ sync of model + optimizer, and a ``run`` decorator that rolls back to the last c
 a collective fails (``HorovodInternalError``).
 
 The reference enables none of this (SURVEY.md §5.3); it is provided for surface parity and
-as the failure-recovery hook for the kernel watchdog (a bounded spin-wait in the sm_100a
+as the failure-recovery hook for the kernel watchdog (a bounded spin-wait in the sm_90a
 kernels sets an error flag -> ``HorovodInternalError``).
 
 Resizing is restart-based (launch/run.py elastic mode): ``state.check_host_updates()`` lets rank 0

@@ -2,7 +2,7 @@
 ``allgather_object`` (Horovod ``horovod/torch/functions.py`` call shapes).
 
 ``broadcast_parameters`` is the startup collective of the reference
-(app/torch_train.py:266; semantics SURVEY.md §2.3 A7).  B200-first difference: instead of
+(app/torch_train.py:266; semantics SURVEY.md §2.3 A7).  H100-first difference: instead of
 one ``ncclBcast`` per tensor, all CUDA tensors of a dtype are packed into ONE flat
 symmetric buffer and broadcast by ONE multicast-store kernel (K4, csrc/comm_kernels.cu);
 the 10 tensors / 1.48 MB of the reference model therefore cost a single launch.

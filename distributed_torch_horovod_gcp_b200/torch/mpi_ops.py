@@ -6,7 +6,7 @@ N8, N10; used by the reference through app/torch_train.py:259,266).
 
 Data plane selection per tensor:
   * CPU tensor            -> Gloo (``torch.distributed``), the CPU plumbing configuration.
-  * CUDA tensor           -> symmetric-memory sm_100a kernels (one-shot / two-shot / NVLS
+  * CUDA tensor           -> symmetric-memory sm_90a kernels (one-shot / two-shot / NVLS
                              allreduce, multicast broadcast, reduce-scatter, all-gather,
                              equal-split all-to-all) from ``runtime.symm``; ragged all-gather /
                              all-to-all shapes keep the torch.distributed path.
@@ -174,7 +174,7 @@ def _ps_size(process_set) -> int:
 def _check_op(op):
     if op is Adasum or getattr(op, "value", None) == 2:
         raise NotImplementedError(
-            "op=Adasum is not implemented in the B200 runtime (Average/Sum/Min/Max/Product are).")
+            "op=Adasum is not implemented in the H100 runtime (Average/Sum/Min/Max/Product are).")
 
 
 def _timeline(name: str, phase: str, **kw):
@@ -399,7 +399,7 @@ def allgather_async(tensor, name=None, process_set=None) -> int:
     symm = _state.get_symm() if (tensor.is_cuda and process_set is None) else None
     row_bytes = (tensor.numel() // max(tensor.shape[0], 1)) * tensor.element_size() if tensor.shape[0] else 0
     if symm is not None and min(sizes) == mx and mx > 0 and (mx * row_bytes) % 16 == 0:
-        # equal shards: every rank pushes its shard into slot `rank` of all peers over NVLink (sm_100a kernel)
+        # equal shards: every rank pushes its shard into slot `rank` of all peers over NVLink (sm_90a kernel)
         src = tensor.contiguous()
         out = torch.empty((n * mx,) + tuple(tensor.shape[1:]), dtype=tensor.dtype, device=tensor.device)
         ev = symm.allgather(src, out)

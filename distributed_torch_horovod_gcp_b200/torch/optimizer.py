@@ -5,14 +5,14 @@ app/torch_train.py:259 (semantics: SURVEY.md §2.3 A6).  The returned object **i
 instance of the wrapped optimizer's class (dynamic subclass) with the same
 ``param_groups`` / ``state``.
 
-B200-first design (vs Horovod's per-tensor ``allreduce_async_`` + host ``synchronize``):
+H100-first design (vs Horovod's per-tensor ``allreduce_async_`` + host ``synchronize``):
 
 * static bucket plan (``parallel/buckets.py``); ``p.grad`` tensors are views into flat
   buckets, so there is no pack/unpack;
 * ``register_post_accumulate_grad_hook`` decrements a per-bucket counter; the bucket that
   completes is launched immediately on a high-priority **side stream** ordered after the
   backward stream by a CUDA event, overlapping communication with the rest of backward;
-* on CUDA with the symmetric-memory runtime the bucket kernel is ONE sm_100a kernel that
+* on CUDA with the symmetric-memory runtime the bucket kernel is ONE sm_90a kernel that
   reduces across peers over NVLink (one-shot / two-shot / NVLS multicast, picked per
   bucket size), applies ``1/N`` (+ ``gradient_predivide_factor``), casts, and performs
   the SGD-momentum / Adam update in its epilogue (``parallel/fused_engine.py``;
@@ -123,7 +123,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
                     f"DistributedOptimizer: gradient bucket plan differs across ranks "
                     f"(ranks {bad} disagree with rank 0) — models are not identical.")
 
-        # try the fused sm_100a engine first
+        # try the fused sm_90a engine first
         self._engine = None
         want_fused = self._fused_request
         on_cuda = all(b.device.type == "cuda" for b in self._buckets) and len(self._buckets) > 0
@@ -133,7 +133,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
             from ..parallel.fused_engine import FusedEngine
             self._engine = FusedEngine.try_create(self, self._buckets, wire)
             if self._engine is None and self._fused_request:
-                raise RuntimeError("fused=True requested but the fused sm_100a engine is "
+                raise RuntimeError("fused=True requested but the fused sm_90a engine is "
                                    "unavailable: " + str(_state.runtime().symm_failed))
         if self._engine is None:
             self._setup_generic()
@@ -204,7 +204,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
                 g = param.grad
                 if g is not None and g.is_sparse:
                     raise NotImplementedError(
-                        "sparse gradients are not supported by the bucketed B200 path; "
+                        "sparse gradients are not supported by the bucketed H100 path; "
                         "pass sparse_as_dense=True and use dense embeddings")
                 if self._engine is None:
                     self._ensure_view(b, param)
@@ -438,7 +438,7 @@ def DistributedOptimizer(optimizer, named_parameters=None, compression=Compressi
     """Wrap ``optimizer`` so gradients are averaged across ranks before the update.
 
     Arguments follow Horovod (SURVEY.md §2.3 A6); ``bucket_bytes`` and ``fused`` are
-    B200-runtime extensions (``fused=None`` → use the fused sm_100a kernel when the
+    H100-runtime extensions (``fused=None`` → use the fused sm_90a kernel when the
     optimizer is plain SGD(-momentum) / Adam / AdamW on CUDA with the symmetric runtime).
     """
     if op is Adasum:

@@ -2,10 +2,10 @@
 
 Horovod surface parity (SURVEY.md §2.3, "not used by the reference").  Statistics
 (sum, sum of squares, count) are packed into one small vector and all-reduced with the
-framework's own ``allreduce`` (one-shot sm_100a kernel on CUDA: 2C+1 floats is a pure
+framework's own ``allreduce`` (one-shot sm_90a kernel on CUDA: 2C+1 floats is a pure
 latency message), forward and backward.
 
-On B200 with NHWC bf16 activations the whole op runs on the fused BN kernels of
+On H100 with NHWC bf16 activations the whole op runs on the fused BN kernels of
 csrc/elementwise.cu with the NVLink allreduce BETWEEN their passes (``_SyncBNKernelFn``):
 stats kernel -> one-shot allreduce -> finalize+apply kernel forward; masked-reduce kernel ->
 one-shot allreduce -> dx kernel backward.  Other layouts / dtypes / CPU use the PyTorch composition
@@ -75,7 +75,7 @@ class _SyncBNFn(torch.autograd.Function):
 
 
 class _SyncBNKernelFn(torch.autograd.Function):
-    """NHWC bf16 SyncBN on the sm_100a BN kernels + one-shot allreduce of the per-channel sums."""
+    """NHWC bf16 SyncBN on the sm_90a BN kernels + one-shot allreduce of the per-channel sums."""
 
     @staticmethod
     def forward(ctx, x, weight, bias, running_mean, running_var, eps, momentum):

@@ -1,5 +1,5 @@
 """Background sampler of SM clocks / throttle reasons during a timed region (bench.py
-``"clocks"`` key; profiling recipe /opt/skills/guides/B200_PROFILING.md).  Uses NVML in a
+``"clocks"`` key).  Uses NVML in a
 thread; falls back to ``nvidia-smi`` polling; never changes clocks."""
 from __future__ import annotations
 

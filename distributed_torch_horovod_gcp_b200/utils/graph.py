@@ -1,7 +1,7 @@
 """Whole-step CUDA-graph capture.
 
 The reference workload (LSTM, batch 32, 1.48 MB of gradients) is launch- and sync-bound on a
-B200 (SURVEY.md §2.6: ~0.4 us of math per step), so the B200-first answer is to capture the
+H100 (SURVEY.md §2.6: ~0.4 us of math per step), so the H100-first answer is to capture the
 complete training step — forward, backward, the fused allreduce+optimizer kernels on their side
 stream, and the gradient zeroing — in ONE CUDA graph and replay it.  The comm kernels keep
 their cross-rank epochs in device memory, so a replayed graph stays in lock-step with its

@@ -1,11 +1,12 @@
 """Tiny instances of every hand-written compute kernel, for compute-sanitizer:
     compute-sanitizer --tool racecheck|synccheck|memcheck python scripts/sanitize_kernels.py
 Shapes are small (the tools slow kernels 10-100x) but cover: multi-tile persistent loops (several tiles per
-CTA are not reachable at these sizes on 148 SMs, so max_ctas is forced down where the API allows), the
-statistics / residual / masked-residual / split-K epilogues, 3x3 halo + generic conv paths, BN, LN,
-pooling, attention and the LSTM recurrence."""
-import sys, torch
-sys.path.insert(0, "/root/repo")
+CTA are not reachable at these sizes on 132 SMs, so max_ctas is forced down where the API allows), the
+statistics / residual / masked-residual / split-K epilogues (per-CTA statistics slots, last-arriver split-K
+reduction), 3x3 / strided / 1x1 conv paths incl. split-K wgrad, BN, LN, pooling, attention and the LSTM
+recurrence."""
+import os, sys, torch
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from distributed_torch_horovod_gcp_b200.ops import kernels, gemm as G, conv as C, bn as B
 import torch.nn as nn
 assert kernels.has("conv_implicit_gemm")
@@ -16,7 +17,7 @@ bf = torch.bfloat16
 def rnd(*s, scale=1.0):
     return (torch.randn(*s, device=dev) * scale).to(bf)
 
-# GEMM: plain+stats, residual, masked residual, split-K fp32 accumulate, 2-CTA; few CTAs -> several tiles each
+# GEMM: plain+stats, residual, masked residual, split-K fp32 accumulate; few CTAs -> several tiles each
 M, N, K = 1536, 256, 128
 a, b, r = rnd(M, K), rnd(N, K, scale=0.1), rnd(M, N)
 out = torch.empty(M, N, device=dev, dtype=bf)
@@ -27,10 +28,9 @@ bits = torch.randint(0, 256, (M, N // 8), device=dev, dtype=torch.uint8)
 G.gemm(a, b, out, M, N, K, residual=r, res_mask=bits, max_ctas=4)
 acc = torch.zeros(N, K, device=dev)
 G.gemm(out, a, acc, N, K, M, a_mn=True, b_mn=True, out_mode=1, splits=4)
-G.gemm(a, b, out, M, N, 512 if False else K, two_cta=True, max_ctas=4)
 print("gemm ok", float(out.float().abs().mean()))
 
-# convolutions: halo (64 ch), generic (256 ch), strided, with BN statistics; dgrad + wgrad through autograd
+# convolutions: 64 / 256 ch, strided, 1x1, with BN statistics; dgrad + wgrad (split-K) through autograd
 for cin, cout, k, s, hw in ((64, 64, 3, 1, 16), (256, 256, 3, 1, 8), (128, 128, 3, 2, 16), (256, 512, 1, 2, 8)):
     conv = nn.Conv2d(cin, cout, k, s, (k - 1) // 2, bias=False).to(dev).to(bf).to(memory_format=torch.channels_last)
     bn = nn.BatchNorm2d(cout).to(dev).to(bf)

@@ -1,4 +1,4 @@
-"""`pip install .` builds the sm_100a libraries in-tree first (nvcc cross-compiles without a GPU);
+"""`pip install .` builds the sm_90a libraries in-tree first (nvcc cross-compiles without a GPU);
 the preferred developer flow is still `python -c "import __graft_entry__ as g; g.build()"` so the
 `.so` files stay inside the repository tree (they travel with the snapshot to the GPU box)."""
 import os

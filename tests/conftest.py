@@ -11,7 +11,7 @@ os.environ.setdefault("B200DP_OFFLINE", "1")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100)")
     config.addinivalue_line("markers", "multigpu: needs >= 2 CUDA devices")
 
 

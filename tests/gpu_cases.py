@@ -272,7 +272,7 @@ def watchdog_timeout(hvd):
 
 
 def native_collectives_match_nccl(hvd):
-    """reduce-scatter / all-gather / all-to-all on the sm_100a kernels vs torch.distributed (NCCL)."""
+    """reduce-scatter / all-gather / all-to-all on the sm_90a kernels vs torch.distributed (NCCL)."""
     s = _symm(hvd)
     r, n = hvd.rank(), hvd.size()
     dev = s.device

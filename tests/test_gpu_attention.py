@@ -1,4 +1,4 @@
-"""tcgen05 flash attention (csrc/attn_sm100.cu) vs an fp32 PyTorch reference: forward and all three
+"""wgmma flash attention (csrc/attn_sm90.cu) vs an fp32 PyTorch reference: forward and all three
 gradients, for the ViT-B/16 shape, a multi-block sequence, short sequences and the strided
 [B,S,H,64] layout the model uses."""
 import math

@@ -1,4 +1,4 @@
-"""sm_100a communication kernels vs NCCL (multi-GPU; run with gpurun --gpus N)."""
+"""sm_90a communication kernels vs NCCL (multi-GPU: skipped on machines with fewer than 2 GPUs)."""
 import pytest
 import torch
 

@@ -1,4 +1,4 @@
-"""Implicit-GEMM convolution (csrc/conv_sm100.cu) vs an fp32 PyTorch reference of the same op:
+"""Implicit-GEMM convolution (csrc/conv_sm90.cu) vs an fp32 PyTorch reference of the same op:
 forward, data gradient and weight gradient for every ResNet shape class (3x3 s1, 3x3 s2, 1x1 s2),
 including pixel spaces that do not tile evenly (odd batch, 7x7 / 14x14 maps)."""
 import pytest
@@ -238,7 +238,7 @@ def test_gemm_masked_residual():
                                                  (256, 2048, 1, 1, 7)])
 def test_bn_statistics_from_conv_epilogue(cin, cout, k, stride, hw):
     """conv+BN(+ReLU) with the batch statistics accumulated by the conv / GEMM epilogue == the same unit
-    with the stand-alone statistics pass, for every convolution path (GEMM, implicit GEMM plain / halo,
+    with the stand-alone statistics pass, for every convolution path (GEMM, implicit GEMM,
     strided, stem), twice in a row (the persistent accumulator is re-zeroed by the finalize kernel)."""
     import torch.nn as nn
     from distributed_torch_horovod_gcp_b200.ops import bn as B

@@ -1,4 +1,4 @@
-"""K5 persistent LSTM recurrence (csrc/lstm_rec_sm100.cu) vs PyTorch's LSTM in fp32 (cuDNN TF32 disabled
+"""K5 persistent LSTM recurrence (csrc/lstm_rec_sm90.cu) vs PyTorch's LSTM in fp32 (cuDNN TF32 disabled
 for the oracle): outputs, final state, and gradients of every input and parameter."""
 import pytest
 import torch

@@ -1,5 +1,5 @@
-"""Acceptance tests for the kernels on docs/ROADMAP.md that are NOT built yet (3x3 implicit-GEMM
-conv, attention, persistent LSTM).  Each test skips until `ops.kernels.has(<name>)` turns true, so
+"""Acceptance tests for the 3x3 implicit-GEMM conv, attention and persistent LSTM kernels through their
+`ops.kernels` entry points.  Each test skips until `ops.kernels.has(<name>)` turns true, so
 wiring a new kernel into `ops/_bind.py` activates its numerics check automatically.
 
 Expected entry points (all NHWC / bf16 unless noted):
@@ -17,7 +17,7 @@ pytestmark = pytest.mark.gpu
 def _kern(name):
     from distributed_torch_horovod_gcp_b200.ops import kernels
     if not kernels.has(name):
-        pytest.skip(f"kernel '{name}' is not built yet (docs/ROADMAP.md)")
+        pytest.skip(f"kernel '{name}' is not built")
     return kernels
 
 

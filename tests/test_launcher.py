@@ -47,7 +47,7 @@ def test_reference_command_line_parses():
     a = make_parser().parse_args(["-np", "2", "--fusion-threshold-mb", "32", "--timeline-filename",
                                   "/tmp/t.json", "--", "python", "-c", "pass"])
     assert a.fusion_threshold_mb == 32 and a.command[-1] == "pass"
-    assert "sm_100a" in check_build()
+    assert "sm_90a" in check_build()
 
 
 def _run(args, timeout=120):
