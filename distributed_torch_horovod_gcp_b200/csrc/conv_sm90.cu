@@ -11,7 +11,8 @@
 //   fprop  y[p, co]  = sum_{r,s,ci} x[p + (r,s) - pad, ci] * w[co, r, s, ci]      A = x boxes, B = w (K-major)
 //   dgrad  dx[p, ci] = sum_{r,s,co} dy[p + pad - (r,s), co] * w[co, r, s, ci]     A = dy boxes, B = w (MN-major)
 //   wgrad  dw[co, r, s, ci] = sum_p dy[p, co] * x[p + (r,s) - pad, ci]            A = dy boxes, B = x boxes,
-//          both MN-major with K = 64-pixel boxes; split-K over pixels, fp32 RED.ADD into [Cout][R*S*Cin]
+//          both MN-major with K = 64-pixel boxes; split-K over pixels, the partials added to the fp32
+//          [Cout][R*S*Cin] accumulator in split order (splitk_finish_tile)
 //
 // Stride 2 never uses strided gathers: the input (fprop/wgrad) or the output (dgrad) is addressed
 // through four parity views {C, W/2, H/2, N} (base offset (ph*W + pw)*C, doubled pitches), so every
@@ -520,7 +521,7 @@ int b200dp_conv_dgrad(const void* dy, const void* w, void* dx, int N, int H, int
   return launch_conv<MODE_DGRAD>(maps, p, BN, work, max_ctas, st);
 }
 
-// dw_acc[Cout][R*S*Cin] (fp32) += dy^T (*) x      — split-K over pixels with RED.ADD; the caller zeroes
+// dw_acc[Cout][R*S*Cin] (fp32) += dy^T (*) x      — split-K over pixels, summed in split order; the caller zeroes
 // dw_acc before the first call and converts it to the weight dtype afterwards.
 int b200dp_conv_wgrad(const void* dy, const void* x, void* dw_acc, int N, int H, int W, int Cin, int Cout, int R,
                       int S, int stride, int pad, int splits, int block_n, int max_ctas, unsigned long long stream) {

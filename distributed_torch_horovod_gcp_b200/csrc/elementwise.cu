@@ -7,7 +7,8 @@
 //             (3 reads + 1 write instead of 5 reads + 3 writes)
 //   backward: reduce pass with the ReLU mask recomputed from y, + ONE apply pass that writes dx and
 //             the residual-branch gradient together.
-// Statistics accumulate in fp32 (vector registers -> shared -> one atomicAdd per block/channel).
+// Statistics accumulate in fp32 (vector registers -> shared -> one slot per block, summed in block order
+// by the last block: see block_reduce_to_global).
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -90,9 +91,8 @@ __device__ __forceinline__ void block_reduce_to_global(float (&acc)[NACC][8], in
   if (tid == 0) g_red_done = 0u;
 }
 
-// Reduction kernels run ONE 1024-thread block per SM: same-address fp32 atomics serialise in L2
-// (~40 ns each), so the number of blocks — not the data size — set the tail of the first version
-// (one block per SM instead of several per SM shortens that tail several-fold).
+// Reduction kernels run ONE 1024-thread block per SM: the last block sums one slot per block, so the
+// number of blocks — not the data size — sets the tail of the reduction.
 constexpr int RTHREADS = 1024;
 
 // HBM3 needs >= ~32 KB in flight per SM to saturate (3.35 TB/s x ~1 us over 132 SMs): every kernel below
@@ -772,7 +772,8 @@ int grid_for(long long nvec, int V) {
 }
 
 // fp32 split-K workspace -> gradient tensor: dst (bf16 or fp32) = (accumulate ? dst : 0) + src, and the
-// workspace is re-zeroed in the same pass so the next step's RED.ADDs start from zero without a memset.
+// workspace is re-zeroed in the same pass so the next step's weight gradient, which the GEMM / convolution
+// adds to the workspace, starts from zero without a memset.
 template <bool OUT_BF16>
 __global__ void cast_acc_zero_kernel(float* __restrict__ src, void* __restrict__ dst, long long n4,
                                      int accumulate, int zero_src) {

@@ -4,7 +4,7 @@
 //
 // A and B can each be K-major (row-major [rows][K]) or MN-major (stored [K][rows]), so the
 // same kernel serves linear / 1x1-conv forward (A=x, B=W), dgrad (A=dy, B=W as MN-major) and
-// wgrad (A=dy^T, B=x^T, both MN-major, split-K with fp32 atomics) without any transpose pass:
+// wgrad (A=dy^T, B=x^T, both MN-major, split-K summed in split order) without any transpose pass:
 // wgmma reads MN-major bf16 operands through its transpose flags.
 //
 // Structure (persistent, warp-specialised, one CTA per SM, 384 threads):
@@ -232,7 +232,8 @@ extern "C" {
 const char* b200dp_gemm_last_error() { return g_err; }
 
 // A: K-major -> [M][lda>=K]; MN-major -> [K][lda>=M].   B: K-major -> [N][ldb>=K]; MN-major -> [K][ldb>=N].
-// C: [M][ldc>=N].  out_mode 0: bf16 = act(alpha*AB + bias) + residual; 1: fp32 atomic +=; 2: fp32 store.
+// C: [M][ldc>=N].  out_mode 0: bf16 = act(alpha*AB + bias) + residual; 1: fp32 += alpha*AB (with splits > 1
+// the last split to finish adds the partials of all splits, in split order); 2: fp32 store.
 // Requirements: K % 8 == 0 for K-major operands, M % 8 (A) / N % 8 (B) == 0 for MN-major, N % 8 == 0,
 // 16-byte aligned base pointers and leading dimensions.
 int b200dp_gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, int lda, int ldb, int ldc,
@@ -256,7 +257,7 @@ int b200dp_gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K,
   p.num_k_blocks = (K + BLOCK_K - 1) / BLOCK_K;
   p.splits = splits < 1 ? 1 : splits;
   if (p.splits > p.num_k_blocks) p.splits = p.num_k_blocks;
-  if (p.splits > 1 && out_mode != 1) return fail("split-K requires out_mode=1 (fp32 atomic add)");
+  if (p.splits > 1 && out_mode != 1) return fail("split-K requires out_mode=1 (fp32 accumulate)");
   {  // no empty splits
     const int per = (p.num_k_blocks + p.splits - 1) / p.splits;
     p.splits = (p.num_k_blocks + per - 1) / per;

@@ -28,7 +28,7 @@ struct GemmParams {
   int num_m_blocks, num_n_blocks, num_k_blocks;
   int splits;              // split-K factor (>=1)
   int act;                 // 0 none, 1 relu, 2 gelu(erf), 3 *gelu'(aux), 4 *(aux>0)  [aux = residual ptr]
-  int out_mode;            // 0: bf16 store, 1: fp32 atomic add (split-K / accumulate), 2: fp32 store
+  int out_mode;            // 0: bf16 store, 1: fp32 add into C (split-K: see splitk_finish_tile), 2: fp32 store
   void* C;
   const void* bias;        // bf16 [N] or nullptr
   const void* bias_f32;    // fp32 [N] or nullptr
@@ -338,7 +338,8 @@ struct Cfg {
 
 // Epilogue of one 32-row slab (rows 32q..32q+31) of a 128 x BN accumulator: accumulator image ->
 // registers -> alpha/bias/activation/residual -> bf16 via swizzled smem + TMA bulk store, or fp32
-// store / atomic add.
+// store / add (one partial per element without split-K; with split-K a store into the split's
+// workspace slice).
 // Where a 32-row slab goes.  rank4 == 0: rows m_row0.. of the row-major [M, ldc] matrix (2D map).
 // rank4 == 1 (convolution): the slab is the {64 c, sw, sh, sn} sub-box at pixel (w, h, n) of an NHWC
 // tensor; c_ptr/ld override p.C/p.ldc for the fp32 modes (per-tap column offset of the wgrad output).
@@ -634,14 +635,21 @@ __device__ __forceinline__ void epilogue_rows(const GemmParams& p, const CUtenso
         // batch statistics of the following BatchNorm: column sums of the bf16 values just staged.  Lane l
         // owns columns 2l, 2l+1 of this 64-column chunk and walks the 32 staged rows (one conflict-free
         // 4-byte shared load per row); partials go to the warp's private shared
-        // accumulators.  GEMM rows past M come from zero-filled operands and add nothing; rows of a
-        // convolution tile outside the image are masked (they see partly valid taps).
+        // accumulators.  Rows that are not part of the output are masked: rows of a convolution tile
+        // outside the image (they see partly valid taps) and GEMM rows past M (zero-filled operands, but
+        // the epilogue may still have added a bias or an activation of it).
         float sum_lo = 0.f, sum_hi = 0.f, sq_lo = 0.f, sq_hi = 0.f;
         const uint32_t base = out_s + (uint32_t)((lane & 3) << 2);
         const uint32_t u = (uint32_t)(lane >> 2);
-        if (at.rank4) {      // lane r decides for slab row r
-          const int rw = lane % at.sw, rh = (lane / at.sw) % at.sh, rn = lane / (at.sw * at.sh);
-          const uint32_t rows_ok = __ballot_sync(0xffffffffu, rw < at.vw && rh < at.vh && rn < at.vn);
+        if (at.rank4 || m_row0 + 32 > p.M) {      // lane r decides for slab row r
+          bool ok;
+          if (at.rank4) {
+            const int rw = lane % at.sw, rh = (lane / at.sw) % at.sh, rn = lane / (at.sw * at.sh);
+            ok = rw < at.vw && rh < at.vh && rn < at.vn;
+          } else {
+            ok = m_row0 + lane < p.M;
+          }
+          const uint32_t rows_ok = __ballot_sync(0xffffffffu, ok);
 #pragma unroll
           for (int rr = 0; rr < 32; ++rr) {
             uint32_t w;

@@ -7,7 +7,8 @@ Weights are consumed as ``[Cout][R][S][Cin]`` — PyTorch's ``channels_last`` la
 ``[Cout, Cin, R, S]`` parameter — so ``model.to(memory_format=torch.channels_last)`` makes the
 parameter itself the GEMM B operand; a parameter in the default layout is re-laid-out per call.
 
-The weight gradient is accumulated in a per-weight fp32 split-K workspace (RED.ADD.F32) that is
+The weight gradient is added to a per-weight fp32 workspace (split-K over pixels: the last split to
+finish adds the partial sums of all splits in split order, so the result is bit-reproducible) that is
 converted to the gradient dtype and re-zeroed by ONE pass (``b200dp_cast_acc_zero``); when the
 parameter carries a ``grad_sink`` (installed by the fused engine) that pass writes straight into
 the parameter's slot of the gradient bucket and fires the bucket counter, so autograd's

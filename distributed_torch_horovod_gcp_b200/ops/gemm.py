@@ -3,7 +3,7 @@
     y = act(x @ W^T + b) (+ residual)          forward : A = x (K-major),  B = W (K-major)
     dx = dy' @ W                                dgrad   : A = dy' (K-major), B = W (MN-major)
     dW = dy'^T @ x                              wgrad   : A = dy' (MN-major), B = x (MN-major),
-                                                          split-K, fp32 atomics
+                                                          split-K, partials summed in split order
 No transposes are materialised: the kernel takes MN-major operands through its GMMA
 descriptors.  ``dy' = dy * act'(z)`` is fused into the dgrad of the *next* layer's epilogue
 where possible; here it is computed by the epilogue modes 3/4 of the kernel when the layer

@@ -64,7 +64,7 @@ def test_gemm_epilogues_and_splitk():
     o32 = torch.empty(M, N, device="cuda", dtype=torch.float32)
     g.gemm(a, b, o32, M, N, K, bias=bias.float(), out_mode=2)
     assert _rel(o32, ref0) < 2e-3
-    # split-K with fp32 atomics accumulates on top of existing contents
+    # split-K (partials summed in split order by the last split) adds onto the existing contents
     acc = torch.ones(M, N, device="cuda", dtype=torch.float32)
     g.gemm(a, b, acc, M, N, K, out_mode=1, splits=5)
     assert _rel(acc, a.float() @ b.float().t() + 1.0) < 2e-3
