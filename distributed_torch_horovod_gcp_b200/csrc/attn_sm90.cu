@@ -439,40 +439,13 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
 }
 
 // ------------------------------------------------------------------ host side
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
-                                  CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
-                                  CUtensorMapFloatOOBfill);
-EncodeTiledFn g_encode = nullptr;
-thread_local char g_err[512];
-
-int fail(const char* msg, int code = 0) {
-  snprintf(g_err, sizeof(g_err), "%s (%d)", msg, code);
-  return -1;
-}
-int ensure_init() {
-  bind_primary_context();
-  if (g_encode) return 0;
-  void* fn = nullptr;
-  cudaDriverEntryPointQueryResult st;
-  cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &st);
-  if (e != cudaSuccess || st != cudaDriverEntryPointSuccess || !fn)
-    return fail("cuTensorMapEncodeTiled entry point unavailable", (int)e);
-  g_encode = reinterpret_cast<EncodeTiledFn>(fn);
-  return 0;
-}
 // {64 d, S, H, B} view with element strides (ss, sh, sb); box {64, 128, 1, 1}
 int make_qkv_map(CUtensorMap* m, const void* ptr, int B, int H, int S, long long sb, long long sh, long long ss) {
   if ((ss % 8) || (sh % 8) || (sb % 8) || ((uintptr_t)ptr & 15)) return fail("attention operands must be 16-byte aligned");
-  cuuint64_t dims[4] = {(cuuint64_t)HD, (cuuint64_t)S, (cuuint64_t)H, (cuuint64_t)B};
-  cuuint64_t strides[3] = {(cuuint64_t)ss * 2, (cuuint64_t)sh * 2, (cuuint64_t)sb * 2};
-  cuuint32_t box[4] = {64, TILE, 1, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled(attention) failed", (int)r);
-  return 0;
+  const cuuint64_t dims[4] = {(cuuint64_t)HD, (cuuint64_t)S, (cuuint64_t)H, (cuuint64_t)B};
+  const cuuint64_t strides[3] = {(cuuint64_t)ss * 2, (cuuint64_t)sh * 2, (cuuint64_t)sb * 2};
+  const cuuint32_t box[4] = {64, TILE, 1, 1};
+  return encode_map(m, ptr, 4, dims, strides, box);
 }
 
 }  // namespace
@@ -500,12 +473,7 @@ int b200dp_attn_fwd(const void* q, const void* k, const void* v, void* o, float*
   p.o = reinterpret_cast<__nv_bfloat16*>(o);
   p.o_sb = os[0]; p.o_sh = os[1]; p.o_ss = os[2];
   p.lse = lse;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FW_SMEM);
-    if (e != cudaSuccess) return fail(cudaGetErrorString(e), (int)e);
-    attr_set = true;
-  }
+  if (smem_attr_once<attn_fwd_kernel>(FW_SMEM)) return -1;
   attn_fwd_kernel<<<B * H * p.q_tiles, AT, FW_SMEM, (cudaStream_t)(uintptr_t)stream>>>(mq, mk, mv, p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(cudaGetErrorString(e), (int)e);
@@ -541,12 +509,7 @@ int b200dp_attn_bwd(const void* q, const void* k, const void* v, const void* o, 
   p.dk = reinterpret_cast<__nv_bfloat16*>(dk); p.dv = reinterpret_cast<__nv_bfloat16*>(dv);
   p.dk_sb = dks[0]; p.dk_sh = dks[1]; p.dk_ss = dks[2];
   p.dv_sb = dvs[0]; p.dv_sh = dvs[1]; p.dv_ss = dvs[2];
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BW_SMEM);
-    if (e != cudaSuccess) return fail(cudaGetErrorString(e), (int)e);
-    attr_set = true;
-  }
+  if (smem_attr_once<attn_bwd_kernel>(BW_SMEM)) return -1;
   attn_bwd_kernel<<<B * H * p.kv_blocks, AT, BW_SMEM, st>>>(mq, mk, mv, mdo, p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(cudaGetErrorString(e), (int)e);

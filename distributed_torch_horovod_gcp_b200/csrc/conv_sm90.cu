@@ -53,6 +53,7 @@ struct ConvParams {
   int num_classes;
   int kc_per_tap;                 // 64-channel chunks of the reduction dimension per tap (fprop/dgrad)
   int bw, bh, bn;                 // pixel box: 128 rows of an M tile (fprop/dgrad) / 64 rows of a K block (wgrad)
+  int sw, sh;                     // fprop/dgrad: {sw, sh, .} pixel box of one 32-row slab of the M tile
   int tiles_w, tiles_h, tiles_n;  // boxes covering the (class) output pixel space
   int num_taps_total;             // wgrad: R*S
   int out_w, out_h, out_n;        // extent of the (class) output pixel space: rows beyond it are clipped / not counted
@@ -66,238 +67,121 @@ struct alignas(64) ConvMaps {
 
 enum { MODE_FPROP = 0, MODE_DGRAD = 1, MODE_WGRAD = 2 };
 
+// fprop/dgrad: work = class x pixel tile x n block (n fastest: the A boxes of one pixel tile are re-used from
+// L2 by the CTAs working on its other n blocks); K blocks = taps x channel chunks.
+// wgrad: work = split x (m block x n block x tap), tap fastest: the dy / x boxes of one pixel range are shared
+// through L2 by the CTAs of the same split; K blocks = 64-pixel boxes.
 template <int BN, int MODE>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-conv_bf16_kernel(const __grid_constant__ ConvMaps maps, const __grid_constant__ ConvParams p) {
-  using C = Cfg<BN>;
-  constexpr bool A_MN = (MODE == MODE_WGRAD);
-  constexpr bool B_MN = (MODE != MODE_FPROP);
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + C::STAGES * C::A_BYTES;
-  uint8_t* smem_store = smem + C::STAGES * C::STAGE_BYTES;
-  uint8_t* smem_acc = smem_store + C::STORE_BYTES;           // accumulator image [128][BN + 4] fp32
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_acc + C::ACC_BYTES);
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + C::STAGES;
-  float* s_stats = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 256);
-  const bool want_stats = MODE == MODE_FPROP && p.g.stats != nullptr;
-  if (want_stats) stats_zero(s_stats, NUM_THREADS, p.g.N);
+struct ConvWork {
+  static constexpr bool kStats = MODE == MODE_FPROP, kSplitK = MODE == MODE_WGRAD;
+  static constexpr bool B_MN = MODE != MODE_FPROP;
+  const ConvMaps& maps;
+  const ConvParams& p;
+  int nnb, pix_tiles, tiles, items, kb_per_split;
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-
-  if (warp == 0 && lane == 0) {
+  __device__ ConvWork(const ConvMaps& maps_, const ConvParams& p_)
+      : maps(maps_), p(p_), nnb(p_.g.num_n_blocks), pix_tiles(p_.tiles_w * p_.tiles_h * p_.tiles_n),
+        tiles(MODE == MODE_WGRAD ? p_.g.num_m_blocks * nnb * p_.num_taps_total : p_.num_classes * pix_tiles * nnb),
+        items(tiles * p_.g.splits),
+        kb_per_split(MODE == MODE_WGRAD ? (pix_tiles + p_.g.splits - 1) / p_.g.splits : 0) {}
+  __device__ void prefetch() const {
     for (int i = 0; i < 4; ++i) tma_prefetch_desc(&maps.a[i]);
     tma_prefetch_desc(&maps.b);
     for (int i = 0; i < 4; ++i) tma_prefetch_desc(&maps.out[i]);
-    for (int i = 0; i < C::STAGES; ++i) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 2);               // one arrival per consumer warpgroup
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  __syncthreads();
-
-  const int nnb = p.g.num_n_blocks;
-  const int pix_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
-  // fprop/dgrad: work = class x pixel tile x n block (n fastest: the A boxes of one pixel tile are
-  // re-used from L2 by the CTAs working on its other n blocks).
-  // wgrad: work = split x (m block x n block x tap), tap fastest: the dy / x boxes of one pixel range
-  // are shared through L2 by the CTAs of the same split.
-  const int tiles = (MODE == MODE_WGRAD) ? p.g.num_m_blocks * nnb * p.num_taps_total
-                                         : p.num_classes * pix_tiles * nnb;
-  const int work_items = tiles * p.g.splits;
-  const int kb_per_split = (MODE == MODE_WGRAD) ? (pix_tiles + p.g.splits - 1) / p.g.splits : 0;
-
-  if (warp < 4) {
-    // ============================ TMA producer ============================
-    if (warp == 0 && lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int w = blockIdx.x; w < work_items; w += gridDim.x) {
-        if (MODE != MODE_WGRAD) {
-          const int nt = w % nnb;
-          const int rest = w / nnb;
-          const int mt = rest % pix_tiles;
-          const ConvClass& cl = p.cls[rest / pix_tiles];
-          const int w0 = (mt % p.tiles_w) * p.bw;
-          const int h0 = ((mt / p.tiles_w) % p.tiles_h) * p.bh;
-          const int n0 = (mt / (p.tiles_w * p.tiles_h)) * p.bn;
-          const int n_idx = nt * BN;
-          for (int t = 0; t < cl.ntaps; ++t) {
-            const ConvTap tap = cl.taps[t];
-            for (int kc = 0; kc < p.kc_per_tap; ++kc) {
-              mbar_wait(&empty_bar[stage], phase ^ 1);
-              mbar_expect_tx(&full_bar[stage], C::STAGE_BYTES);
-              uint8_t* sa = smem_a + stage * C::A_BYTES;
-              uint8_t* sb = smem_b + stage * C::B_BYTES;
-              tma_load_4d(&maps.a[tap.amap], &full_bar[stage], sa, kc * BLOCK_K, w0 + tap.dw, h0 + tap.dh, n0);
-              if (!B_MN) {
-                tma_load_2d(&maps.b, &full_bar[stage], sb, tap.wcol + kc * BLOCK_K, n_idx);   // box {64 k, BN co}
-              } else {
+  __device__ int num_kb(int w) const {
+    if (MODE != MODE_WGRAD) return p.cls[(w / nnb) / pix_tiles].ntaps * p.kc_per_tap;
+    const int kb0 = (w / tiles) * kb_per_split;
+    return min(kb0 + kb_per_split, pix_tiles) - kb0;
+  }
+  template <class Next>
+  __device__ void load(int w, Next& next) const {
+    if (MODE != MODE_WGRAD) {
+      const int nt = w % nnb;
+      const int rest = w / nnb;
+      const int mt = rest % pix_tiles;
+      const ConvClass& cl = p.cls[rest / pix_tiles];
+      const int w0 = (mt % p.tiles_w) * p.bw;
+      const int h0 = ((mt / p.tiles_w) % p.tiles_h) * p.bh;
+      const int n0 = (mt / (p.tiles_w * p.tiles_h)) * p.bn;
+      const int n_idx = nt * BN;
+      for (int t = 0; t < cl.ntaps; ++t) {
+        const ConvTap tap = cl.taps[t];
+        for (int kc = 0; kc < p.kc_per_tap; ++kc) {
+          const Stage s = next();
+          tma_load_4d(&maps.a[tap.amap], s.bar, s.a, kc * BLOCK_K, w0 + tap.dw, h0 + tap.dh, n0);
+          if (!B_MN) {
+            tma_load_2d(&maps.b, s.bar, s.b, tap.wcol + kc * BLOCK_K, n_idx);   // box {64 k, BN co}
+          } else {
 #pragma unroll
-                for (int c = 0; c < BN / 64; ++c)                                           // box {64 ci, 64 co}
-                  tma_load_2d(&maps.b, &full_bar[stage], sb + c * (BLOCK_K * 128), tap.wcol + n_idx + 64 * c,
-                              kc * BLOCK_K);
-              }
-              if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-            }
-          }
-        } else {
-          const int tile = w % tiles, split = w / tiles;
-          const ConvTap tap = p.cls[0].taps[tile % p.num_taps_total];
-          const int mn = tile / p.num_taps_total;
-          const int m_idx = (mn / nnb) * BLOCK_M;
-          const int n_idx = (mn % nnb) * BN;
-          const int kb0 = split * kb_per_split;
-          const int kb1 = min(kb0 + kb_per_split, pix_tiles);
-          for (int kb = kb0; kb < kb1; ++kb) {
-            const int w0 = (kb % p.tiles_w) * p.bw;
-            const int h0 = ((kb / p.tiles_w) % p.tiles_h) * p.bh;
-            const int n0 = (kb / (p.tiles_w * p.tiles_h)) * p.bn;
-            mbar_wait(&empty_bar[stage], phase ^ 1);
-            mbar_expect_tx(&full_bar[stage], C::STAGE_BYTES);
-            uint8_t* sa = smem_a + stage * C::A_BYTES;
-            uint8_t* sb = smem_b + stage * C::B_BYTES;
-#pragma unroll
-            for (int c = 0; c < BLOCK_M / 64; ++c)      // dy: 64 pixels x 64 output channels per box
-              tma_load_4d(&maps.out[0], &full_bar[stage], sa + c * (BLOCK_K * 128), m_idx + 64 * c, w0, h0, n0);
-#pragma unroll
-            for (int c = 0; c < BN / 64; ++c)           // x : the same pixels shifted by the tap
-              tma_load_4d(&maps.a[tap.amap], &full_bar[stage], sb + c * (BLOCK_K * 128), n_idx + 64 * c,
-                          w0 + tap.dw, h0 + tap.dh, n0);
-            if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+            for (int c = 0; c < BN / 64; ++c)                                  // box {64 ci, 64 co}
+              tma_load_2d(&maps.b, s.bar, s.b + c * (BLOCK_K * 128), tap.wcol + n_idx + 64 * c, kc * BLOCK_K);
           }
         }
       }
+    } else {
+      const int tile = w % tiles, split = w / tiles;
+      const ConvTap tap = p.cls[0].taps[tile % p.num_taps_total];
+      const int mn = tile / p.num_taps_total;
+      const int m_idx = (mn / nnb) * BLOCK_M;
+      const int n_idx = (mn % nnb) * BN;
+      const int kb0 = split * kb_per_split;
+      const int kb1 = min(kb0 + kb_per_split, pix_tiles);
+      for (int kb = kb0; kb < kb1; ++kb) {
+        const int w0 = (kb % p.tiles_w) * p.bw;
+        const int h0 = ((kb / p.tiles_w) % p.tiles_h) * p.bh;
+        const int n0 = (kb / (p.tiles_w * p.tiles_h)) * p.bn;
+        const Stage s = next();
+#pragma unroll
+        for (int c = 0; c < BLOCK_M / 64; ++c)      // dy: 64 pixels x 64 output channels per box
+          tma_load_4d(&maps.out[0], s.bar, s.a + c * (BLOCK_K * 128), m_idx + 64 * c, w0, h0, n0);
+#pragma unroll
+        for (int c = 0; c < BN / 64; ++c)           // x : the same pixels shifted by the tap
+          tma_load_4d(&maps.a[tap.amap], s.bar, s.b + c * (BLOCK_K * 128), n_idx + 64 * c, w0 + tap.dw,
+                      h0 + tap.dh, n0);
+      }
     }
-  } else {
-    // ============================ wgmma + epilogue (warpgroups 1-2) ============================
-    const int cw = warp - 4;
-    const int wg = cw >> 2;
-    const int q = cw & 3;
-    const int half = cw >> 2;
-    const int c_begin = (BN >= 128) ? half * (BN / 2) : 0;
-    const int c_end = (BN >= 128) ? c_begin + BN / 2 : (half == 0 ? BN : 0);
-    uint8_t* my_store = smem_store + cw * (2 * 4096);
-    float* my_stats = s_stats + cw * STATS_WARP_FLOATS;
-    const uint32_t img = smem_u32(smem_acc);
-    __shared__ int s_last;
-    int stats_n = -1;
-    int stage = 0, acc = 0;
-    uint32_t phase = 0;
-    float d[BN / 2];
-    for (int w = blockIdx.x; w < work_items; w += gridDim.x) {
-      int nkb;
-      if (MODE != MODE_WGRAD) {
-        nkb = p.cls[(w / nnb) / pix_tiles].ntaps * p.kc_per_tap;
-      } else {
-        const int kb0 = (w / tiles) * kb_per_split;
-        nkb = min(kb0 + kb_per_split, pix_tiles) - kb0;
-      }
-      wg_mainloop<BN, A_MN, B_MN, C::STAGES, C::A_BYTES, C::B_BYTES>(d, smem_u32(smem_a), smem_u32(smem_b), full_bar,
-                                                                     empty_bar, stage, phase, nkb, wg);
-      if (want_stats && (w % nnb) != stats_n) {
-        if (stats_n >= 0) stats_flush<BN>(p.g, s_stats, stats_n * BN, cw * 32 + lane);
-        stats_n = w % nnb;
-      }
-      named_bar(1, 256);                          // the previous tile's image has been read
-      acc_to_smem<BN>(d, img, BN + 4, wg * 64);
-      named_bar(1, 256);
-      if (MODE != MODE_WGRAD) {
-        const int nt = w % nnb;
-        const int rest = w / nnb;
-        const int mt = rest % pix_tiles;
-        const ConvClass& cl = p.cls[rest / pix_tiles];
-        const int r0 = q * 32;                                   // first row of this warp's slab in the box
-        StoreAt at;
-        at.rank4 = 1;
-        at.w = (mt % p.tiles_w) * p.bw + (r0 % p.bw);
-        at.h = ((mt / p.tiles_w) % p.tiles_h) * p.bh + (r0 / p.bw) % p.bh;
-        at.n = (mt / (p.tiles_w * p.tiles_h)) * p.bn + r0 / (p.bw * p.bh);
-        at.c_ptr = nullptr;
-        at.sw = p.bw < 32 ? p.bw : 32;
-        at.sh = (32 / at.sw) < p.bh ? (32 / at.sw) : p.bh;
-        at.vw = p.out_w - at.w; at.vh = p.out_h - at.h; at.vn = p.out_n - at.n;
-        epilogue_rows<BN>(p.g, &maps.out[cl.out_map], nullptr, img, acc, q, lane, 0, nt * BN, c_begin,
-                          c_end, my_store, at, want_stats ? my_stats : nullptr);
-      } else {
-        const int tile = w % tiles;
-        const ConvTap tap = p.cls[0].taps[tile % p.num_taps_total];
-        const int mn = tile / p.num_taps_total;
-        StoreAt at;
-        at.rank4 = 0; at.w = at.h = at.n = 0;
-        at.sw = 32; at.sh = 1; at.vw = 32; at.vh = 1; at.vn = 1;
-        at.c_ptr = (p.g.splits > 1 ? p.g.splitk_ws + (long long)(w / tiles) * p.g.splitk_slice
-                                   : reinterpret_cast<float*>(p.g.C)) + tap.wcol;
-        epilogue_rows<BN>(p.g, nullptr, nullptr, img, acc, q, lane, (mn / nnb) * BLOCK_M + q * 32,
-                          (mn % nnb) * BN, c_begin, c_end, my_store, at);
-        if (p.g.splits > 1)
-          splitk_finish_tile(p.g, tile, (mn / nnb) * BLOCK_M, (mn % nnb) * BN, BN, tap.wcol, cw * 32 + lane, &s_last);
-      }
-      acc ^= 1;
-    }
-    if (want_stats && stats_n >= 0) stats_flush<BN>(p.g, s_stats, stats_n * BN, cw * 32 + lane);
-    if (want_stats) stats_finalize(p.g, cw * 32 + lane);
-    if (MODE != MODE_WGRAD && lane == 0) tma_store_wait_all();
   }
-}
+  __device__ Slab slab(int w, int q) const {
+    if (MODE != MODE_WGRAD) {
+      const int nt = w % nnb;
+      const int rest = w / nnb;
+      const int mt = rest % pix_tiles;
+      const int r0 = q * 32;                                   // first row of this warp's slab in the box
+      StoreAt at;
+      at.rank4 = 1;
+      at.w = (mt % p.tiles_w) * p.bw + (r0 % p.bw);
+      at.h = ((mt / p.tiles_w) % p.tiles_h) * p.bh + (r0 / p.bw) % p.bh;
+      at.n = (mt / (p.tiles_w * p.tiles_h)) * p.bn + r0 / (p.bw * p.bh);
+      at.c_ptr = nullptr;
+      at.sw = p.sw; at.sh = p.sh;
+      at.vw = p.out_w - at.w; at.vh = p.out_h - at.h; at.vn = p.out_n - at.n;
+      return Slab{&maps.out[p.cls[rest / pix_tiles].out_map], nullptr, 0, nt * BN, at, 0, 0, 0};
+    }
+    const int tile = w % tiles;
+    const ConvTap tap = p.cls[0].taps[tile % p.num_taps_total];
+    const int mn = tile / p.num_taps_total;
+    const int m_idx = (mn / nnb) * BLOCK_M;
+    float* c_ptr = (p.g.splits > 1 ? p.g.splitk_ws + (long long)(w / tiles) * p.g.splitk_slice
+                                   : reinterpret_cast<float*>(p.g.C)) + tap.wcol;
+    return Slab{nullptr, nullptr, m_idx + q * 32, (mn % nnb) * BN, StoreAt{0, 0, 0, 0, c_ptr, 32, 1, 32, 1, 1},
+                tile, m_idx, tap.wcol};
+  }
+};
 
-// ------------------------------------------------------------------ host side
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
-                                  CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
-                                  CUtensorMapFloatOOBfill);
-EncodeTiledFn g_encode = nullptr;
-thread_local char g_err[512];
-int g_num_sms = 0;
-
-int fail(const char* msg, int code = 0) {
-  snprintf(g_err, sizeof(g_err), "%s (%d)", msg, code);
-  return -1;
-}
-
-int ensure_init() {
-  bind_primary_context();
-  if (g_encode) return 0;
-  void* fn = nullptr;
-  cudaDriverEntryPointQueryResult st;
-  cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &st);
-  if (e != cudaSuccess || st != cudaDriverEntryPointSuccess || !fn)
-    return fail("cuTensorMapEncodeTiled entry point unavailable", (int)e);
-  g_encode = reinterpret_cast<EncodeTiledFn>(fn);
-  int dev = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-  return 0;
+template <int BN, int MODE>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+conv_bf16_kernel(const __grid_constant__ ConvMaps maps, const __grid_constant__ ConvParams p) {
+  persistent_body<BN, MODE == MODE_WGRAD, MODE != MODE_FPROP>(ConvWork<BN, MODE>(maps, p), p.g);
 }
 
 // 4D bf16 view {C, Wd, Hd, Nd} of an NHWC tensor (element pitches pw/ph/pn), box {64, bw, bh, bn}.
 int make_map4(CUtensorMap* m, const void* ptr, uint64_t C, uint64_t Wd, uint64_t Hd, uint64_t Nd, uint64_t pw,
               uint64_t ph, uint64_t pn, uint32_t bw, uint32_t bh, uint32_t bn) {
-  cuuint64_t dims[4] = {C, Wd, Hd, Nd};
-  cuuint64_t strides[3] = {pw * 2, ph * 2, pn * 2};
-  cuuint32_t box[4] = {64, bw, bh, bn};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                        CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled(4D) failed", (int)r);
-  return 0;
-}
-int make_map2(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows) {
-  cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {ld * 2};
-  cuuint32_t box[2] = {64, box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                        CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled(2D) failed", (int)r);
-  return 0;
+  const cuuint64_t dims[4] = {C, Wd, Hd, Nd};
+  const cuuint64_t strides[3] = {pw * 2, ph * 2, pn * 2};
+  const cuuint32_t box[4] = {64, bw, bh, bn};
+  return encode_map(m, ptr, 4, dims, strides, box);
 }
 
 // Pixel box {bw, bh, bn} (powers of two, bw*bh*bn == rows) that covers a W x H x N pixel space with the
@@ -344,52 +228,43 @@ int make_parity_maps(CUtensorMap* maps, const void* base, int C, int W, int H, i
   return 0;
 }
 
-void slab_box(int bw, int bh, int bn, int* sw, int* sh, int* sn) {
-  *sw = bw < 32 ? bw : 32;
-  *sh = (32 / *sw) < bh ? (32 / *sw) : bh;
-  *sn = 32 / (*sw * *sh);
-  (void)bn;
+// Taps of fprop and wgrad: tap (r, s) reads the input box shifted by (r - pad, s - pad); with stride 2 that is a
+// shift inside one of the four parity views of the input.
+void forward_taps(ConvClass& cl, int R, int S, int Cin, int stride, int pad) {
+  for (int r = 0; r < R; ++r)
+    for (int c = 0; c < S; ++c) {
+      ConvTap& t = cl.taps[cl.ntaps++];
+      const int eh = r - pad, ew = c - pad;
+      if (stride == 1) {
+        t.amap = 0; t.dh = eh; t.dw = ew;
+      } else {
+        const int ph = eh & 1, pw = ew & 1;
+        t.amap = ph * 2 + pw; t.dh = floordiv2(eh - ph); t.dw = floordiv2(ew - pw);
+      }
+      t.wcol = (r * S + c) * Cin;
+    }
+}
+
+// {sw, sh, 32 / (sw * sh)} pixel box of one 32-row slab of the {bw, bh, bn} M tile: the bulk-store box
+void slab_box(ConvParams& p) {
+  p.sw = p.bw < 32 ? p.bw : 32;
+  p.sh = (32 / p.sw) < p.bh ? (32 / p.sw) : p.bh;
 }
 
 template <int MODE>
 int launch_conv(const ConvMaps& maps, const ConvParams& p, int BN, int work, int max_ctas, cudaStream_t st) {
-  int grid = work < g_num_sms ? work : g_num_sms;
-  if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
-  if (grid > STATS_MAX_CTAS) grid = STATS_MAX_CTAS;
-#define CONV_LAUNCH(BNV)                                                                                \
-  if (BN == BNV) {                                                                                      \
-    auto kern = conv_bf16_kernel<BNV, MODE>;                                                            \
-    static bool attr_set = false;                                                                       \
-    if (!attr_set) {                                                                                    \
-      cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,           \
-                                           Cfg<BNV>::SMEM_BYTES);                                       \
-      if (e != cudaSuccess) return fail(cudaGetErrorString(e), (int)e);                                 \
-      attr_set = true;                                                                                  \
-    }                                                                                                   \
-    kern<<<grid, NUM_THREADS, Cfg<BNV>::SMEM_BYTES, st>>>(maps, p);                                     \
-    cudaError_t e = cudaGetLastError();                                                                 \
-    if (e != cudaSuccess) return fail(cudaGetErrorString(e), (int)e);                                   \
-    return 0;                                                                                           \
-  }
-  CONV_LAUNCH(64)
-  CONV_LAUNCH(128)
-#undef CONV_LAUNCH
-  return fail("block_n must be 64/128/256");
+  if (BN == 64) return launch_persistent<conv_bf16_kernel<64, MODE>, 64>(work, max_ctas, st, maps, p);
+  return launch_persistent<conv_bf16_kernel<128, MODE>, 128>(work, max_ctas, st, maps, p);
 }
 
-
-void init_gemm_params(GemmParams& g) {
-  memset(&g, 0, sizeof(g));
-  g.M = INT_MAX;
-  g.splits = 1;
-  g.alpha = 1.0f;
-  g.n_fastest = 1;
-}
-
-int pick_bn(int n, int block_n) {
-  // 128 is the widest tile whose accumulator image fits in shared memory next to the operand ring
-  if (block_n) return block_n == 256 ? 128 : block_n;
-  return n > 64 ? 128 : 64;
+// zeroed parameters of a single-split convolution (no row limit: rows outside the output are clipped by TMA)
+ConvParams conv_params() {
+  ConvParams p;
+  memset(&p, 0, sizeof(p));
+  p.g.M = INT_MAX;
+  p.g.splits = 1;
+  p.g.alpha = 1.0f;
+  return p;
 }
 
 }  // namespace
@@ -406,11 +281,10 @@ int b200dp_conv_fprop(const void* x, const void* w, void* y, int N, int H, int W
   if (check_shape(s)) return -1;
   if (((uintptr_t)x | (uintptr_t)w | (uintptr_t)y) & 15) return fail("pointers must be 16-byte aligned");
   const int BN = pick_bn(Cout, block_n);
+  if (BN < 0) return -1;
   ConvMaps maps;
-  ConvParams p;
-  memset(&p, 0, sizeof(p));
-  init_gemm_params(p.g);
-  p.g.N = Cout; p.g.K = Cin; p.g.ldc = Cout; p.g.C = y; p.g.out_mode = 0; p.g.tma_store = 1;
+  ConvParams p = conv_params();
+  p.g.N = Cout; p.g.ldc = Cout; p.g.C = y; p.g.out_mode = 0;
   p.g.stats = stats;
   if (stats != nullptr && Cout > STATS_MAX_N) return fail("stats: Cout <= 2048 required");
   p.g.num_n_blocks = (Cout + BN - 1) / BN;
@@ -421,20 +295,7 @@ int b200dp_conv_fprop(const void* x, const void* w, void* y, int N, int H, int W
   p.num_classes = 1;
   p.num_taps_total = R * S;
   p.out_w = s.OW; p.out_h = s.OH; p.out_n = N;
-  ConvClass& cl = p.cls[0];
-  cl.out_map = 0;
-  for (int r = 0; r < R; ++r)
-    for (int c = 0; c < S; ++c) {
-      ConvTap& t = cl.taps[cl.ntaps++];
-      const int eh = r - pad, ew = c - pad;
-      if (stride == 1) {
-        t.amap = 0; t.dh = eh; t.dw = ew;
-      } else {
-        const int ph = eh & 1, pw = ew & 1;
-        t.amap = ph * 2 + pw; t.dh = floordiv2(eh - ph); t.dw = floordiv2(ew - pw);
-      }
-      t.wcol = (r * S + c) * Cin;
-    }
+  forward_taps(p.cls[0], R, S, Cin, stride, pad);
   if (stride == 1) {
     if (make_map4(&maps.a[0], x, Cin, W, H, N, Cin, (uint64_t)W * Cin, (uint64_t)H * W * Cin, p.bw, p.bh, p.bn))
       return -1;
@@ -443,10 +304,9 @@ int b200dp_conv_fprop(const void* x, const void* w, void* y, int N, int H, int W
     return -1;
   }
   if (make_map2(&maps.b, w, Cout, (uint64_t)R * S * Cin, (uint64_t)R * S * Cin, BN)) return -1;
-  int sw, sh, sn;
-  slab_box(p.bw, p.bh, p.bn, &sw, &sh, &sn);
-  if (make_map4(&maps.out[0], y, Cout, s.OW, s.OH, N, Cout, (uint64_t)s.OW * Cout, (uint64_t)s.OH * s.OW * Cout, sw,
-                sh, sn))
+  slab_box(p);
+  if (make_map4(&maps.out[0], y, Cout, s.OW, s.OH, N, Cout, (uint64_t)s.OW * Cout, (uint64_t)s.OH * s.OW * Cout, p.sw,
+                p.sh, 32 / (p.sw * p.sh)))
     return -1;
   maps.out[1] = maps.out[2] = maps.out[3] = maps.out[0];
   const int work = p.tiles_w * p.tiles_h * p.tiles_n * p.g.num_n_blocks;
@@ -462,11 +322,10 @@ int b200dp_conv_dgrad(const void* dy, const void* w, void* dx, int N, int H, int
   if (((uintptr_t)dy | (uintptr_t)w | (uintptr_t)dx) & 15) return fail("pointers must be 16-byte aligned");
   cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
   const int BN = pick_bn(Cin, block_n);
+  if (BN < 0) return -1;
   ConvMaps maps;
-  ConvParams p;
-  memset(&p, 0, sizeof(p));
-  init_gemm_params(p.g);
-  p.g.N = Cin; p.g.K = Cout; p.g.ldc = Cin; p.g.C = dx; p.g.out_mode = 0; p.g.tma_store = 1;
+  ConvParams p = conv_params();
+  p.g.N = Cin; p.g.ldc = Cin; p.g.C = dx; p.g.out_mode = 0;
   p.g.num_n_blocks = (Cin + BN - 1) / BN;
   p.g.num_k_blocks = (Cout + BLOCK_K - 1) / BLOCK_K;
   p.kc_per_tap = p.g.num_k_blocks;
@@ -474,8 +333,8 @@ int b200dp_conv_dgrad(const void* dy, const void* w, void* dx, int N, int H, int
   p.tiles_w = (s.OW + p.bw - 1) / p.bw; p.tiles_h = (s.OH + p.bh - 1) / p.bh; p.tiles_n = (N + p.bn - 1) / p.bn;
   p.num_taps_total = R * S;
   p.out_w = s.OW; p.out_h = s.OH; p.out_n = N;
-  int sw, sh, sn;
-  slab_box(p.bw, p.bh, p.bn, &sw, &sh, &sn);
+  slab_box(p);
+  const int sn = 32 / (p.sw * p.sh);
   if (make_map4(&maps.a[0], dy, Cout, s.OW, s.OH, N, Cout, (uint64_t)s.OW * Cout, (uint64_t)s.OH * s.OW * Cout,
                 p.bw, p.bh, p.bn))
     return -1;
@@ -490,11 +349,11 @@ int b200dp_conv_dgrad(const void* dy, const void* w, void* dx, int N, int H, int
         ConvTap& t = cl.taps[cl.ntaps++];
         t.amap = 0; t.dh = pad - r; t.dw = pad - c; t.wcol = (r * S + c) * Cin;
       }
-    if (make_map4(&maps.out[0], dx, Cin, W, H, N, Cin, (uint64_t)W * Cin, (uint64_t)H * W * Cin, sw, sh, sn))
+    if (make_map4(&maps.out[0], dx, Cin, W, H, N, Cin, (uint64_t)W * Cin, (uint64_t)H * W * Cin, p.sw, p.sh, sn))
       return -1;
     maps.out[1] = maps.out[2] = maps.out[3] = maps.out[0];
   } else {
-    if (make_parity_maps(maps.out, dx, Cin, W, H, N, sw, sh, sn)) return -1;
+    if (make_parity_maps(maps.out, dx, Cin, W, H, N, p.sw, p.sh, sn)) return -1;
     bool any_empty = false;
     for (int ph = 0; ph < 2; ++ph)
       for (int pw = 0; pw < 2; ++pw) {
@@ -530,11 +389,10 @@ int b200dp_conv_wgrad(const void* dy, const void* x, void* dw_acc, int N, int H,
   if (check_shape(s)) return -1;
   if (((uintptr_t)dy | (uintptr_t)x | (uintptr_t)dw_acc) & 15) return fail("pointers must be 16-byte aligned");
   const int BN = pick_bn(Cin, block_n);
+  if (BN < 0) return -1;
   ConvMaps maps;
-  ConvParams p;
-  memset(&p, 0, sizeof(p));
-  init_gemm_params(p.g);
-  p.g.M = Cout; p.g.N = Cin; p.g.ldc = R * S * Cin; p.g.C = dw_acc; p.g.out_mode = 1; p.g.tma_store = 0;
+  ConvParams p = conv_params();
+  p.g.M = Cout; p.g.N = Cin; p.g.ldc = R * S * Cin; p.g.C = dw_acc; p.g.out_mode = 1;
   p.g.num_m_blocks = (Cout + BLOCK_M - 1) / BLOCK_M;
   p.g.num_n_blocks = (Cin + BN - 1) / BN;
   choose_box(s.OW, s.OH, N, BLOCK_K, &p.bw, &p.bh, &p.bn);     // 64-pixel K blocks
@@ -542,19 +400,7 @@ int b200dp_conv_wgrad(const void* dy, const void* x, void* dw_acc, int N, int H,
   const int kblocks = p.tiles_w * p.tiles_h * p.tiles_n;
   p.num_classes = 1;
   p.num_taps_total = R * S;
-  ConvClass& cl = p.cls[0];
-  for (int r = 0; r < R; ++r)
-    for (int c = 0; c < S; ++c) {
-      ConvTap& t = cl.taps[cl.ntaps++];
-      const int eh = r - pad, ew = c - pad;
-      if (stride == 1) {
-        t.amap = 0; t.dh = eh; t.dw = ew;
-      } else {
-        const int ph = eh & 1, pw = ew & 1;
-        t.amap = ph * 2 + pw; t.dh = floordiv2(eh - ph); t.dw = floordiv2(ew - pw);
-      }
-      t.wcol = (r * S + c) * Cin;
-    }
+  forward_taps(p.cls[0], R, S, Cin, stride, pad);
   const int tiles = p.g.num_m_blocks * p.g.num_n_blocks * R * S;
   if (splits <= 0) {
     splits = g_num_sms / tiles;                          // one wave: never a second, short one
@@ -562,13 +408,7 @@ int b200dp_conv_wgrad(const void* dy, const void* x, void* dw_acc, int N, int H,
     const int max_splits = kblocks / 8 > 1 ? kblocks / 8 : 1;
     if (splits > max_splits) splits = max_splits;
   }
-  if (splits > kblocks) splits = kblocks;
-  if (splits < 1) splits = 1;
-  {  // no empty splits
-    const int per = (kblocks + splits - 1) / splits;
-    splits = (kblocks + per - 1) / per;
-  }
-  p.g.splits = splits;
+  p.g.splits = normalize_splits(splits, kblocks);
   if (stride == 1) {
     if (make_map4(&maps.a[0], x, Cin, W, H, N, Cin, (uint64_t)W * Cin, (uint64_t)H * W * Cin, p.bw, p.bh, p.bn))
       return -1;
@@ -582,18 +422,9 @@ int b200dp_conv_wgrad(const void* dy, const void* x, void* dw_acc, int N, int H,
   maps.out[1] = maps.out[2] = maps.out[3] = maps.out[0];
   maps.b = maps.out[0];   // unused
   cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
-  void* ws = nullptr;
-  if (splits > 1) {
-    p.g.splitk_slice = (long long)Cout * p.g.ldc;
-    cudaError_t e = splitk_alloc(&ws, &p.g, tiles, st);
-    if (e != cudaSuccess) return fail(cudaGetErrorString(e), (int)e);
-  }
-  const int rc = launch_conv<MODE_WGRAD>(maps, p, BN, tiles * splits, max_ctas, st);
-  if (ws != nullptr) {
-    cudaError_t e = cudaFreeAsync(ws, st);
-    if (e != cudaSuccess && rc == 0) return fail(cudaGetErrorString(e), (int)e);
-  }
-  return rc;
+  if (p.g.splits > 1) p.g.splitk_slice = (long long)Cout * p.g.ldc;
+  return run_splitk(p.g, tiles, st,
+                    [&] { return launch_conv<MODE_WGRAD>(maps, p, BN, tiles * p.g.splits, max_ctas, st); });
 }
 
 }  // extern "C"

@@ -1,6 +1,7 @@
-// Shared sm_90a device helpers: mbarrier / TMA / wgmma PTX wrappers, GMMA shared-memory descriptors and the
-// fused accumulator->register->smem->TMA-store epilogue used by the GEMM (gemm_sm90.cu), the implicit-GEMM
-// convolution (conv_sm90.cu) and the attention kernels (attn_sm90.cu).
+// Shared sm_90a device helpers: mbarrier / TMA / wgmma PTX wrappers, GMMA shared-memory descriptors, the
+// fused accumulator->register->smem->TMA-store epilogue and the persistent kernel body of the GEMM
+// (gemm_sm90.cu) and the implicit-GEMM convolution (conv_sm90.cu), and their host side (tensor maps,
+// launches, split-K workspaces), partly shared with the attention kernels (attn_sm90.cu).
 //
 // wgmma keeps its accumulator in the registers of the issuing warpgroup, in a fragment layout (each warp
 // holds 16 rows, each thread two rows x pairs of columns).  The epilogues work on one accumulator ROW per
@@ -12,6 +13,7 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <stdio.h>
 
 namespace {
 
@@ -23,18 +25,18 @@ constexpr int EPI_WARPS = 8;
 constexpr int SMEM_LIMIT = 232448;   // 227 KB of dynamic shared memory per block on sm_90
 
 struct GemmParams {
-  int M, N, K;
+  int M, N;
   int ldc;                 // elements
   int num_m_blocks, num_n_blocks, num_k_blocks;
   int splits;              // split-K factor (>=1)
   int act;                 // 0 none, 1 relu, 2 gelu(erf), 3 *gelu'(aux), 4 *(aux>0)  [aux = residual ptr]
-  int out_mode;            // 0: bf16 store, 1: fp32 add into C (split-K: see splitk_finish_tile), 2: fp32 store
+  int out_mode;            // 0: bf16 via swizzled smem + TMA bulk store, 1: fp32 add into C (split-K: see
+                           // splitk_finish_tile), 2: fp32 store
   void* C;
   const void* bias;        // bf16 [N] or nullptr
   const void* bias_f32;    // fp32 [N] or nullptr
   const void* residual;    // bf16 [M, ldc] or nullptr (added after act; or `aux` for act 3/4)
   void* preact;            // optional bf16 [M, ldc]: pre-activation values (saved for backward)
-  int tma_store;           // out_mode 0: stage the tile in swizzled smem and write it with TMA bulk stores
   int n_fastest;           // tile order: consecutive CTAs walk the N blocks of one M block first (A tile is
                            // fetched from HBM once and re-used from L2 while the whole B matrix stays in L2)
   float alpha;
@@ -381,15 +383,14 @@ template <int BN>
 __device__ __forceinline__ void epilogue_rows(const GemmParams& p, const CUtensorMap* map_c,
                                               const CUtensorMap* map_z, uint32_t acc_img, int acc, int q,
                                               int lane, int m_row0, int n_idx, int c_begin, int c_end,
-                                              uint8_t* my_store, const StoreAt at = StoreAt{0, 0, 0, 0, nullptr, 32, 1, 32, 1, 1},
-                                              float* s_stats = nullptr) {
+                                              uint8_t* my_store, const StoreAt at, float* s_stats) {
   // A 64-column chunk (one 128-byte bf16 row per lane, one TMA store box) is produced in two 32-column
   // halves: 32 accumulator values + 32 results live per thread instead of 64 + 64 — the previous
   // single-pass version spilled ~300 B per thread at the 168-register budget of a 320-thread CTA, and the
   // epilogue, not the MMA, bounds every K <= 512 GEMM / convolution here.
   const int row = m_row0 + lane;
   const bool row_ok = row < p.M;
-  const bool to_tma = p.out_mode == 0 && p.tma_store;
+  const bool to_tma = p.out_mode == 0;
   const bool z_tma = p.preact != nullptr && to_tma;
   const bool res_smem = p.residual != nullptr && p.preact == nullptr && p.out_mode != 1;
   // the common case (plain bf16 output, optionally with BN statistics): no per-element work at all
@@ -612,19 +613,12 @@ __device__ __forceinline__ void epilogue_rows(const GemmParams& p, const CUtenso
           }
         }
         __syncwarp();
-      } else if (row_ok) {
-        if (p.out_mode == 0) {
-          uint4* dst = reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.C) + (size_t)row * p.ldc + col0 + hc);
+      } else if (row_ok) {   // out_mode 2: fp32 store
+        float* dst = reinterpret_cast<float*>(at.c_ptr ? at.c_ptr : p.C) + (size_t)row * p.ldc + col0 + hc;
 #pragma unroll
-          for (int j = 0; j < 4; ++j)
-            if (j * 8 < hcols) dst[j] = pack8(v + j * 8);
-        } else {   // out_mode 2: fp32 store
-          float* dst = reinterpret_cast<float*>(at.c_ptr ? at.c_ptr : p.C) + (size_t)row * p.ldc + col0 + hc;
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            if (j * 4 < hcols)
-              reinterpret_cast<float4*>(dst)[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-        }
+        for (int j = 0; j < 8; ++j)
+          if (j * 4 < hcols)
+            reinterpret_cast<float4*>(dst)[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
       }
     }
     }
@@ -787,16 +781,136 @@ __device__ __forceinline__ void stats_flush(const GemmParams& p, float* s_stats,
   asm volatile("bar.sync 2, 256;" ::: "memory");
 }
 
-// Split-K workspace for one launch, stream-ordered on the launch stream (so concurrent launches never share
-// one; freed with cudaFreeAsync on the same stream after the launch): the fp32 slices and the zeroed per-tile
-// arrival counters of splitk_finish_tile.
-inline cudaError_t splitk_alloc(void** ws, GemmParams* p, int tiles, cudaStream_t st) {
-  const size_t slices = (size_t)p->splits * (size_t)p->splitk_slice * sizeof(float);
-  cudaError_t e = cudaMallocAsync(ws, slices + (size_t)tiles * sizeof(int), st);
-  if (e != cudaSuccess) return e;
-  p->splitk_ws = reinterpret_cast<float*>(*ws);
-  p->splitk_count = reinterpret_cast<int*>(reinterpret_cast<char*>(*ws) + slices);
-  return cudaMemsetAsync(p->splitk_count, 0, (size_t)tiles * sizeof(int), st);
+// ------------------------------------------------------------------ persistent GEMM / convolution body
+// Persistent, warp-specialised, one CTA per SM, NUM_THREADS threads:
+//   warpgroup 0    : TMA producer (one thread) filling the STAGES-deep operand ring
+//   warpgroups 1-2 : 64 rows of the 128 x BN tile each (wg_mainloop); then all 8 warps run the epilogue
+//                    (epilogue_rows), two warps per 32-row slab, each taking half of the columns.  The
+//                    producer keeps filling the ring during the epilogue.
+// CTA b takes work items b, b + gridDim.x, ...; an item is one output tile, or one split of it.  What the
+// items are is the kernel's Work description:
+//   items             number of work items
+//   kStats, kSplitK   whether the kernel can produce BN statistics / split-K partials at all
+//   prefetch()        prefetches the tensor maps the kernel reads
+//   num_kb(w)         64-deep K blocks of item w
+//   load(w, next)     issues the TMA loads of item w: for each K block, `const Stage s = next()` waits for a
+//                     free stage and arms its barrier for STAGE_BYTES; the A / B tiles go to s.a / s.b on s.bar
+//   slab(w, q)        where rows 32q..32q+31 of item w's tile go
+// Work holds POINTERS to the kernel's __grid_constant__ tensor maps: TMA reads a map from parameter,
+// constant or global memory, never from a local copy.
+struct Stage {
+  uint8_t* a;
+  uint8_t* b;
+  uint64_t* bar;
+};
+struct Slab {
+  const CUtensorMap* map_c;   // out_mode 0: output and pre-activation store maps
+  const CUtensorMap* map_z;
+  int m_row0, n_idx;          // first row of the slab in a row-major output (rank-2 StoreAt), first column
+  StoreAt at;
+  int tile, m_idx;            // split-K: arrival counter and first row of the output tile,
+  long long c_off;            // and its column offset in C and in each workspace slice
+};
+
+template <int BN, bool A_MN, bool B_MN, class Work>
+__device__ __forceinline__ void persistent_body(const Work& wk, const GemmParams& p) {
+  using C = Cfg<BN>;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
+                                             ~static_cast<uintptr_t>(1023));
+  uint8_t* smem_a = smem;
+  uint8_t* smem_b = smem + C::STAGES * C::A_BYTES;
+  uint8_t* smem_store = smem + C::STAGES * C::STAGE_BYTES;   // 1024B-aligned staging for TMA stores
+  uint8_t* smem_acc = smem_store + C::STORE_BYTES;           // accumulator image [128][BN + 4] fp32
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_acc + C::ACC_BYTES);
+  uint64_t* full_bar = bars;                     // [STAGES]
+  uint64_t* empty_bar = bars + C::STAGES;        // [STAGES]
+  float* s_stats = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 256);
+  const bool want_stats = Work::kStats && p.stats != nullptr && p.out_mode == 0;
+  if (want_stats) stats_zero(s_stats, NUM_THREADS, p.N);
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+
+  if (warp == 0 && lane == 0) {
+    wk.prefetch();
+    for (int i = 0; i < C::STAGES; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 2);               // one arrival per consumer warpgroup
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  if (warp < 4) {
+    // ============================ TMA producer ============================
+    if (warp == 0 && lane == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      auto next = [&]() {
+        mbar_wait(&empty_bar[stage], phase ^ 1);
+        mbar_expect_tx(&full_bar[stage], C::STAGE_BYTES);
+        const Stage s{smem_a + stage * C::A_BYTES, smem_b + stage * C::B_BYTES, &full_bar[stage]};
+        if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+        return s;
+      };
+      for (int w = blockIdx.x; w < wk.items; w += gridDim.x) wk.load(w, next);
+    }
+  } else {
+    // ============================ wgmma + epilogue (warpgroups 1-2) ============================
+    const int cw = warp - 4;                      // consumer warp 0..7
+    const int wg = cw >> 2;                       // rows 64*wg .. 64*wg+63 of the tile
+    const int q = cw & 3;                         // 32-row slab this warp drains
+    const int half = cw >> 2;                     // which half of the columns this warp drains
+    const int c_begin = (BN >= 128) ? half * (BN / 2) : 0;
+    const int c_end = (BN >= 128) ? c_begin + BN / 2 : (half == 0 ? BN : 0);
+    const int epi_tid = cw * 32 + lane;
+    uint8_t* my_store = smem_store + cw * (2 * 4096);
+    float* my_stats = s_stats + cw * STATS_WARP_FLOATS;
+    const uint32_t img = smem_u32(smem_acc);
+    __shared__ int s_last;
+    int stats_n = -1;                             // column block the shared statistics belong to
+    int stage = 0, acc = 0;
+    uint32_t phase = 0;
+    float d[BN / 2];
+    for (int w = blockIdx.x; w < wk.items; w += gridDim.x) {
+      // where the tile goes is worked out while the first operand stage is still in flight, not after the MMAs
+      const Slab s = wk.slab(w, q);
+      wg_mainloop<BN, A_MN, B_MN, C::STAGES, C::A_BYTES, C::B_BYTES>(d, smem_u32(smem_a), smem_u32(smem_b), full_bar,
+                                                                     empty_bar, stage, phase, wk.num_kb(w), wg);
+      if (want_stats && s.n_idx != stats_n) {
+        if (stats_n >= 0) stats_flush<BN>(p, s_stats, stats_n, epi_tid);
+        stats_n = s.n_idx;
+      }
+      named_bar(1, 256);                          // the previous tile's image has been read
+      acc_to_smem<BN>(d, img, BN + 4, wg * 64);
+      named_bar(1, 256);
+      epilogue_rows<BN>(p, s.map_c, s.map_z, img, acc, q, lane, s.m_row0, s.n_idx, c_begin, c_end, my_store, s.at,
+                        want_stats ? my_stats : nullptr);
+      if (Work::kSplitK && p.splits > 1) {
+        const Slab t = wk.slab(w, q);             // recomputed: keeping s live across the epilogue costs spills
+        splitk_finish_tile(p, t.tile, t.m_idx, t.n_idx, BN, t.c_off, epi_tid, &s_last);
+      }
+      acc ^= 1;
+    }
+    if (want_stats && stats_n >= 0) stats_flush<BN>(p, s_stats, stats_n, epi_tid);
+    if (want_stats) stats_finalize(p, epi_tid);
+    if (p.out_mode == 0 && lane == 0) tma_store_wait_all();   // smem must outlive the bulk reads
+  }
+}
+
+// ------------------------------------------------------------------ host side
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
+                                  CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
+                                  CUtensorMapFloatOOBfill);
+EncodeTiledFn g_encode = nullptr;
+thread_local char g_err[512];    // one per source file: its b200dp_*_last_error
+int g_num_sms = 0;
+
+int fail(const char* msg, int code = 0) {
+  snprintf(g_err, sizeof(g_err), "%s (%d)", msg, code);
+  return -1;
 }
 
 // cuTensorMapEncode* is a driver-API call: it fails with CUDA_ERROR_INVALID_CONTEXT on a thread that
@@ -807,6 +921,109 @@ inline void bind_primary_context() {
     cudaFree(nullptr);
     bound = true;
   }
+}
+
+int ensure_init() {
+  bind_primary_context();
+  if (g_encode) return 0;
+  void* fn = nullptr;
+  cudaDriverEntryPointQueryResult st;
+  cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &st);
+  if (e != cudaSuccess || st != cudaDriverEntryPointSuccess || !fn)
+    return fail("cuTensorMapEncodeTiled entry point unavailable", (int)e);
+  g_encode = reinterpret_cast<EncodeTiledFn>(fn);
+  int dev = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
+  return 0;
+}
+
+// bf16 tensor map of `rank` dimensions, 128B swizzle: dims[0] is contiguous, byte_strides[i] is the pitch of
+// dims[i + 1], out-of-bounds elements read as zero.
+int encode_map(CUtensorMap* m, const void* ptr, int rank, const cuuint64_t* dims, const cuuint64_t* byte_strides,
+               const cuuint32_t* box) {
+  const cuuint32_t estr[4] = {1, 1, 1, 1};
+  CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(ptr), dims, byte_strides, box,
+                        estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                        CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled failed", (int)r);
+  return 0;
+}
+
+// 2D bf16 map: `rows` x `cols` (cols contiguous), row pitch `ld` elements, box {64, box_rows}
+// (the same encoding serves the operand loads and the 32-row bulk stores)
+int make_map2(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows) {
+  const cuuint64_t dims[2] = {cols, rows};
+  const cuuint64_t strides[1] = {ld * 2};
+  const cuuint32_t box[2] = {64, box_rows};
+  return encode_map(m, ptr, 2, dims, strides, box);
+}
+
+// sets Kernel's dynamic shared memory limit on its first launch
+template <auto Kernel>
+int smem_attr_once(int bytes) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e != cudaSuccess) return fail(cudaGetErrorString(e), (int)e);
+    attr_set = true;
+  }
+  return 0;
+}
+
+// A persistent_body kernel over `work` items: one CTA per SM at most, fewer with max_ctas > 0, and never more
+// than the BN statistics have slots for.
+template <auto Kernel, int BN, class... Args>
+int launch_persistent(int work, int max_ctas, cudaStream_t st, const Args&... args) {
+  if (smem_attr_once<Kernel>(Cfg<BN>::SMEM_BYTES)) return -1;
+  int grid = work < g_num_sms ? work : g_num_sms;
+  if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
+  if (grid > STATS_MAX_CTAS) grid = STATS_MAX_CTAS;
+  Kernel<<<grid, NUM_THREADS, Cfg<BN>::SMEM_BYTES, st>>>(args...);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(cudaGetErrorString(e), (int)e);
+  return 0;
+}
+
+// Runs launch() with a split-K workspace (p.splits > 1) for `tiles` output tiles of p.splitk_slice elements,
+// stream-ordered on the launch stream so that concurrent launches never share one: the fp32 slices and the
+// zeroed per-tile arrival counters of splitk_finish_tile, freed with cudaFreeAsync after the launch.
+template <class Launch>
+int run_splitk(GemmParams& p, int tiles, cudaStream_t st, Launch&& launch) {
+  void* ws = nullptr;
+  if (p.splits > 1) {
+    const size_t slices = (size_t)p.splits * (size_t)p.splitk_slice * sizeof(float);
+    cudaError_t e = cudaMallocAsync(&ws, slices + (size_t)tiles * sizeof(int), st);
+    if (e == cudaSuccess) {
+      p.splitk_ws = reinterpret_cast<float*>(ws);
+      p.splitk_count = reinterpret_cast<int*>(reinterpret_cast<char*>(ws) + slices);
+      e = cudaMemsetAsync(p.splitk_count, 0, (size_t)tiles * sizeof(int), st);
+    }
+    if (e != cudaSuccess) return fail(cudaGetErrorString(e), (int)e);
+  }
+  const int rc = launch();
+  if (ws != nullptr) {
+    cudaError_t e = cudaFreeAsync(ws, st);
+    if (e != cudaSuccess && rc == 0) return fail(cudaGetErrorString(e), (int)e);
+  }
+  return rc;
+}
+
+// K splits over kblocks K blocks, clamped to 1..kblocks and reduced until no split is empty
+int normalize_splits(int splits, int kblocks) {
+  if (splits > kblocks) splits = kblocks;
+  if (splits < 1) splits = 1;
+  const int per = (kblocks + splits - 1) / splits;
+  return (kblocks + per - 1) / per;
+}
+
+// tile width: 0 picks 64 or 128 from the output width n; 256 runs as 128, the widest tile whose accumulator
+// image fits in shared memory next to the operand ring
+int pick_bn(int n, int block_n) {
+  if (block_n == 0) return n > 64 ? 128 : 64;
+  if (block_n == 256) return 128;
+  if (block_n != 64 && block_n != 128) return fail("block_n must be 64/128/256");
+  return block_n;
 }
 
 }  // namespace
