@@ -156,7 +156,7 @@ struct ConvWork {
       at.c_ptr = nullptr;
       at.sw = p.sw; at.sh = p.sh;
       at.vw = p.out_w - at.w; at.vh = p.out_h - at.h; at.vn = p.out_n - at.n;
-      return Slab{&maps.out[p.cls[rest / pix_tiles].out_map], nullptr, 0, nt * BN, at, 0, 0, 0};
+      return Slab{&maps.out[p.cls[rest / pix_tiles].out_map], 0, nt * BN, at, 0, 0, 0};
     }
     const int tile = w % tiles;
     const ConvTap tap = p.cls[0].taps[tile % p.num_taps_total];
@@ -164,7 +164,7 @@ struct ConvWork {
     const int m_idx = (mn / nnb) * BLOCK_M;
     float* c_ptr = (p.g.splits > 1 ? p.g.splitk_ws + (long long)(w / tiles) * p.g.splitk_slice
                                    : reinterpret_cast<float*>(p.g.C)) + tap.wcol;
-    return Slab{nullptr, nullptr, m_idx + q * 32, (mn % nnb) * BN, StoreAt{0, 0, 0, 0, c_ptr, 32, 1, 32, 1, 1},
+    return Slab{nullptr, m_idx + q * 32, (mn % nnb) * BN, StoreAt{0, 0, 0, 0, c_ptr, 32, 1, 32, 1, 1},
                 tile, m_idx, tap.wcol};
   }
 };

@@ -24,19 +24,17 @@ namespace {
 template <int BN, bool A_MN, bool B_MN>
 struct GemmWork {
   static constexpr bool kStats = true, kSplitK = true;
-  const CUtensorMap *a, *b, *c, *z;
+  const CUtensorMap *a, *b, *c;
   const GemmParams& p;
   int tiles, items, kb_per_split;
 
-  __device__ GemmWork(const CUtensorMap* a_, const CUtensorMap* b_, const CUtensorMap* c_, const CUtensorMap* z_,
-                      const GemmParams& p_)
-      : a(a_), b(b_), c(c_), z(z_), p(p_), tiles(p_.num_m_blocks * p_.num_n_blocks), items(tiles * p_.splits),
+  __device__ GemmWork(const CUtensorMap* a_, const CUtensorMap* b_, const CUtensorMap* c_, const GemmParams& p_)
+      : a(a_), b(b_), c(c_), p(p_), tiles(p_.num_m_blocks * p_.num_n_blocks), items(tiles * p_.splits),
         kb_per_split((p_.num_k_blocks + p_.splits - 1) / p_.splits) {}
   __device__ void prefetch() const {
     tma_prefetch_desc(a);
     tma_prefetch_desc(b);
     if (p.out_mode == 0) tma_prefetch_desc(c);
-    if (p.out_mode == 0 && p.preact != nullptr) tma_prefetch_desc(z);
   }
   __device__ int m_idx(int tile) const {
     return (p.n_fastest ? tile / p.num_n_blocks : tile % p.num_m_blocks) * BLOCK_M;
@@ -74,7 +72,7 @@ struct GemmWork {
   __device__ Slab slab(int w, int q) const {
     const int tile = w % tiles, split = w / tiles;
     const int m0 = m_idx(tile);
-    return Slab{c, z, m0 + q * 32, n_idx(tile),
+    return Slab{c, m0 + q * 32, n_idx(tile),
                 StoreAt{0, 0, 0, 0, p.splits > 1 ? p.splitk_ws + (long long)split * p.splitk_slice : nullptr},
                 tile, m0, 0};
   }
@@ -83,16 +81,15 @@ struct GemmWork {
 template <int BN, bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                 const __grid_constant__ CUtensorMap map_c, const __grid_constant__ CUtensorMap map_z,
-                 const __grid_constant__ GemmParams p) {
-  persistent_body<BN, A_MN, B_MN>(GemmWork<BN, A_MN, B_MN>(&map_a, &map_b, &map_c, &map_z, p), p);
+                 const __grid_constant__ CUtensorMap map_c, const __grid_constant__ GemmParams p) {
+  persistent_body<BN, A_MN, B_MN>(GemmWork<BN, A_MN, B_MN>(&map_a, &map_b, &map_c, p), p);
 }
 
 int launch_bn(int BN, int a_mn, int b_mn, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mc,
-              const CUtensorMap& mz, const GemmParams& p, int max_ctas, cudaStream_t st) {
+              const GemmParams& p, int max_ctas, cudaStream_t st) {
   const int work = p.num_m_blocks * p.num_n_blocks * p.splits;
 #define LAUNCH(BNV, AMN, BMN) \
-  launch_persistent<gemm_bf16_kernel<BNV, AMN, BMN>, BNV>(work, max_ctas, st, ma, mb, mc, mz, p)
+  launch_persistent<gemm_bf16_kernel<BNV, AMN, BMN>, BNV>(work, max_ctas, st, ma, mb, mc, p)
 #define DISPATCH(BNV)                                          \
   if (BN == BNV) {                                             \
     if (!a_mn && !b_mn) return LAUNCH(BNV, false, false);      \
@@ -146,7 +143,7 @@ int b200dp_gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K,
   if (stats != nullptr && (N > STATS_MAX_N || out_mode != 0)) return fail("stats: N <= 2048 and bf16 output required");
   // B (N x K bf16) small enough to live in the 50 MB L2 next to the in-flight A tiles -> walk N first
   p.n_fastest = ((size_t)N * (size_t)K * 2 <= ((size_t)20 << 20)) ? 1 : 0;
-  CUtensorMap ma, mb, mc, mz;
+  CUtensorMap ma, mb, mc;
   if (a_mn ? make_map2(&ma, A, K, M, lda, BLOCK_K) : make_map2(&ma, A, M, K, lda, BLOCK_M)) return -1;
   if (b_mn ? make_map2(&mb, B, K, N, ldb, BLOCK_K) : make_map2(&mb, B, N, K, ldb, BN)) return -1;
   if (out_mode == 0) {
@@ -154,15 +151,10 @@ int b200dp_gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K,
   } else {
     mc = ma;   // unused
   }
-  if (out_mode == 0 && preact != nullptr) {
-    if (make_map2(&mz, preact, M, N, ldc, 32)) return -1;
-  } else {
-    mz = mc;   // unused
-  }
   cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
   if (p.splits > 1) p.splitk_slice = (long long)M * ldc;
   return run_splitk(p, p.num_m_blocks * p.num_n_blocks, st,
-                    [&] { return launch_bn(BN, a_mn, b_mn, ma, mb, mc, mz, p, max_ctas, st); });
+                    [&] { return launch_bn(BN, a_mn, b_mn, ma, mb, mc, p, max_ctas, st); });
 }
 
 }  // extern "C"

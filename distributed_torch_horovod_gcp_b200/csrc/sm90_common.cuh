@@ -1,13 +1,14 @@
 // Shared sm_90a device helpers: mbarrier / TMA / wgmma PTX wrappers, GMMA shared-memory descriptors, the
-// fused accumulator->register->smem->TMA-store epilogue and the persistent kernel body of the GEMM
-// (gemm_sm90.cu) and the implicit-GEMM convolution (conv_sm90.cu), and their host side (tensor maps,
-// launches, split-K workspaces), partly shared with the attention kernels (attn_sm90.cu).
+// fused register->smem->TMA-store epilogue and the persistent kernel body of the GEMM (gemm_sm90.cu) and
+// the implicit-GEMM convolution (conv_sm90.cu), and their host side (tensor maps, launches, split-K
+// workspaces), partly shared with the attention kernels (attn_sm90.cu).
 //
 // wgmma keeps its accumulator in the registers of the issuing warpgroup, in a fragment layout (each warp
-// holds 16 rows, each thread two rows x pairs of columns).  The epilogues work on one accumulator ROW per
-// lane, so a finished tile is written once to a row-major fp32 image in shared memory ("accumulator
-// image", row pitch = columns + 4 floats: conflict-free 16-byte reads of one row per lane) and the
-// epilogue warps read 32-column runs of their rows from it.
+// holds 16 rows, each thread two rows x pairs of columns).  The epilogue works on that fragment: each
+// thread applies it to its own elements and writes bf16 pairs into a 128B-swizzled staging copy of the
+// whole tile (or fp32 pairs to global memory).  After a barrier, each warp bulk-stores one 32-row x
+// 64-column box of it and walks its columns for the BatchNorm statistics.  No fp32 copy of the tile goes
+// through shared memory, so the space goes to the operand ring instead.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -21,7 +22,6 @@ constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;          // 64 bf16 = 128 bytes = one 128B swizzle atom
 constexpr int WGMMA_K = 16;        // K of one wgmma (bf16)
 constexpr int NUM_THREADS = 384;     // warpgroup 0: TMA producer; warpgroups 1-2: wgmma + epilogue (8 warps)
-constexpr int EPI_WARPS = 8;
 constexpr int SMEM_LIMIT = 232448;   // 227 KB of dynamic shared memory per block on sm_90
 
 struct GemmParams {
@@ -182,29 +182,6 @@ __device__ __forceinline__ void wgmma_tf32_n32(float* d, uint64_t a, uint64_t b,
 }
 
 
-// m64 x N accumulator fragment of this thread's warpgroup -> rows row0.. of a row-major fp32 image
-template <int N>
-__device__ __forceinline__ void acc_to_smem(const float* d, uint32_t img, int ld, int row0) {
-  const int t = threadIdx.x & 127;
-  const int r = row0 + (t >> 5) * 16 + ((t & 31) >> 2);
-  const uint32_t p0 = img + (uint32_t)((r * ld + 2 * (t & 3)) * 4);
-  const uint32_t p1 = p0 + (uint32_t)(8 * ld * 4);
-#pragma unroll
-  for (int j = 0; j < N / 8; ++j) {
-    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(p0 + j * 32), "f"(d[4 * j]), "f"(d[4 * j + 1]) : "memory");
-    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(p1 + j * 32), "f"(d[4 * j + 2]), "f"(d[4 * j + 3]) : "memory");
-  }
-}
-// 32 consecutive fp32 of one image row (bit patterns)
-__device__ __forceinline__ void acc_ld32(uint32_t addr, uint32_t* r) {
-#pragma unroll
-  for (int i = 0; i < 8; ++i)
-    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];"
-                 : "=r"(r[4 * i]), "=r"(r[4 * i + 1]), "=r"(r[4 * i + 2]), "=r"(r[4 * i + 3])
-                 : "r"(addr + 16 * i)
-                 : "memory");
-}
-
 // 64-bit GMMA shared-memory descriptor, 128B swizzle.
 //   K-major  : rows of 128 B (64 bf16 of K), 8-row groups 1024 B apart (SBO); LBO unused (=1).
 //   MN-major : [k rows][64 mn elements] atoms of 128 B rows; 8-row k-groups SBO=1024 B apart,
@@ -313,38 +290,28 @@ __device__ __forceinline__ void unpack8(const uint4& x, float* f) {
   }
 }
 
-__device__ __forceinline__ uint4 pack8(const float* v) {
-  uint32_t wv[4];
-#pragma unroll
-  for (int t = 0; t < 4; ++t) {
-    __nv_bfloat162 h = __floats2bfloat162_rn(v[2 * t], v[2 * t + 1]);
-    wv[t] = *reinterpret_cast<uint32_t*>(&h);
-  }
-  return make_uint4(wv[0], wv[1], wv[2], wv[3]);
-}
-
 template <int BN>
 struct Cfg {
   static constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;
   static constexpr int B_BYTES = BN * BLOCK_K * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int ACC_LD = BN + 4;          // accumulator image row pitch (floats)
-  static constexpr int ACC_BYTES = BLOCK_M * ACC_LD * 4;
-  static constexpr int STORE_BYTES = EPI_WARPS * 2 * 4096;   // per epilogue warp: out + preact staging (32 rows x 128 B each)
-  static constexpr int FIXED_BYTES = STORE_BYTES + ACC_BYTES + 1024 /*align*/ + 256 /*barriers*/ + STATS_SMEM_BYTES;
-  // as many operand stages as fit next to the accumulator image (BN 64: 4, BN 128: 2)
-  static constexpr int STAGES = (SMEM_LIMIT - FIXED_BYTES) / STAGE_BYTES > 4 ? 4 : (SMEM_LIMIT - FIXED_BYTES) / STAGE_BYTES;
+  // bf16 staging of one whole output tile: [4 slabs][BN / 64 chunks] boxes of 32 rows x 128 B (128B-swizzled),
+  // one bulk store each
+  static constexpr int NCH = BN / 64;
+  static constexpr int STORE_BYTES = BLOCK_M * BN * 2;
+  static constexpr int FIXED_BYTES = STORE_BYTES + 1024 /*align*/ + 256 /*barriers*/ + STATS_SMEM_BYTES;
+  // as many operand stages as fit next to the staging tile: BN 64: 8, BN 128: 5 (measured on an H100, a
+  // 4-stage cap for BN 64 gained nothing)
+  static constexpr int STAGES = (SMEM_LIMIT - FIXED_BYTES) / STAGE_BYTES;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + FIXED_BYTES;
-  static_assert(STAGES >= 2, "shared memory");
+  static_assert(STAGES >= 4, "shared memory");
+  static_assert(2 * STAGES * 8 <= 256, "barrier space");
 };
 
-// Epilogue of one 32-row slab (rows 32q..32q+31) of a 128 x BN accumulator: accumulator image ->
-// registers -> alpha/bias/activation/residual -> bf16 via swizzled smem + TMA bulk store, or fp32
-// store / add (one partial per element without split-K; with split-K a store into the split's
-// workspace slice).
-// Where a 32-row slab goes.  rank4 == 0: rows m_row0.. of the row-major [M, ldc] matrix (2D map).
-// rank4 == 1 (convolution): the slab is the {64 c, sw, sh, sn} sub-box at pixel (w, h, n) of an NHWC
-// tensor; c_ptr/ld override p.C/p.ldc for the fp32 modes (per-tap column offset of the wgrad output).
+// Where the rows of a tile go.  rank4 == 0: rows m_row0.. of the row-major [M, ldc] matrix (2D map).
+// rank4 == 1 (convolution): a 32-row slab is the {64 c, sw, sh, sn} sub-box at pixel (w, h, n) of an NHWC
+// tensor.  c_ptr overrides p.C for the fp32 modes (split-K workspace slice, per-tap column offset of the
+// wgrad output).
 struct StoreAt {
   int rank4, w, h, n;
   void* c_ptr;
@@ -359,9 +326,12 @@ struct StoreAt {
 __device__ __forceinline__ void epi_sts128(uint32_t addr, const uint4& v) {
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
 }
-__device__ __forceinline__ uint4 epi_lds128(uint32_t addr) {
-  uint4 v;
-  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+__device__ __forceinline__ void epi_sts32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ uint32_t epi_lds32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
   return v;
 }
 // prmt.b32 in its default mode: selector nibble bit 3 = replicate the selected byte's sign bit
@@ -370,319 +340,230 @@ __device__ __forceinline__ uint32_t prmt_sign(uint32_t a, uint32_t sel) {
   asm("prmt.b32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(0u), "r"(sel));
   return d;
 }
-__device__ __forceinline__ uint4 pack8r(const uint32_t* r) {   // 8 fp32 bit patterns -> 8 bf16
-  uint4 o;
-  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(o.x) : "f"(__uint_as_float(r[1])), "f"(__uint_as_float(r[0])));
-  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(o.y) : "f"(__uint_as_float(r[3])), "f"(__uint_as_float(r[2])));
-  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(o.z) : "f"(__uint_as_float(r[5])), "f"(__uint_as_float(r[4])));
-  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(o.w) : "f"(__uint_as_float(r[7])), "f"(__uint_as_float(r[6])));
+__device__ __forceinline__ uint32_t cvt_bf16x2(float lo, float hi) {
+  uint32_t o;
+  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(o) : "f"(hi), "f"(lo));
   return o;
 }
 
+// Byte offset of (tile row r, 16-byte column unit u) in the staging tile: box (r / 32, u / 8), row r % 32, and
+// unit u % 8 at its 128B-swizzle position (u ^ r) % 8 — the shared-memory image the bulk stores read.
 template <int BN>
-__device__ __forceinline__ void epilogue_rows(const GemmParams& p, const CUtensorMap* map_c,
-                                              const CUtensorMap* map_z, uint32_t acc_img, int acc, int q,
-                                              int lane, int m_row0, int n_idx, int c_begin, int c_end,
-                                              uint8_t* my_store, const StoreAt at, float* s_stats) {
-  // A 64-column chunk (one 128-byte bf16 row per lane, one TMA store box) is produced in two 32-column
-  // halves: 32 accumulator values + 32 results live per thread instead of 64 + 64 — the previous
-  // single-pass version spilled ~300 B per thread at the 168-register budget of a 320-thread CTA, and the
-  // epilogue, not the MMA, bounds every K <= 512 GEMM / convolution here.
-  const int row = m_row0 + lane;
-  const bool row_ok = row < p.M;
-  const bool to_tma = p.out_mode == 0;
-  const bool z_tma = p.preact != nullptr && to_tma;
-  const bool res_smem = p.residual != nullptr && p.preact == nullptr && p.out_mode != 1;
-  // the common case (plain bf16 output, optionally with BN statistics): no per-element work at all
-  const bool plain = to_tma && p.alpha == 1.0f && p.bias == nullptr && p.bias_f32 == nullptr &&
+__device__ __forceinline__ uint32_t stage_off(int r, int u) {
+  return (uint32_t)((((r >> 5) * (BN / 64) + (u >> 3)) << 12) + ((r & 31) << 7) + (((u ^ r) & 7) << 4));
+}
+
+// Residual of the 16 tile rows r0.. that this warp holds in its fragment (rows m0 + r0.. of the [M, ldc]
+// matrix): COALESCED 16-byte loads, zero past M and past N, then staged at the output's place in the staging
+// tile (res_stage) so that each thread reads its elements back in fragment layout.
+template <int BN>
+__device__ __forceinline__ void res_load(const GemmParams& p, uint4* rv, int m0, int r0, int n_idx, int lane) {
+  const __nv_bfloat16* rbase = reinterpret_cast<const __nv_bfloat16*>(p.residual);
+#pragma unroll
+  for (int i = 0; i < BN / 16; ++i) {
+    const int e = i * 32 + lane, row = m0 + r0 + e / (BN / 8), col = n_idx + (e % (BN / 8)) * 8;
+    rv[i] = (row < p.M && col < p.N) ? *reinterpret_cast<const uint4*>(rbase + (size_t)row * p.ldc + col)
+                                     : make_uint4(0, 0, 0, 0);
+  }
+  if (p.res_mask != nullptr) {
+    // ReLU sign bits of the residual (1 byte per 8 channels): bit j -> 16-bit lane j.  Byte k of
+    // ((bits * 0x01010101) & 0x08040201) + 0x7f7f7f7f has its MSB set iff bit k is, and PRMT's
+    // sign-replicate mode turns that MSB into 0x00 / 0xff bytes.
+    uint32_t mbits[BN / 16];
+#pragma unroll
+    for (int i = 0; i < BN / 16; ++i) {
+      const int e = i * 32 + lane, row = m0 + r0 + e / (BN / 8), col = n_idx + (e % (BN / 8)) * 8;
+      mbits[i] = (row < p.M && col < p.N) ? (uint32_t)p.res_mask[(size_t)row * (size_t)(p.N >> 3) + (size_t)(col >> 3)]
+                                          : 0u;
+    }
+#pragma unroll
+    for (int i = 0; i < BN / 16; ++i) {
+      const uint32_t rep = mbits[i] * 0x01010101u;
+      const uint32_t lo = (rep & 0x08040201u) + 0x7f7f7f7fu, hi = (rep & 0x80402010u) + 0x7f7f7f7fu;
+      rv[i].x &= prmt_sign(lo, 0x9988u);
+      rv[i].y &= prmt_sign(lo, 0xbbaau);
+      rv[i].z &= prmt_sign(hi, 0x9988u);
+      rv[i].w &= prmt_sign(hi, 0xbbaau);
+    }
+  }
+}
+template <int BN>
+__device__ __forceinline__ void res_stage(const uint4* rv, uint32_t stg, int r0, int lane) {
+#pragma unroll
+  for (int i = 0; i < BN / 16; ++i) {
+    const int e = i * 32 + lane;
+    epi_sts128(stg + stage_off<BN>(r0 + e / (BN / 8), e % (BN / 8)), rv[i]);
+  }
+}
+
+// Epilogue of this thread's part of a finished 128 x BN tile, straight from the wgmma fragment d of
+// warpgroup wg — tile rows r and r + 8 (r = 64 wg + 16 warp + lane / 4), columns 8j + 2 (lane % 4) + {0, 1}:
+// alpha, bias, pre-activation, activation, residual; then bf16 pairs into the staging tile (out_mode 0: the 8
+// rows of a warp store hit 8 different swizzle positions, so the 4-byte stores are conflict-free), fp32
+// pairs added into C (out_mode 1; with split-K stored into the split's workspace slice, cbase) or stored
+// (out_mode 2).  m0: first row of the tile in the [M, ldc] matrix.  A residual (out_mode != 1) has been
+// staged at the output's place; every element is read and then overwritten by the one thread that owns it.
+template <int BN>
+__device__ __forceinline__ void epilogue_frag(const GemmParams& p, const float* d, uint32_t stg, int wg, int m0,
+                                              int n_idx, float* cbase) {
+  const int t = threadIdx.x & 127, lane = t & 31;
+  const int r = wg * 64 + (t >> 5) * 16 + (lane >> 2);
+  const uint32_t x = (uint32_t)(r & 7);
+  const uint32_t sbase = stg + (uint32_t)(((r >> 5) * (BN / 64)) << 12) + (uint32_t)((r & 31) << 7) +
+                         (uint32_t)(lane & 3) * 4u;
+  // staging address of column pair j of row r + 8h
+  auto sa = [&](int j, int h) -> uint32_t {
+    return sbase + (uint32_t)(h * 1024 + ((j >> 3) << 12)) + ((((uint32_t)j & 7u) ^ x) << 4);
+  };
+  const bool plain = p.out_mode == 0 && p.alpha == 1.0f && p.bias == nullptr && p.bias_f32 == nullptr &&
                      p.preact == nullptr && p.act == 0 && p.residual == nullptr;
-  const bool res_only = to_tma && res_smem && p.alpha == 1.0f && p.bias == nullptr && p.bias_f32 == nullptr &&
-                        p.act == 0;
-  const uint32_t store_s = smem_u32(my_store);
-  const uint32_t lane_row = (uint32_t)lane * 128u;
-  const uint32_t lsw = (uint32_t)(lane & 7);
+  const bool res_only = p.out_mode == 0 && p.residual != nullptr && p.preact == nullptr && p.alpha == 1.0f &&
+                        p.bias == nullptr && p.bias_f32 == nullptr && p.act == 0;
+  if (plain) {
+    // the common case (plain bf16 output, optionally with BN statistics)
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) epi_sts32(sa(j, h), cvt_bf16x2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]));
+    return;
+  }
+  if (res_only) {
+    // skip-gradient path of the dgrad GEMMs: bf16(acc + residual)
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const uint32_t a = epi_lds32(sa(j, h));
+        epi_sts32(sa(j, h), cvt_bf16x2(d[4 * j + 2 * h] + __uint_as_float(a << 16),
+                                       d[4 * j + 2 * h + 1] + __uint_as_float(a & 0xffff0000u)));
+      }
+    return;
+  }
+  const int cq = n_idx + 2 * (lane & 3);
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int col = cq + 8 * j;
+    const bool col_ok = col < p.N;                    // N % 8 == 0: col + 1 < N too
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = m0 + r + 8 * h;
+      float v0 = d[4 * j + 2 * h], v1 = d[4 * j + 2 * h + 1];
+      if (p.alpha != 1.0f) {
+        v0 *= p.alpha;
+        v1 *= p.alpha;
+      }
+      if (p.out_mode != 1) {
+        if (p.bias != nullptr) {
+          if (col_ok) {
+            const __nv_bfloat16* b = reinterpret_cast<const __nv_bfloat16*>(p.bias) + col;
+            v0 += __bfloat162float(b[0]);
+            v1 += __bfloat162float(b[1]);
+          }
+        } else if (p.bias_f32 != nullptr) {
+          if (col_ok) {
+            const float* b = reinterpret_cast<const float*>(p.bias_f32) + col;
+            v0 += b[0];
+            v1 += b[1];
+          }
+        }
+        if (p.preact != nullptr && row < p.M && col_ok)
+          *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.preact) + (size_t)row * p.ldc + col) =
+              cvt_bf16x2(v0, v1);
+        if (p.act == 1) {
+          v0 = fmaxf(v0, 0.0f);
+          v1 = fmaxf(v1, 0.0f);
+        } else if (p.act == 2) {
+          v0 = gelu_erf(v0);
+          v1 = gelu_erf(v1);
+        }
+        if (p.residual != nullptr) {
+          const uint32_t a = epi_lds32(sa(j, h));
+          const float a0 = __uint_as_float(a << 16), a1 = __uint_as_float(a & 0xffff0000u);
+          if (p.act == 3) {
+            v0 *= gelu_erf_grad(a0);
+            v1 *= gelu_erf_grad(a1);
+          } else if (p.act == 4) {
+            v0 = a0 > 0.0f ? v0 : 0.0f;
+            v1 = a1 > 0.0f ? v1 : 0.0f;
+          } else {
+            v0 += a0;
+            v1 += a1;
+          }
+        }
+      }
+      if (p.out_mode == 0) {
+        epi_sts32(sa(j, h), cvt_bf16x2(v0, v1));
+      } else if (row < p.M && col_ok) {
+        float* dst = cbase + (size_t)row * p.ldc + col;
+        if (p.out_mode == 2 || p.splits > 1)
+          asm volatile("st.global.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(v0), "f"(v1) : "memory");
+        else
+          asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(v0), "f"(v1) : "memory");
+      }
+    }
+  }
+}
+
+// Bulk store of slab q (tile rows 32q..32q+31, columns c_begin..c_end-1) of the staged tile, after the tile's
+// epilogue barrier, and the batch statistics of the following BatchNorm: column sums of the staged bf16
+// values.  Lane l owns columns 2l, 2l+1 of a 64-column chunk and walks the 32 rows of the slab in order
+// (one conflict-free 4-byte shared load per row); partials go to the warp's private shared accumulators.
+// Rows that are not part of the output are masked: rows of a convolution tile outside the image (they see
+// partly valid taps) and GEMM rows past M (zero-filled operands, but the epilogue may still have added a bias
+// or an activation of it).
+template <int BN>
+__device__ __forceinline__ void store_slab(const GemmParams& p, const CUtensorMap* map_c, const uint8_t* stg_ptr,
+                                           int q, int lane, int m_row0, int n_idx, int c_begin, int c_end,
+                                           const StoreAt at, float* s_stats) {
 #pragma unroll 1
   for (int c0 = c_begin; c0 < c_end; c0 += 64) {
     const int col0 = n_idx + c0;
     if (col0 >= p.N) continue;                       // warp-uniform
-    const int ncols = min(64, p.N - col0);           // N % 8 == 0 is enforced by the host
-    // Residual / auxiliary operand of the slab: COALESCED 16-byte loads (a warp instruction covers 4 rows
-    // x 128 B), issued before the accumulator loads so that their latency overlaps, then transposed to
-    // row-per-lane through the second (pre-activation) staging buffer.
-    uint4 resv[8];
-    if (res_smem) {
-      const __nv_bfloat16* rbase = reinterpret_cast<const __nv_bfloat16*>(p.residual);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int rr = i * 4 + (lane >> 3), u = lane & 7;
-        resv[i] = (m_row0 + rr < p.M && u * 8 < ncols)
-                      ? *reinterpret_cast<const uint4*>(rbase + (size_t)(m_row0 + rr) * p.ldc + col0 + u * 8)
-                      : make_uint4(0, 0, 0, 0);
-      }
-      if (p.res_mask != nullptr) {
-        // ReLU sign bits of the residual (1 byte per 8 channels): bit j -> 16-bit lane j.  Byte k of
-        // ((bits * 0x01010101) & 0x08040201) + 0x7f7f7f7f has its MSB set iff bit k is, and PRMT's
-        // sign-replicate mode turns that MSB into 0x00 / 0xff bytes.
-        uint32_t mbits[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int rr = i * 4 + (lane >> 3), u = lane & 7;
-          mbits[i] = (m_row0 + rr < p.M && u * 8 < ncols)
-                         ? (uint32_t)p.res_mask[(size_t)(m_row0 + rr) * (size_t)(p.N >> 3) + (size_t)((col0 >> 3) + u)]
-                         : 0u;
-        }
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const uint32_t rep = mbits[i] * 0x01010101u;
-          const uint32_t lo = (rep & 0x08040201u) + 0x7f7f7f7fu, hi = (rep & 0x80402010u) + 0x7f7f7f7fu;
-          resv[i].x &= prmt_sign(lo, 0x9988u);
-          resv[i].y &= prmt_sign(lo, 0xbbaau);
-          resv[i].z &= prmt_sign(hi, 0x9988u);
-          resv[i].w &= prmt_sign(hi, 0xbbaau);
-        }
-      }
-    }
-    // Staging: two 4 KB buffers per warp.  When the second one is not needed for the pre-activation tile or
-    // the residual transpose, consecutive chunks ALTERNATE between them and only wait for the store issued
-    // two chunks ago (cp.async.bulk.wait_group.read 1) — otherwise every chunk stalls on its predecessor's
-    // bulk store reading shared memory.
-    const bool dbuf = to_tma && !z_tma && !res_smem;
-    // buffer parity must alternate over the sequence of chunks THIS warp stages, across tiles: with an even
-    // number of chunks per tile the chunk index does it, with one chunk per tile the (alternating) accumulator
-    // index does
-    const int par = (((c0 - c_begin) >> 6) + acc * (((c_end - c_begin) >> 6) & 1)) & 1;
-    const uint32_t out_s = store_s + ((dbuf && par) ? 4096u : 0u);
-    if (res_smem) {
-      if (lane == 0) tma_store_wait_read<0>();       // (second buffer is about to be rewritten)
-      __syncwarp();
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int rr = i * 4 + (lane >> 3), u = lane & 7;
-        epi_sts128(store_s + 4096u + rr * 128 + ((u ^ (rr & 7)) << 4), resv[i]);
-      }
-      __syncwarp();
-    }
-    const uint32_t taddr = acc_img + (uint32_t)(((q * 32 + lane) * (BN + 4) + c0) * 4);
-    if (plain) {
-      // ---- fast path: accumulator -> bf16 -> swizzled staging rows, nothing else ----
-      uint32_t r[32];
-      acc_ld32(taddr, r);
-      if (lane == 0) {       // the bulk store that last read this buffer must be done reading it
-        if (dbuf) tma_store_wait_read<1>();
-        else tma_store_wait_read<0>();
-      }
-      __syncwarp();
-#pragma unroll
-      for (int j = 0; j < 4; ++j) epi_sts128(out_s + lane_row + ((j ^ lsw) << 4), pack8r(r + j * 8));
-      if (ncols > 32) {
-        acc_ld32(taddr + 128, r);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) epi_sts128(out_s + lane_row + (((4 + j) ^ lsw) << 4), pack8r(r + j * 8));
-      }
-    } else if (res_only) {
-      // ---- skip-gradient path of the dgrad GEMMs: bf16(acc + residual) ----
-#pragma unroll 1
-      for (int half = 0; half < 2; ++half) {
-        if (half * 32 >= ncols) break;
-        uint32_t r[32];
-        acc_ld32(taddr + half * 128, r);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const uint32_t off = lane_row + (((half * 4 + j) ^ lsw) << 4);
-          const uint4 rv = epi_lds128(store_s + 4096u + off);
-          const uint32_t rw[4] = {rv.x, rv.y, rv.z, rv.w};
-          uint4 o;
-          uint32_t* ow = reinterpret_cast<uint32_t*>(&o);
-#pragma unroll
-          for (int w = 0; w < 4; ++w) {
-            const float s0 = __uint_as_float(r[j * 8 + 2 * w]) + __uint_as_float(rw[w] << 16);
-            const float s1 = __uint_as_float(r[j * 8 + 2 * w + 1]) + __uint_as_float(rw[w] & 0xffff0000u);
-            asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(ow[w]) : "f"(s1), "f"(s0));
-          }
-          epi_sts128(out_s + off, o);      // the store that read this buffer was waited for above (res_smem)
-        }
-      }
-    } else {
-#pragma unroll 1
-    for (int half = 0; half < 2; ++half) {
-      const int hc = half * 32;                      // first column of this half inside the chunk
-      if (hc >= ncols) break;                        // warp-uniform
-      const int hcols = min(32, ncols - hc);
-      uint32_t r[32];
-      acc_ld32(taddr + hc * 4, r);
-      float v[32];
-#pragma unroll
-      for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-      if (p.alpha != 1.0f) {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] *= p.alpha;
-      }
-      if (p.out_mode != 1) {
-        if (p.bias != nullptr) {
-          const __nv_bfloat16* b = reinterpret_cast<const __nv_bfloat16*>(p.bias) + col0 + hc;
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (i < hcols) v[i] += __bfloat162float(b[i]);
-        } else if (p.bias_f32 != nullptr) {
-          const float* b = reinterpret_cast<const float*>(p.bias_f32) + col0 + hc;
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (i < hcols) v[i] += b[i];
-        }
-        if (p.preact != nullptr) {
-          if (z_tma) {            // pre-activation tile -> second staging buffer (stored by TMA with the output)
-            if (half == 0) {
-              if (lane == 0) tma_store_wait_read<0>();
-              __syncwarp();
-            }
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-              epi_sts128(store_s + 4096u + lane_row + (((half * 4 + j) ^ lsw) << 4), pack8(v + j * 8));
-          } else if (row_ok) {
-            uint4* pp = reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.preact) +
-                                                 (size_t)row * p.ldc + col0 + hc);
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-              if (j * 8 < hcols) pp[j] = pack8(v + j * 8);
-          }
-        }
-        if (p.act == 1) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = fmaxf(v[i], 0.0f);
-        } else if (p.act == 2) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = gelu_erf(v[i]);
-        }
-        if (p.residual != nullptr && (row_ok || res_smem)) {
-          const uint4* rp = reinterpret_cast<const uint4*>(
-              reinterpret_cast<const __nv_bfloat16*>(p.residual) + (size_t)row * p.ldc + col0 + hc);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            if (j * 8 < hcols) {
-              float a[8];
-              unpack8(res_smem ? epi_lds128(store_s + 4096u + lane_row + (((half * 4 + j) ^ lsw) << 4)) : rp[j], a);
-#pragma unroll
-              for (int t = 0; t < 8; ++t) {
-                if (p.act == 3) v[j * 8 + t] *= gelu_erf_grad(a[t]);
-                else if (p.act == 4) v[j * 8 + t] = a[t] > 0.0f ? v[j * 8 + t] : 0.0f;
-                else v[j * 8 + t] += a[t];
-              }
-            }
-          }
-        }
-      }
-      if (to_tma) {
-        if (half == 0) {       // the bulk store that last read this buffer must be done reading it
-          if (lane == 0) {
-            if (dbuf) tma_store_wait_read<1>();
-            else tma_store_wait_read<0>();
-          }
-          __syncwarp();
-        }
-        // this half of the 32 x 128 B swizzled staging rows (conflict-free 16-byte stores)
-#pragma unroll
-        for (int j = 0; j < 4; ++j)
-          epi_sts128(out_s + lane_row + (((half * 4 + j) ^ lsw) << 4), pack8(v + j * 8));
-      } else if (p.out_mode == 1) {
-        // fp32 accumulation: transpose the 32 x 32 fp32 half through the staging buffer so that a
-        // warp-level RED covers four 128-byte row segments with 16-byte vectors (red.global.add.v4.f32).
-        // With split-K the partial tile is STORED into this split's workspace slice (at.c_ptr) instead.
-        __syncwarp();
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          epi_sts128(store_s + lane_row + ((j ^ lsw) << 4),
-                 make_uint4(__float_as_uint(v[4 * j]), __float_as_uint(v[4 * j + 1]), __float_as_uint(v[4 * j + 2]),
-                            __float_as_uint(v[4 * j + 3])));
-        __syncwarp();
-        float* cbase = reinterpret_cast<float*>(at.c_ptr ? at.c_ptr : p.C);
-        const int ch = lane & 7;
-#pragma unroll
-        for (int it = 0; it < 8; ++it) {
-          const int rr = it * 4 + (lane >> 3);
-          const uint4 t = epi_lds128(store_s + rr * 128 + ((ch ^ (rr & 7)) << 4));
-          if (m_row0 + rr < p.M && ch * 4 < hcols) {
-            float* dst = cbase + (size_t)(m_row0 + rr) * p.ldc + col0 + hc + ch * 4;
-            if (p.splits > 1)
-              asm volatile("st.global.v4.b32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "r"(t.x), "r"(t.y), "r"(t.z),
-                           "r"(t.w)
-                           : "memory");
-            else
-              asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "r"(t.x), "r"(t.y), "r"(t.z),
-                           "r"(t.w)
-                           : "memory");
-          }
-        }
-        __syncwarp();
-      } else if (row_ok) {   // out_mode 2: fp32 store
-        float* dst = reinterpret_cast<float*>(at.c_ptr ? at.c_ptr : p.C) + (size_t)row * p.ldc + col0 + hc;
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          if (j * 4 < hcols)
-            reinterpret_cast<float4*>(dst)[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-      }
-    }
-    }
-    if (to_tma) {
-      fence_async_smem();
-      __syncwarp();
-      if (s_stats != nullptr) {
-        // batch statistics of the following BatchNorm: column sums of the bf16 values just staged.  Lane l
-        // owns columns 2l, 2l+1 of this 64-column chunk and walks the 32 staged rows (one conflict-free
-        // 4-byte shared load per row); partials go to the warp's private shared
-        // accumulators.  Rows that are not part of the output are masked: rows of a convolution tile
-        // outside the image (they see partly valid taps) and GEMM rows past M (zero-filled operands, but
-        // the epilogue may still have added a bias or an activation of it).
-        float sum_lo = 0.f, sum_hi = 0.f, sq_lo = 0.f, sq_hi = 0.f;
-        const uint32_t base = out_s + (uint32_t)((lane & 3) << 2);
-        const uint32_t u = (uint32_t)(lane >> 2);
-        if (at.rank4 || m_row0 + 32 > p.M) {      // lane r decides for slab row r
-          bool ok;
-          if (at.rank4) {
-            const int rw = lane % at.sw, rh = (lane / at.sw) % at.sh, rn = lane / (at.sw * at.sh);
-            ok = rw < at.vw && rh < at.vh && rn < at.vn;
-          } else {
-            ok = m_row0 + lane < p.M;
-          }
-          const uint32_t rows_ok = __ballot_sync(0xffffffffu, ok);
-#pragma unroll
-          for (int rr = 0; rr < 32; ++rr) {
-            uint32_t w;
-            asm volatile("ld.shared.u32 %0, [%1];" : "=r"(w) : "r"(base + rr * 128 + ((u ^ (rr & 7)) << 4)));
-            if (!((rows_ok >> rr) & 1u)) w = 0u;
-            const float lo = __uint_as_float(w << 16), hi = __uint_as_float(w & 0xffff0000u);
-            sum_lo += lo; sum_hi += hi;
-            sq_lo = fmaf(lo, lo, sq_lo); sq_hi = fmaf(hi, hi, sq_hi);
-          }
-        } else {
-#pragma unroll
-          for (int rr = 0; rr < 32; ++rr) {
-            uint32_t w;
-            asm volatile("ld.shared.u32 %0, [%1];" : "=r"(w) : "r"(base + rr * 128 + ((u ^ (rr & 7)) << 4)));
-            const float lo = __uint_as_float(w << 16), hi = __uint_as_float(w & 0xffff0000u);
-            sum_lo += lo; sum_hi += hi;
-            sq_lo = fmaf(lo, lo, sq_lo); sq_hi = fmaf(hi, hi, sq_hi);
-          }
-        }
-        // lane-private slots of the warp's region (columns past N hold zeros: zero-filled B rows)
-        const uint32_t ps = smem_u32(s_stats) + (uint32_t)(((c0 - c_begin) + 2 * lane) << 2);
-        float a0, a1, b0, b1;
-        asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(a0), "=f"(a1) : "r"(ps));
-        asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(b0), "=f"(b1) : "r"(ps + (STATS_WARP_FLOATS / 2) * 4));
-        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(ps), "f"(a0 + sum_lo), "f"(a1 + sum_hi) : "memory");
-        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(ps + (STATS_WARP_FLOATS / 2) * 4), "f"(b0 + sq_lo),
-                     "f"(b1 + sq_hi)
-                     : "memory");
-      }
-      if (lane == 0) {
-        const uint8_t* buf = my_store + (out_s - store_s);
+    const uint8_t* buf = stg_ptr + ((q * (BN / 64) + (c0 >> 6)) << 12);
+    if (s_stats != nullptr) {
+      float sum_lo = 0.f, sum_hi = 0.f, sq_lo = 0.f, sq_hi = 0.f;
+      const uint32_t base = smem_u32(buf) + (uint32_t)((lane & 3) << 2);
+      const uint32_t u = (uint32_t)(lane >> 2);
+      if (at.rank4 || m_row0 + 32 > p.M) {      // lane r decides for slab row r
+        bool ok;
         if (at.rank4) {
-          tma_store_4d(map_c, buf, col0, at.w, at.h, at.n);
+          const int rw = lane % at.sw, rh = (lane / at.sw) % at.sh, rn = lane / (at.sw * at.sh);
+          ok = rw < at.vw && rh < at.vh && rn < at.vn;
         } else {
-          tma_store_2d(map_c, buf, col0, m_row0);
-          if (p.preact != nullptr) tma_store_2d(map_z, buf + 4096, col0, m_row0);
+          ok = m_row0 + lane < p.M;
         }
-        tma_store_commit();
+        const uint32_t rows_ok = __ballot_sync(0xffffffffu, ok);
+#pragma unroll
+        for (int rr = 0; rr < 32; ++rr) {
+          uint32_t w = epi_lds32(base + rr * 128 + ((u ^ (rr & 7)) << 4));
+          if (!((rows_ok >> rr) & 1u)) w = 0u;
+          const float lo = __uint_as_float(w << 16), hi = __uint_as_float(w & 0xffff0000u);
+          sum_lo += lo; sum_hi += hi;
+          sq_lo = fmaf(lo, lo, sq_lo); sq_hi = fmaf(hi, hi, sq_hi);
+        }
+      } else {
+#pragma unroll
+        for (int rr = 0; rr < 32; ++rr) {
+          const uint32_t w = epi_lds32(base + rr * 128 + ((u ^ (rr & 7)) << 4));
+          const float lo = __uint_as_float(w << 16), hi = __uint_as_float(w & 0xffff0000u);
+          sum_lo += lo; sum_hi += hi;
+          sq_lo = fmaf(lo, lo, sq_lo); sq_hi = fmaf(hi, hi, sq_hi);
+        }
       }
+      // lane-private slots of the warp's region (columns past N hold zeros: zero-filled B rows)
+      const uint32_t ps = smem_u32(s_stats) + (uint32_t)(((c0 - c_begin) + 2 * lane) << 2);
+      float a0, a1, b0, b1;
+      asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(a0), "=f"(a1) : "r"(ps));
+      asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(b0), "=f"(b1) : "r"(ps + (STATS_WARP_FLOATS / 2) * 4));
+      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(ps), "f"(a0 + sum_lo), "f"(a1 + sum_hi) : "memory");
+      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(ps + (STATS_WARP_FLOATS / 2) * 4), "f"(b0 + sq_lo),
+                   "f"(b1 + sq_hi)
+                   : "memory");
+    }
+    if (lane == 0) {
+      if (at.rank4) tma_store_4d(map_c, buf, col0, at.w, at.h, at.n);
+      else tma_store_2d(map_c, buf, col0, m_row0);
+      tma_store_commit();
     }
   }
 }
@@ -784,9 +665,10 @@ __device__ __forceinline__ void stats_flush(const GemmParams& p, float* s_stats,
 // ------------------------------------------------------------------ persistent GEMM / convolution body
 // Persistent, warp-specialised, one CTA per SM, NUM_THREADS threads:
 //   warpgroup 0    : TMA producer (one thread) filling the STAGES-deep operand ring
-//   warpgroups 1-2 : 64 rows of the 128 x BN tile each (wg_mainloop); then all 8 warps run the epilogue
-//                    (epilogue_rows), two warps per 32-row slab, each taking half of the columns.  The
-//                    producer keeps filling the ring during the epilogue.
+//   warpgroups 1-2 : 64 rows of the 128 x BN tile each (wg_mainloop), then the epilogue of those rows from
+//                    the fragment (epilogue_frag) into the staging tile; after a barrier each of the 8 warps
+//                    stores one 32-row slab, half of the columns (store_slab).  The producer keeps filling
+//                    the ring during the epilogue.
 // CTA b takes work items b, b + gridDim.x, ...; an item is one output tile, or one split of it.  What the
 // items are is the kernel's Work description:
 //   items             number of work items
@@ -804,12 +686,12 @@ struct Stage {
   uint64_t* bar;
 };
 struct Slab {
-  const CUtensorMap* map_c;   // out_mode 0: output and pre-activation store maps
-  const CUtensorMap* map_z;
+  const CUtensorMap* map_c;   // out_mode 0: output store map
   int m_row0, n_idx;          // first row of the slab in a row-major output (rank-2 StoreAt), first column
   StoreAt at;
-  int tile, m_idx;            // split-K: arrival counter and first row of the output tile,
-  long long c_off;            // and its column offset in C and in each workspace slice
+  int tile;                   // split-K: arrival counter of the output tile
+  int m_idx;                  // rank-2 outputs: first row of the output tile
+  long long c_off;            // split-K: column offset of the tile in C and in each workspace slice
 };
 
 template <int BN, bool A_MN, bool B_MN, class Work>
@@ -820,9 +702,8 @@ __device__ __forceinline__ void persistent_body(const Work& wk, const GemmParams
                                              ~static_cast<uintptr_t>(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + C::STAGES * C::A_BYTES;
-  uint8_t* smem_store = smem + C::STAGES * C::STAGE_BYTES;   // 1024B-aligned staging for TMA stores
-  uint8_t* smem_acc = smem_store + C::STORE_BYTES;           // accumulator image [128][BN + 4] fp32
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_acc + C::ACC_BYTES);
+  uint8_t* smem_store = smem + C::STAGES * C::STAGE_BYTES;   // 1024B-aligned staging tile of the bulk stores
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_store + C::STORE_BYTES);
   uint64_t* full_bar = bars;                     // [STAGES]
   uint64_t* empty_bar = bars + C::STAGES;        // [STAGES]
   float* s_stats = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 256);
@@ -844,6 +725,8 @@ __device__ __forceinline__ void persistent_body(const Work& wk, const GemmParams
 
   if (warp < 4) {
     // ============================ TMA producer ============================
+    // one thread issues the loads: the warpgroup hands its registers to the consumers
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
     if (warp == 0 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -858,19 +741,20 @@ __device__ __forceinline__ void persistent_body(const Work& wk, const GemmParams
     }
   } else {
     // ============================ wgmma + epilogue (warpgroups 1-2) ============================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
     const int cw = warp - 4;                      // consumer warp 0..7
-    const int wg = cw >> 2;                       // rows 64*wg .. 64*wg+63 of the tile
-    const int q = cw & 3;                         // 32-row slab this warp drains
-    const int half = cw >> 2;                     // which half of the columns this warp drains
+    const int wg = cw >> 2;                       // rows 64*wg .. 64*wg+63 of the tile: its wgmma fragment
+    const int r0 = wg * 64 + (cw & 3) * 16;       // the 16 fragment rows of this warp
+    const int q = cw & 3;                         // 32-row slab this warp stores
+    const int half = cw >> 2;                     // which half of the columns this warp stores
     const int c_begin = (BN >= 128) ? half * (BN / 2) : 0;
     const int c_end = (BN >= 128) ? c_begin + BN / 2 : (half == 0 ? BN : 0);
     const int epi_tid = cw * 32 + lane;
-    uint8_t* my_store = smem_store + cw * (2 * 4096);
     float* my_stats = s_stats + cw * STATS_WARP_FLOATS;
-    const uint32_t img = smem_u32(smem_acc);
+    const uint32_t stg = smem_u32(smem_store);
     __shared__ int s_last;
     int stats_n = -1;                             // column block the shared statistics belong to
-    int stage = 0, acc = 0;
+    int stage = 0;
     uint32_t phase = 0;
     float d[BN / 2];
     for (int w = blockIdx.x; w < wk.items; w += gridDim.x) {
@@ -882,16 +766,27 @@ __device__ __forceinline__ void persistent_body(const Work& wk, const GemmParams
         if (stats_n >= 0) stats_flush<BN>(p, s_stats, stats_n, epi_tid);
         stats_n = s.n_idx;
       }
-      named_bar(1, 256);                          // the previous tile's image has been read
-      acc_to_smem<BN>(d, img, BN + 4, wg * 64);
-      named_bar(1, 256);
-      epilogue_rows<BN>(p, s.map_c, s.map_z, img, acc, q, lane, s.m_row0, s.n_idx, c_begin, c_end, my_store, s.at,
-                        want_stats ? my_stats : nullptr);
-      if (Work::kSplitK && p.splits > 1) {
-        const Slab t = wk.slab(w, q);             // recomputed: keeping s live across the epilogue costs spills
-        splitk_finish_tile(p, t.tile, t.m_idx, t.n_idx, BN, t.c_off, epi_tid, &s_last);
+      const bool res = p.residual != nullptr && p.out_mode != 1;
+      uint4 rv[BN / 16];
+      if (res) res_load<BN>(p, rv, s.m_idx, r0, s.n_idx, lane);
+      if (p.out_mode == 0) {
+        // the staging tile is rewritten once every bulk store and statistics walk of the previous tile has read it
+        if (lane == 0) tma_store_wait_read<0>();
+        named_bar(1, 256);
       }
-      acc ^= 1;
+      if (res) {
+        __syncwarp();
+        res_stage<BN>(rv, stg, r0, lane);
+        __syncwarp();
+      }
+      epilogue_frag<BN>(p, d, stg, wg, s.m_idx, s.n_idx, reinterpret_cast<float*>(s.at.c_ptr ? s.at.c_ptr : p.C));
+      if (p.out_mode == 0) {
+        fence_async_smem();                       // the staged tile -> visible to the bulk stores
+        named_bar(1, 256);
+        store_slab<BN>(p, s.map_c, smem_store, q, lane, s.m_row0, s.n_idx, c_begin, c_end, s.at,
+                       want_stats ? my_stats : nullptr);
+      }
+      if (Work::kSplitK && p.splits > 1) splitk_finish_tile(p, s.tile, s.m_idx, s.n_idx, BN, s.c_off, epi_tid, &s_last);
     }
     if (want_stats && stats_n >= 0) stats_flush<BN>(p, s_stats, stats_n, epi_tid);
     if (want_stats) stats_finalize(p, epi_tid);
