@@ -11,8 +11,8 @@
 //   fprop  y[p, co]  = sum_{r,s,ci} x[p + (r,s) - pad, ci] * w[co, r, s, ci]      A = x boxes, B = w (K-major)
 //   dgrad  dx[p, ci] = sum_{r,s,co} dy[p + pad - (r,s), co] * w[co, r, s, ci]     A = dy boxes, B = w (MN-major)
 //   wgrad  dw[co, r, s, ci] = sum_p dy[p, co] * x[p + (r,s) - pad, ci]            A = dy boxes, B = x boxes,
-//          both MN-major with K = 64-pixel boxes; split-K over pixels, the partials added to the fp32
-//          [Cout][R*S*Cin] accumulator in split order (splitk_finish_tile)
+//          both MN-major with K = 64-pixel boxes; split-K over pixels, the partials summed in split order
+//          and written to the [Cout][R*S*Cin] weight gradient in its dtype (splitk_finish_tile)
 //
 // Stride 2 never uses strided gathers: the input (fprop/wgrad) or the output (dgrad) is addressed
 // through four parity views {C, W/2, H/2, N} (base offset (ph*W + pw)*C, doubled pitches), so every
@@ -153,19 +153,15 @@ struct ConvWork {
       at.w = (mt % p.tiles_w) * p.bw + (r0 % p.bw);
       at.h = ((mt / p.tiles_w) % p.tiles_h) * p.bh + (r0 / p.bw) % p.bh;
       at.n = (mt / (p.tiles_w * p.tiles_h)) * p.bn + r0 / (p.bw * p.bh);
-      at.c_ptr = nullptr;
       at.sw = p.sw; at.sh = p.sh;
       at.vw = p.out_w - at.w; at.vh = p.out_h - at.h; at.vn = p.out_n - at.n;
-      return Slab{&maps.out[p.cls[rest / pix_tiles].out_map], 0, nt * BN, at, 0, 0, 0};
+      return Slab{&maps.out[p.cls[rest / pix_tiles].out_map], 0, nt * BN, at, 0, 0, 0, 0};
     }
     const int tile = w % tiles;
     const ConvTap tap = p.cls[0].taps[tile % p.num_taps_total];
     const int mn = tile / p.num_taps_total;
     const int m_idx = (mn / nnb) * BLOCK_M;
-    float* c_ptr = (p.g.splits > 1 ? p.g.splitk_ws + (long long)(w / tiles) * p.g.splitk_slice
-                                   : reinterpret_cast<float*>(p.g.C)) + tap.wcol;
-    return Slab{nullptr, m_idx + q * 32, (mn % nnb) * BN, StoreAt{0, 0, 0, 0, c_ptr, 32, 1, 32, 1, 1},
-                tile, m_idx, tap.wcol};
+    return Slab{nullptr, m_idx + q * 32, (mn % nnb) * BN, StoreAt{}, tile, m_idx, tap.wcol, w / tiles};
   }
 };
 
@@ -380,19 +376,22 @@ int b200dp_conv_dgrad(const void* dy, const void* w, void* dx, int N, int H, int
   return launch_conv<MODE_DGRAD>(maps, p, BN, work, max_ctas, st);
 }
 
-// dw_acc[Cout][R*S*Cin] (fp32) += dy^T (*) x      — split-K over pixels, summed in split order; the caller zeroes
-// dw_acc before the first call and converts it to the weight dtype afterwards.
-int b200dp_conv_wgrad(const void* dy, const void* x, void* dw_acc, int N, int H, int W, int Cin, int Cout, int R,
-                      int S, int stride, int pad, int splits, int block_n, int max_ctas, unsigned long long stream) {
+// dw[Cout][R*S*Cin] (+)= dy^T (*) x   (accumulate: add to dw; out_bf16: dw is bf16, else fp32) — split-K over
+// pixels, summed in fp32 in split order and rounded once to dw's dtype.
+int b200dp_conv_wgrad(const void* dy, const void* x, void* dw, int N, int H, int W, int Cin, int Cout, int R, int S,
+                      int stride, int pad, int splits, int block_n, int max_ctas, int accumulate, int out_bf16,
+                      unsigned long long stream) {
   if (ensure_init()) return -1;
   ConvShape s{N, H, W, Cin, Cout, R, S, stride, pad, 0, 0};
   if (check_shape(s)) return -1;
-  if (((uintptr_t)dy | (uintptr_t)x | (uintptr_t)dw_acc) & 15) return fail("pointers must be 16-byte aligned");
+  if (((uintptr_t)dy | (uintptr_t)x | (uintptr_t)dw) & 15) return fail("pointers must be 16-byte aligned");
   const int BN = pick_bn(Cin, block_n);
   if (BN < 0) return -1;
   ConvMaps maps;
   ConvParams p = conv_params();
-  p.g.M = Cout; p.g.N = Cin; p.g.ldc = R * S * Cin; p.g.C = dw_acc; p.g.out_mode = 1;
+  p.g.M = Cout; p.g.N = Cin; p.g.ldc = R * S * Cin; p.g.C = dw;
+  p.g.out_mode = accumulate ? 1 : 2;
+  p.g.c_bf16 = out_bf16 ? 1 : 0;
   p.g.num_m_blocks = (Cout + BLOCK_M - 1) / BLOCK_M;
   p.g.num_n_blocks = (Cin + BN - 1) / BN;
   choose_box(s.OW, s.OH, N, BLOCK_K, &p.bw, &p.bh, &p.bn);     // 64-pixel K blocks

@@ -693,56 +693,6 @@ __global__ void __launch_bounds__(THREADS) avgpool_bwd_kernel(const uint4* __res
   }
 }
 
-
-// ---- multi-tensor form of cast_acc_zero: one launch converts (and re-zeroes) the fp32 split-K workspaces of
-// every weight gradient of a gradient bucket (blockIdx.y = segment) — 52 launches per ResNet-50 step otherwise.
-constexpr int MULTI_CAST_MAX = 48;
-struct MultiCastSeg {
-  float* src;
-  void* dst;
-  long long n;        // elements, % 4 == 0
-  int flags;          // bit 0: bf16 destination, bit 1: accumulate into dst
-  int pad;
-};
-struct MultiCastArgs {
-  MultiCastSeg seg[MULTI_CAST_MAX];
-  int first_block[MULTI_CAST_MAX + 1];   // 1-D grid: blocks [first_block[i], first_block[i+1]) work on segment i
-  int nseg;
-};
-__global__ void __launch_bounds__(THREADS) multi_cast_acc_zero_kernel(const __grid_constant__ MultiCastArgs a) {
-  int si = 0;
-  while (si + 1 < a.nseg && (int)blockIdx.x >= a.first_block[si + 1]) ++si;
-  const MultiCastSeg& s = a.seg[si];
-  const int lb = blockIdx.x - a.first_block[si], nb = a.first_block[si + 1] - a.first_block[si];
-  const long long nv = s.n >> 2;
-  const bool bf = s.flags & 1, accum = s.flags & 2;
-  float4* src = reinterpret_cast<float4*>(s.src);
-  for (long long i = (long long)lb * THREADS + threadIdx.x; i < nv; i += (long long)nb * THREADS) {
-    float4 v = src[i];
-    src[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (bf) {
-      uint2* d = reinterpret_cast<uint2*>(s.dst) + i;
-      if (accum) {
-        const uint2 o = *d;
-        v.x += __uint_as_float(o.x << 16); v.y += __uint_as_float(o.x & 0xffff0000u);
-        v.z += __uint_as_float(o.y << 16); v.w += __uint_as_float(o.y & 0xffff0000u);
-      }
-      __nv_bfloat162 lo = __floats2bfloat162_rn(v.x, v.y), hi = __floats2bfloat162_rn(v.z, v.w);
-      uint2 o;
-      o.x = *reinterpret_cast<uint32_t*>(&lo);
-      o.y = *reinterpret_cast<uint32_t*>(&hi);
-      *d = o;
-    } else {
-      float4* d = reinterpret_cast<float4*>(s.dst) + i;
-      if (accum) {
-        const float4 o = *d;
-        v.x += o.x; v.y += o.y; v.z += o.z; v.w += o.w;
-      }
-      *d = v;
-    }
-  }
-}
-
 thread_local char g_err[256];
 int fail(const char* what, cudaError_t e) {
   snprintf(g_err, sizeof(g_err), "%s: %s", what, cudaGetErrorString(e));
@@ -771,9 +721,9 @@ int grid_for(long long nvec, int V) {
   return (int)blocks;
 }
 
-// fp32 split-K workspace -> gradient tensor: dst (bf16 or fp32) = (accumulate ? dst : 0) + src, and the
-// workspace is re-zeroed in the same pass so the next step's weight gradient, which the GEMM / convolution
-// adds to the workspace, starts from zero without a memset.
+// fp32 accumulator -> gradient tensor (the attention dQ): dst (bf16 or fp32) = (accumulate ? dst : 0) + src,
+// and the accumulator is re-zeroed in the same pass so the next backward, which adds to it, starts from zero
+// without a memset.
 template <bool OUT_BF16>
 __global__ void cast_acc_zero_kernel(float* __restrict__ src, void* __restrict__ dst, long long n4,
                                      int accumulate, int zero_src) {
@@ -999,31 +949,6 @@ int b200dp_maxpool_bwd(const void* dy, const void* idx, void* dx, int N, int H, 
                                                                              (uint4*)dx, N, H, W, OH, OW, V);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail("maxpool_bwd launch", e);
-  return 0;
-}
-
-// segs: host array of n {src, dst, elements, flags} records (layout of MultiCastSeg); any n (chunked by 48)
-int b200dp_multi_cast_acc_zero(const void* segs, int n, unsigned long long stream) {
-  const MultiCastSeg* h = reinterpret_cast<const MultiCastSeg*>(segs);
-  for (int base = 0; base < n; base += MULTI_CAST_MAX) {
-    const int m = (n - base < MULTI_CAST_MAX) ? n - base : MULTI_CAST_MAX;
-    MultiCastArgs a;
-    a.nseg = m;
-    int total = 0;
-    for (int i = 0; i < m; ++i) {
-      a.seg[i] = h[base + i];
-      if (a.seg[i].n % 4) return -1;
-      long long nb = (a.seg[i].n / 4 + THREADS * 2 - 1) / (THREADS * 2);      // two float4 per thread
-      if (nb < 1) nb = 1;
-      if (nb > 592) nb = 592;
-      a.first_block[i] = total;
-      total += (int)nb;
-    }
-    a.first_block[m] = total;
-    multi_cast_acc_zero_kernel<<<total, THREADS, 0, (cudaStream_t)(uintptr_t)stream>>>(a);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail("multi_cast_acc_zero launch", e);
-  }
   return 0;
 }
 

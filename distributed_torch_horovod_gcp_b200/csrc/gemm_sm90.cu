@@ -72,9 +72,7 @@ struct GemmWork {
   __device__ Slab slab(int w, int q) const {
     const int tile = w % tiles, split = w / tiles;
     const int m0 = m_idx(tile);
-    return Slab{c, m0 + q * 32, n_idx(tile),
-                StoreAt{0, 0, 0, 0, p.splits > 1 ? p.splitk_ws + (long long)split * p.splitk_slice : nullptr},
-                tile, m0, 0};
+    return Slab{c, m0 + q * 32, n_idx(tile), StoreAt{}, tile, m0, 0, split};
   }
 };
 
@@ -111,17 +109,18 @@ extern "C" {
 const char* b200dp_gemm_last_error() { return g_err; }
 
 // A: K-major -> [M][lda>=K]; MN-major -> [K][lda>=M].   B: K-major -> [N][ldb>=K]; MN-major -> [K][ldb>=N].
-// C: [M][ldc>=N].  out_mode 0: bf16 = act(alpha*AB + bias) + residual; 1: fp32 += alpha*AB (with splits > 1
-// the last split to finish adds the partials of all splits, in split order); 2: fp32 store.
+// C: [M][ldc>=N].  out_mode 0: bf16 = act(alpha*AB + bias) + residual; 1: C += alpha*AB; 2: C = alpha*AB, in
+// C's dtype (out_bf16: bf16, else fp32), rounded once from fp32.  With splits > 1 (out_mode 1/2 only) the last
+// split to finish a tile sums the partials of all splits in split order.
 // Requirements: K % 8 == 0 for K-major operands, M % 8 (A) / N % 8 (B) == 0 for MN-major, N % 8 == 0,
 // 16-byte aligned base pointers and leading dimensions.
 int b200dp_gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, int lda, int ldb, int ldc,
                      int a_mn, int b_mn, const void* bias_bf16, const void* bias_f32, const void* residual,
-                     void* preact, int act, int out_mode, float alpha, int splits, int block_n, int max_ctas,
-                     float* stats, const void* res_mask, unsigned long long stream) {
+                     void* preact, int act, int out_mode, int out_bf16, float alpha, int splits, int block_n,
+                     int max_ctas, float* stats, const void* res_mask, unsigned long long stream) {
   if (ensure_init()) return -1;
   if (M <= 0 || N <= 0 || K <= 0) return fail("bad shape");
-  if ((N % 8) || (lda % 8) || (ldb % 8) || (ldc % 4) || ((out_mode == 0) && (ldc % 8)))
+  if ((N % 8) || (lda % 8) || (ldb % 8) || (ldc % 4) || ((out_mode == 0 || out_bf16) && (ldc % 8)))
     return fail("alignment: N, lda, ldb, ldc must be multiples of 8");
   if (((uintptr_t)A | (uintptr_t)B | (uintptr_t)C) & 15) return fail("pointers must be 16-byte aligned");
   const int BN = pick_bn(N, block_n);
@@ -132,8 +131,9 @@ int b200dp_gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K,
   p.num_n_blocks = (N + BN - 1) / BN;
   p.num_k_blocks = (K + BLOCK_K - 1) / BLOCK_K;
   p.splits = normalize_splits(splits, p.num_k_blocks);
-  if (p.splits > 1 && out_mode != 1) return fail("split-K requires out_mode=1 (fp32 accumulate)");
-  p.act = act; p.out_mode = out_mode; p.C = C; p.bias = bias_bf16; p.bias_f32 = bias_f32;
+  if (p.splits > 1 && (out_mode == 0 || bias_bf16 || bias_f32 || residual || preact || act))
+    return fail("split-K requires out_mode 1/2 without bias, residual or activation");
+  p.act = act; p.out_mode = out_mode; p.c_bf16 = out_bf16 ? 1 : 0; p.C = C; p.bias = bias_bf16; p.bias_f32 = bias_f32;
   p.residual = residual; p.preact = preact; p.alpha = alpha;
   p.stats = stats;
   p.res_mask = reinterpret_cast<const unsigned char*>(res_mask);

@@ -6,8 +6,8 @@
 // wgmma keeps its accumulator in the registers of the issuing warpgroup, in a fragment layout (each warp
 // holds 16 rows, each thread two rows x pairs of columns).  The epilogue works on that fragment: each
 // thread applies it to its own elements and writes bf16 pairs into a 128B-swizzled staging copy of the
-// whole tile (or fp32 pairs to global memory).  After a barrier, each warp bulk-stores one 32-row x
-// 64-column box of it and walks its columns for the BatchNorm statistics.  No fp32 copy of the tile goes
+// whole tile (or, in the add / store modes, pairs straight to global memory).  After a barrier, each warp
+// bulk-stores one 32-row x 64-column box of it and walks its columns for the BatchNorm statistics.  No fp32 copy of the tile goes
 // through shared memory, so the space goes to the operand ring instead.
 #pragma once
 #include <cuda.h>
@@ -30,8 +30,9 @@ struct GemmParams {
   int num_m_blocks, num_n_blocks, num_k_blocks;
   int splits;              // split-K factor (>=1)
   int act;                 // 0 none, 1 relu, 2 gelu(erf), 3 *gelu'(aux), 4 *(aux>0)  [aux = residual ptr]
-  int out_mode;            // 0: bf16 via swizzled smem + TMA bulk store, 1: fp32 add into C (split-K: see
-                           // splitk_finish_tile), 2: fp32 store
+  int out_mode;            // 0: bf16 via swizzled smem + TMA bulk store, 1: add into C, 2: store into C (1/2
+                           // with split-K: see splitk_finish_tile)
+  int c_bf16;              // out_mode 1/2: C is bf16 (else fp32)
   void* C;
   const void* bias;        // bf16 [N] or nullptr
   const void* bias_f32;    // fp32 [N] or nullptr
@@ -45,7 +46,7 @@ struct GemmParams {
                            // skip-branch gradient the residual is (N % 64 == 0 required)
   float* stats;            // optional fp32 [2][N]: per-column sum | sum of squares of the bf16 OUTPUT (the batch
                            // statistics of the BatchNorm that follows), accumulated by the epilogue
-  // split-K (splits > 1, out_mode 1): per-launch workspace — one fp32 slice of splitk_slice elements per split,
+  // split-K (splits > 1, out_mode 1/2): per-launch workspace — one fp32 slice of splitk_slice elements per split,
   // laid out like C, and one arrival counter per output tile (zero on entry); see splitk_finish_tile
   float* splitk_ws;
   int* splitk_count;
@@ -310,11 +311,9 @@ struct Cfg {
 
 // Where the rows of a tile go.  rank4 == 0: rows m_row0.. of the row-major [M, ldc] matrix (2D map).
 // rank4 == 1 (convolution): a 32-row slab is the {64 c, sw, sh, sn} sub-box at pixel (w, h, n) of an NHWC
-// tensor.  c_ptr overrides p.C for the fp32 modes (split-K workspace slice, per-tap column offset of the
-// wgrad output).
+// tensor.
 struct StoreAt {
   int rank4, w, h, n;
-  void* c_ptr;
   // rank4 only (statistics of a convolution output): the slab is an {sw, sh, .} pixel box of which only
   // vw x vh x vn pixels lie inside the image / batch — rows outside are computed from partly valid taps
   // (NOT zero) and must not be counted; the TMA store clips them by itself.
@@ -343,6 +342,13 @@ __device__ __forceinline__ uint32_t prmt_sign(uint32_t a, uint32_t sel) {
 __device__ __forceinline__ uint32_t cvt_bf16x2(float lo, float hi) {
   uint32_t o;
   asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(o) : "f"(hi), "f"(lo));
+  return o;
+}
+// (+0) + v with subnormals flushed: what red.add.f32 (RED.ADD.F32.FTZ) leaves in a zeroed fp32 buffer, so a
+// -0 becomes +0.  Written as PTX so that the add is neither folded nor done without FTZ.
+__device__ __forceinline__ float zero_plus_ftz(float v) {
+  float o;
+  asm("add.ftz.f32 %0, %1, %2;" : "=f"(o) : "f"(0.0f), "f"(v));
   return o;
 }
 
@@ -399,13 +405,14 @@ __device__ __forceinline__ void res_stage(const uint4* rv, uint32_t stg, int r0,
 // Epilogue of this thread's part of a finished 128 x BN tile, straight from the wgmma fragment d of
 // warpgroup wg — tile rows r and r + 8 (r = 64 wg + 16 warp + lane / 4), columns 8j + 2 (lane % 4) + {0, 1}:
 // alpha, bias, pre-activation, activation, residual; then bf16 pairs into the staging tile (out_mode 0: the 8
-// rows of a warp store hit 8 different swizzle positions, so the 4-byte stores are conflict-free), fp32
-// pairs added into C (out_mode 1; with split-K stored into the split's workspace slice, cbase) or stored
-// (out_mode 2).  m0: first row of the tile in the [M, ldc] matrix.  A residual (out_mode != 1) has been
-// staged at the output's place; every element is read and then overwritten by the one thread that owns it.
+// rows of a warp store hit 8 different swizzle positions, so the 4-byte stores are conflict-free), or pairs
+// added into C (out_mode 1) or stored (out_mode 2) at column offset c_off, in C's dtype; with split-K, fp32
+// pairs stored into the workspace slice of the item's split.  m0: first row of the tile in the [M, ldc]
+// matrix.  A residual (out_mode != 1) has been staged at the output's place; every element is read and then
+// overwritten by the one thread that owns it.
 template <int BN>
 __device__ __forceinline__ void epilogue_frag(const GemmParams& p, const float* d, uint32_t stg, int wg, int m0,
-                                              int n_idx, float* cbase) {
+                                              int n_idx, int split, long long c_off) {
   const int t = threadIdx.x & 127, lane = t & 31;
   const int r = wg * 64 + (t >> 5) * 16 + (lane >> 2);
   const uint32_t x = (uint32_t)(r & 7);
@@ -440,6 +447,13 @@ __device__ __forceinline__ void epilogue_frag(const GemmParams& p, const float* 
     return;
   }
   const int cq = n_idx + 2 * (lane & 3);
+  // out_mode 1/2: C in its dtype, or with split-K the fp32 workspace slice of the item's split
+  const size_t esz = (p.splits > 1 || !p.c_bf16) ? 4 : 2;
+  char* const cbase = (p.splits > 1 ? reinterpret_cast<char*>(p.splitk_ws + split * p.splitk_slice)
+                                    : reinterpret_cast<char*>(p.C)) + c_off * esz;
+  // bias, pre-activation, activation, residual (out_mode 0 / 2; the add mode ignores them)
+  const bool fused = p.out_mode != 1 && (p.bias != nullptr || p.bias_f32 != nullptr || p.preact != nullptr ||
+                                         p.act != 0 || p.residual != nullptr);
 #pragma unroll
   for (int j = 0; j < BN / 8; ++j) {
     const int col = cq + 8 * j;
@@ -452,7 +466,7 @@ __device__ __forceinline__ void epilogue_frag(const GemmParams& p, const float* 
         v0 *= p.alpha;
         v1 *= p.alpha;
       }
-      if (p.out_mode != 1) {
+      if (fused) {
         if (p.bias != nullptr) {
           if (col_ok) {
             const __nv_bfloat16* b = reinterpret_cast<const __nv_bfloat16*>(p.bias) + col;
@@ -494,11 +508,32 @@ __device__ __forceinline__ void epilogue_frag(const GemmParams& p, const float* 
       if (p.out_mode == 0) {
         epi_sts32(sa(j, h), cvt_bf16x2(v0, v1));
       } else if (row < p.M && col_ok) {
-        float* dst = cbase + (size_t)row * p.ldc + col;
-        if (p.out_mode == 2 || p.splits > 1)
+        const size_t e = (size_t)row * p.ldc + col;
+        if (p.splits > 1) {
+          float* dst = reinterpret_cast<float*>(cbase) + e;
           asm volatile("st.global.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(v0), "f"(v1) : "memory");
-        else
-          asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(v0), "f"(v1) : "memory");
+        } else {
+          // one split: this thread is the only writer of the pair.  (+0) + v first, so that the result is
+          // that of accumulating into a zeroed fp32 buffer and then adding it to C
+          v0 = zero_plus_ftz(v0);
+          v1 = zero_plus_ftz(v1);
+          if (p.c_bf16) {
+            __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(cbase) + e;
+            if (p.out_mode == 1) {
+              uint32_t o;
+              asm volatile("ld.global.b32 %0, [%1];" : "=r"(o) : "l"(dst) : "memory");
+              v0 += __uint_as_float(o << 16);
+              v1 += __uint_as_float(o & 0xffff0000u);
+            }
+            asm volatile("st.global.b32 [%0], %1;" ::"l"(dst), "r"(cvt_bf16x2(v0, v1)) : "memory");
+          } else {
+            float* dst = reinterpret_cast<float*>(cbase) + e;
+            if (p.out_mode == 2)
+              asm volatile("st.global.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(v0), "f"(v1) : "memory");
+            else
+              asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(v0), "f"(v1) : "memory");
+          }
+        }
       }
     }
   }
@@ -609,10 +644,12 @@ __device__ __forceinline__ void stats_finalize(const GemmParams& p, int epi_tid)
 
 // Split-K in a fixed order without waiting: every split stores its partial tile into its own workspace
 // slice, then counts itself in on the tile's counter; the split that arrives LAST sums the slices of all
-// splits in split order and adds the sum to C.  No CTA ever waits for another, so the kernel needs no
-// co-residency, and the result is bit-identical from run to run (fp32 RED.ADDs from the splits would
-// sum in arrival order).  All 256 epilogue threads, after the tile's epilogue; c_off = column offset of
-// the tile's output inside C and inside each slice (the convolution's tap column).
+// splits in split order and writes C + (0 + sum) (out_mode 1) or 0 + sum (out_mode 2), rounded once to C's
+// dtype — the bits of adding the sum to a zeroed fp32 buffer and that buffer to C, signed zeros included.
+// No CTA ever waits for another, so the kernel needs no co-residency, and the result is bit-identical from
+// run to run (fp32 RED.ADDs from the splits would sum in arrival order).  All 256 epilogue threads, after
+// the tile's epilogue; c_off = column offset of the tile's output inside C and inside each slice (the
+// convolution's tap column).
 __device__ __forceinline__ void splitk_finish_tile(const GemmParams& p, int tile, int m_idx, int n_idx, int bn,
                                                    long long c_off, int epi_tid, int* s_last) {
   __threadfence();
@@ -622,7 +659,7 @@ __device__ __forceinline__ void splitk_finish_tile(const GemmParams& p, int tile
   if (!*s_last) return;
   __threadfence();
   const int rows = min(BLOCK_M, p.M - m_idx), c4n = min(bn, p.N - n_idx) >> 2;   // N % 8 == 0
-  float* C = reinterpret_cast<float*>(p.C);
+  const bool add = p.out_mode == 1;
   for (int e = epi_tid; e < rows * c4n; e += 256) {
     const long long off = c_off + (long long)(m_idx + e / c4n) * p.ldc + n_idx + (e % c4n) * 4;
     float4 s = __ldcg(reinterpret_cast<const float4*>(p.splitk_ws + off));
@@ -630,10 +667,24 @@ __device__ __forceinline__ void splitk_finish_tile(const GemmParams& p, int tile
       const float4 v = __ldcg(reinterpret_cast<const float4*>(p.splitk_ws + (long long)k * p.splitk_slice + off));
       s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
     }
-    float4* c = reinterpret_cast<float4*>(C + off);
-    float4 o = *c;
-    o.x += s.x; o.y += s.y; o.z += s.z; o.w += s.w;
-    *c = o;
+    // not an identity for -0, so the compiler keeps these adds
+    s.x = 0.0f + s.x; s.y = 0.0f + s.y; s.z = 0.0f + s.z; s.w = 0.0f + s.w;
+    if (p.c_bf16) {
+      uint2* c = reinterpret_cast<uint2*>(reinterpret_cast<__nv_bfloat16*>(p.C) + off);
+      if (add) {
+        const uint2 o = *c;
+        s.x += __uint_as_float(o.x << 16); s.y += __uint_as_float(o.x & 0xffff0000u);
+        s.z += __uint_as_float(o.y << 16); s.w += __uint_as_float(o.y & 0xffff0000u);
+      }
+      *c = make_uint2(cvt_bf16x2(s.x, s.y), cvt_bf16x2(s.z, s.w));
+    } else {
+      float4* c = reinterpret_cast<float4*>(reinterpret_cast<float*>(p.C) + off);
+      if (add) {
+        const float4 o = *c;
+        s.x += o.x; s.y += o.y; s.z += o.z; s.w += o.w;
+      }
+      *c = s;
+    }
   }
 }
 
@@ -691,7 +742,8 @@ struct Slab {
   StoreAt at;
   int tile;                   // split-K: arrival counter of the output tile
   int m_idx;                  // rank-2 outputs: first row of the output tile
-  long long c_off;            // split-K: column offset of the tile in C and in each workspace slice
+  long long c_off;            // out_mode 1/2: column offset of the tile in C and in each workspace slice
+  int split;                  // split-K: the item's split, whose workspace slice its partial tile goes to
 };
 
 template <int BN, bool A_MN, bool B_MN, class Work>
@@ -725,9 +777,11 @@ __device__ __forceinline__ void persistent_body(const Work& wk, const GemmParams
 
   if (warp < 4) {
     // ============================ TMA producer ============================
-    // one thread issues the loads: the warpgroup hands its registers to the consumers
+    // one thread issues the loads: the warpgroup hands its registers to the consumers.  It is elected here
+    // rather than tested with the lane == 0 of the set-up above, whose predicate would otherwise stay live
+    // through the whole kernel (ptxas then spills the predicates of the 128-column GEMM to local memory)
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
-    if (warp == 0 && lane == 0) {
+    if (warp == 0 && elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
       auto next = [&]() {
@@ -779,7 +833,7 @@ __device__ __forceinline__ void persistent_body(const Work& wk, const GemmParams
         res_stage<BN>(rv, stg, r0, lane);
         __syncwarp();
       }
-      epilogue_frag<BN>(p, d, stg, wg, s.m_idx, s.n_idx, reinterpret_cast<float*>(s.at.c_ptr ? s.at.c_ptr : p.C));
+      epilogue_frag<BN>(p, d, stg, wg, s.m_idx, s.n_idx, s.split, s.c_off);
       if (p.out_mode == 0) {
         fence_async_smem();                       // the staged tile -> visible to the bulk stores
         named_bar(1, 256);

@@ -7,12 +7,11 @@ Weights are consumed as ``[Cout][R][S][Cin]`` — PyTorch's ``channels_last`` la
 ``[Cout, Cin, R, S]`` parameter — so ``model.to(memory_format=torch.channels_last)`` makes the
 parameter itself the GEMM B operand; a parameter in the default layout is re-laid-out per call.
 
-The weight gradient is added to a per-weight fp32 workspace (split-K over pixels: the last split to
-finish adds the partial sums of all splits in split order, so the result is bit-reproducible) that is
-converted to the gradient dtype and re-zeroed by ONE pass (``b200dp_cast_acc_zero``); when the
-parameter carries a ``grad_sink`` (installed by the fused engine) that pass writes straight into
-the parameter's slot of the gradient bucket and fires the bucket counter, so autograd's
-``AccumulateGrad`` add/copy kernels disappear (VERDICT r1 item 2c).
+The weight-gradient kernel writes the gradient in the weight's dtype itself (split-K over pixels: the
+last split to finish a tile sums the fp32 partials of all splits in split order, so the result is
+bit-reproducible, and rounds once).  When the parameter carries a ``grad_sink`` (installed by the fused
+engine) it writes, or adds, straight into the parameter's slot of the gradient bucket and the bucket
+counter fires, so autograd's ``AccumulateGrad`` add/copy kernels disappear.
 """
 from __future__ import annotations
 
@@ -34,14 +33,11 @@ def register(lib, have):
     if not hasattr(lib, "b200dp_conv_fprop"):
         return
     _lib = lib
-    vp, i, u64, ll = ctypes.c_void_p, ctypes.c_int, ctypes.c_uint64, ctypes.c_longlong
+    vp, i, u64 = ctypes.c_void_p, ctypes.c_int, ctypes.c_uint64
     lib.b200dp_conv_fprop.argtypes = [vp, vp, vp] + [i] * 11 + [vp, u64]
     lib.b200dp_conv_dgrad.argtypes = [vp, vp, vp] + [i] * 11 + [u64]
-    lib.b200dp_conv_wgrad.argtypes = [vp, vp, vp] + [i] * 12 + [u64]
+    lib.b200dp_conv_wgrad.argtypes = [vp, vp, vp] + [i] * 14 + [u64]
     lib.b200dp_conv_last_error.restype = ctypes.c_char_p
-    lib.b200dp_cast_acc_zero.argtypes = [vp, vp, ll, i, i, i, u64]
-    if hasattr(lib, "b200dp_multi_cast_acc_zero"):
-        lib.b200dp_multi_cast_acc_zero.argtypes = [vp, i, u64]
     have["conv3x3"] = True
     have["conv_implicit_gemm"] = True
 
@@ -78,19 +74,6 @@ def _krsc(weight: torch.Tensor) -> torch.Tensor:
     return weight.contiguous(memory_format=torch.channels_last)
 
 
-_ws_cache = {}
-
-
-def _workspace(weight: torch.Tensor) -> torch.Tensor:
-    """Per-weight fp32 split-K accumulator; zero on entry (re-zeroed by the cast pass)."""
-    key = (weight.data_ptr(), tuple(weight.shape), weight.device.index)
-    ws = _ws_cache.get(key)
-    if ws is None:
-        ws = torch.zeros(weight.numel(), dtype=torch.float32, device=weight.device)
-        _ws_cache[key] = ws
-    return ws
-
-
 def conv_fprop(x, w_krsc, stride: int, pad: int, stats=None):
     N, Cin, H, W = x.shape
     Cout, _, R, S = w_krsc.shape
@@ -118,24 +101,16 @@ def conv_wgrad(dy, x, weight, stride: int, pad: int) -> Optional[torch.Tensor]:
     """Returns dW in the weight's layout, or ``None`` when it was written into the gradient bucket."""
     N, Cin, H, W = x.shape
     Cout, _, R, S = weight.shape
-    st = torch.cuda.current_stream(dy.device).cuda_stream
-    ws = _workspace(weight)
-    _ck(_lib.b200dp_conv_wgrad(dy.data_ptr(), x.data_ptr(), ws.data_ptr(), N, H, W, Cin, Cout, R, S,
-                               stride, pad, 0, 0, 0, st))
-    # ws is [Cout][R][S][Cin]; the destination must have the same element order
+    # the kernel writes [Cout][R][S][Cin]: the channels_last order of the weight
     dst, acc, done = grad_sink.begin(weight, krsc=True)
     ret = None
     if dst is None:
         dst = torch.empty_like(weight, memory_format=torch.channels_last)
         acc, ret = False, dst
-    if done is not None and grad_sink.defer_cast(_lib, ws, dst, weight.numel(), acc):
-        counters.bump("conv_wgrad", 1)       # converted with the bucket's other gradients (multi-tensor pass)
-    else:
-        rc = _lib.b200dp_cast_acc_zero(ws.data_ptr(), dst.data_ptr(), weight.numel(),
-                                       int(dst.dtype == torch.bfloat16), int(acc), 1, st)
-        if rc != 0:
-            raise RuntimeError("cast_acc_zero failed")
-        counters.bump("conv_wgrad", 2)
+    _ck(_lib.b200dp_conv_wgrad(dy.data_ptr(), x.data_ptr(), dst.data_ptr(), N, H, W, Cin, Cout, R, S,
+                               stride, pad, 0, 0, 0, int(acc), int(dst.dtype == torch.bfloat16),
+                               torch.cuda.current_stream(dy.device).cuda_stream))
+    counters.bump("conv_wgrad", 1)
     if done is not None:
         done()
     return ret

@@ -29,14 +29,10 @@ def register(lib, have):
         return
     _lib = lib
     vp, i, f = ctypes.c_void_p, ctypes.c_int, ctypes.c_float
-    lib.b200dp_gemm_bf16.argtypes = [vp, vp, vp, i, i, i, i, i, i, i, i, vp, vp, vp, vp, i, i, f, i,
+    lib.b200dp_gemm_bf16.argtypes = [vp, vp, vp, i, i, i, i, i, i, i, i, vp, vp, vp, vp, i, i, i, f, i,
                                      i, i, vp, vp, ctypes.c_uint64]
     lib.b200dp_gemm_bf16.restype = i
     lib.b200dp_gemm_last_error.restype = ctypes.c_char_p
-    if hasattr(lib, "b200dp_cast_acc_zero"):
-        lib.b200dp_cast_acc_zero.argtypes = [vp, vp, ctypes.c_longlong, i, i, i, ctypes.c_uint64]
-    if hasattr(lib, "b200dp_multi_cast_acc_zero"):
-        lib.b200dp_multi_cast_acc_zero.argtypes = [vp, i, ctypes.c_uint64]
     have["gemm"] = True
     have["linear"] = True
 
@@ -48,14 +44,15 @@ def gemm(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor, M: int, N: int, K:
          max_ctas: int = 0, stats: Optional[torch.Tensor] = None,
          res_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Raw kernel call.  ``a``: [M,K] (K-major) or [K,M] (MN-major) bf16 with contiguous rows;
-    ``b``: [N,K] or [K,N]; ``out``: [M,N] bf16 (out_mode 0) or fp32 (1: add, 2: store).
-    Split-K (out_mode 1, splits > 1) sums in split order through a workspace allocated per launch on the
-    current stream, so it may run on any stream.  ``stats`` accumulates through one per-library set of
+    ``b``: [N,K] or [K,N]; ``out``: [M,N] bf16 (out_mode 0), or bf16 / fp32 (1: add, 2: store; rounded once
+    from the fp32 result).  Split-K (out_mode 1/2, splits > 1) sums in split order through an fp32 workspace
+    allocated per launch on the current stream, so it may run on any stream.  ``stats`` accumulates through one per-library set of
     per-CTA slots: calls with ``stats`` (and the BatchNorm reductions of ``ops.bn``) must not run
     concurrently on different streams."""
     assert _lib is not None, "libb200dp_kernels.so not loaded"
     assert a.dtype == torch.bfloat16 and b.dtype == torch.bfloat16
     assert a.stride(-1) == 1 and b.stride(-1) == 1 and out.stride(-1) == 1
+    assert out.dtype == torch.bfloat16 or (out_mode != 0 and out.dtype == torch.float32)
     bias_bf = bias.data_ptr() if bias is not None and bias.dtype == torch.bfloat16 else None
     bias_f32 = bias.data_ptr() if bias is not None and bias.dtype == torch.float32 else None
     rc = _lib.b200dp_gemm_bf16(
@@ -63,7 +60,7 @@ def gemm(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor, M: int, N: int, K:
         int(a_mn), int(b_mn), bias_bf, bias_f32,
         residual.data_ptr() if residual is not None else None,
         preact.data_ptr() if preact is not None else None,
-        act, out_mode, float(alpha), splits, block_n, max_ctas,
+        act, out_mode, int(out.dtype == torch.bfloat16), float(alpha), splits, block_n, max_ctas,
         stats.data_ptr() if stats is not None else None,
         res_mask.data_ptr() if res_mask is not None else None,
         torch.cuda.current_stream(a.device).cuda_stream)
@@ -101,50 +98,19 @@ def _ones(M: int, device) -> torch.Tensor:
     return t
 
 
-_ws_cache = {}
-
-
-def _workspace(key, numel: int, device) -> torch.Tensor:
-    """fp32 split-K accumulator, zero on entry: ``b200dp_cast_acc_zero`` re-zeroes it while converting,
-    so no per-step memset / allocation is needed."""
-    ws = _ws_cache.get(key)
-    if ws is None or ws.numel() != numel:
-        ws = torch.zeros(numel, dtype=torch.float32, device=device)
-        _ws_cache[key] = ws
-    return ws
-
-
 def wgrad(dz: torch.Tensor, x2: torch.Tensor, N: int, K: int, M: int, dtype, owner=None):
-    """dW[N,K] = dz[M,N]^T @ x2[M,K] with both operands MN-major (no transposes).  With ``owner`` (the
-    parameter) carrying a grad sink the result goes straight into its gradient-bucket slot and
-    ``None`` is returned (ops/grad_sink.py)."""
+    """dW[N,K] = dz[M,N]^T @ x2[M,K] with both operands MN-major (no transposes), written in ``dtype`` by the
+    GEMM itself.  With ``owner`` (the parameter) carrying a grad sink the result goes straight into its
+    gradient-bucket slot and ``None`` is returned (ops/grad_sink.py)."""
     dst, acc, done = grad_sink.begin(owner) if owner is not None else (None, False, None)
     if dst is not None and dst.dtype != dtype:
         dst, acc, done = None, False, None
-    out = dst.as_strided((N, K), (K, 1)) if dst is not None else None
+    dw = dst.as_strided((N, K), (K, 1)) if dst is not None else torch.empty((N, K), dtype=dtype, device=dz.device)
     splits = _splits_for(N, K, M)
     if splits == 1 and dtype == torch.bfloat16:
-        dw = out if out is not None else torch.empty((N, K), dtype=torch.bfloat16, device=dz.device)
         gemm(dz, x2, dw, N, K, M, a_mn=True, b_mn=True, residual=dw if acc else None)
     else:
-        key = (owner.data_ptr() if owner is not None else 0, N, K, dz.device.index)
-        if owner is None or (N * K) % 4 or not hasattr(_lib, "b200dp_cast_acc_zero"):
-            accum = torch.zeros((N, K), dtype=torch.float32, device=dz.device)
-            gemm(dz, x2, accum, N, K, M, a_mn=True, b_mn=True, out_mode=1, splits=splits)
-            dw = accum.to(dtype)
-            if out is not None:
-                out.add_(dw) if acc else out.copy_(dw)
-        else:
-            ws = _workspace(key, N * K, dz.device).view(N, K)
-            gemm(dz, x2, ws, N, K, M, a_mn=True, b_mn=True, out_mode=1, splits=splits)
-            dw = out if out is not None else torch.empty((N, K), dtype=dtype, device=dz.device)
-            if not (done is not None and out is not None and grad_sink.defer_cast(_lib, ws, dw, N * K, acc)):
-                rc = _lib.b200dp_cast_acc_zero(ws.data_ptr(), dw.data_ptr(), N * K, int(dtype == torch.bfloat16),
-                                               int(acc and out is not None), 1,
-                                               torch.cuda.current_stream(dz.device).cuda_stream)
-                if rc != 0:
-                    raise RuntimeError("cast_acc_zero failed")
-                counters.bump("cast_acc_zero")
+        gemm(dz, x2, dw, N, K, M, a_mn=True, b_mn=True, out_mode=1 if acc else 2, splits=splits)
     if done is not None:
         done()
         return None

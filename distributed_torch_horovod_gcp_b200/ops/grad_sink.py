@@ -17,7 +17,6 @@ when the fused engine owns the gradients.
 """
 from __future__ import annotations
 
-import ctypes
 import os
 from typing import Callable, Optional, Tuple
 
@@ -75,54 +74,6 @@ def begin(weight, krsc: bool = False) -> Tuple[Optional[torch.Tensor], bool, Opt
                 g.is_contiguous(memory_format=torch.channels_last)):
             return None, False, None
     return g, sink.passes_done() > 0, sink.fire
-
-
-# ------------------------------------------------------------------ deferred fp32 -> grad-dtype casts
-# Split-K weight-gradient kernels accumulate in a per-weight fp32 workspace that one pass converts into the
-# gradient-bucket slot and re-zeroes.  With a sink, that pass is DEFERRED: records queue up here and one
-# multi-tensor kernel converts all of them when the first bucket becomes ready (``flush_casts`` is called by
-# the optimizer right before it launches a bucket's reduction, and by ``synchronize``).
-class _CastSeg(ctypes.Structure):
-    _fields_ = [("src", ctypes.c_void_p), ("dst", ctypes.c_void_p), ("n", ctypes.c_longlong),
-                ("flags", ctypes.c_int), ("pad", ctypes.c_int)]
-
-
-_pending_casts: list = []       # (device index, src ptr, dst ptr, n, flags, keep-alive tensors)
-_DEFER = os.environ.get("B200DP_DEFER_CASTS", "1") == "1"
-
-
-def defer_cast(lib, ws: torch.Tensor, dst: torch.Tensor, numel: int, acc: bool) -> bool:
-    """Queue ``dst (+)= cast(ws); ws = 0``.  False when deferral is off / unsupported (caller casts now)."""
-    if not _DEFER or not hasattr(lib, "b200dp_multi_cast_acc_zero") or numel % 4:
-        return False
-    flags = (1 if dst.dtype == torch.bfloat16 else 0) | (2 if acc else 0)
-    if not _pending_casts:
-        try:      # gradients must be complete when backward() returns, bucket launch or not
-            torch.autograd.Variable._execution_engine.queue_callback(flush_casts)
-        except RuntimeError:
-            return False          # not inside a backward pass
-    _pending_casts.append((lib, ws.device.index, ws.data_ptr(), dst.data_ptr(), numel, flags, (ws, dst)))
-    return True
-
-
-def flush_casts() -> None:
-    if not _pending_casts:
-        return
-    by_dev = {}
-    for rec in _pending_casts:
-        by_dev.setdefault(rec[1], []).append(rec)
-    _pending_casts.clear()
-    for dev, recs in by_dev.items():
-        lib = recs[0][0]
-        arr = (_CastSeg * len(recs))()
-        for i, (_, _, src, dst, n, flags, _keep) in enumerate(recs):
-            arr[i].src, arr[i].dst, arr[i].n, arr[i].flags = src, dst, n, flags
-        rc = lib.b200dp_multi_cast_acc_zero(ctypes.byref(arr), len(recs),
-                                            torch.cuda.current_stream(dev).cuda_stream)
-        if rc != 0:
-            raise RuntimeError("multi_cast_acc_zero failed")
-        from . import counters
-        counters.bump("multi_cast_acc_zero")
 
 
 class GradBox:

@@ -231,8 +231,6 @@ class _DistributedOptimizer(torch.optim.Optimizer):
 
     # ------------------------------------------------------------------ launch / sync
     def _launch_bucket(self, b: Bucket):
-        from ..ops import grad_sink
-        grad_sink.flush_casts()        # queued fp32 -> grad-dtype conversions of weight gradients (one launch)
         tl = _state.runtime().timeline
         if tl is not None:
             tl.mark(f"bucket.{b.index}", "BUCKET_READY", bytes=b.nbytes, tensors=len(b.slots))

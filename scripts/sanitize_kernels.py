@@ -3,7 +3,7 @@
 Shapes are small (the tools slow kernels 10-100x) but cover: multi-tile persistent loops (several tiles per
 CTA are not reachable at these sizes on 132 SMs, so max_ctas is forced down where the API allows), the
 statistics / residual / masked-residual / split-K epilogues (per-CTA statistics slots, last-arriver split-K
-reduction), 3x3 / strided / 1x1 conv paths incl. split-K wgrad, BN, LN, pooling, attention and the LSTM
+reduction, fp32 and bf16 add / store outputs), 3x3 / strided / 1x1 conv paths incl. split-K wgrad, BN, LN, pooling, attention and the LSTM
 recurrence."""
 import os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -28,6 +28,10 @@ bits = torch.randint(0, 256, (M, N // 8), device=dev, dtype=torch.uint8)
 G.gemm(a, b, out, M, N, K, residual=r, res_mask=bits, max_ctas=4)
 acc = torch.zeros(N, K, device=dev)
 G.gemm(out, a, acc, N, K, M, a_mn=True, b_mn=True, out_mode=1, splits=4)
+# the same into a bf16 C: split-K store, then a single-split add (no atomics, one writer per element)
+acc16 = torch.empty(N, K, device=dev, dtype=bf)
+G.gemm(out, a, acc16, N, K, M, a_mn=True, b_mn=True, out_mode=2, splits=4)
+G.gemm(out, a, acc16, N, K, M, a_mn=True, b_mn=True, out_mode=1, max_ctas=1)
 print("gemm ok", float(out.float().abs().mean()))
 
 # convolutions: 64 / 256 ch, strided, 1x1, with BN statistics; dgrad + wgrad (split-K) through autograd

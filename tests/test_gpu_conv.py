@@ -53,7 +53,7 @@ def test_conv_matches_fp32_reference(N, C, H, W, K, R, stride):
     yr.backward(g.float())
     assert _rel(x.grad, xr.grad) < 1.5e-2
     assert _rel(w.grad, wr.grad) < 1.5e-2
-    # second backward through a fresh graph: the fp32 split-K workspace must have been re-zeroed
+    # second backward through a fresh graph: no state from the first weight gradient may leak into it
     x.grad = None
     w.grad = None
     y2 = k.conv2d_implicit(x, w, stride, pad)

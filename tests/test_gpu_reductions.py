@@ -4,16 +4,17 @@ Every cross-CTA reduction on the ResNet training path sums its parts in a fixed 
 step computes the same bits on every run:
 
 - split-K GEMM / convolution weight gradient (``splitk_finish_tile``): each split stores its partial tile
-  into its own workspace slice; the last split to arrive sums the slices in split order and adds the sum
-  to C;
+  into its own fp32 workspace slice; the last split to arrive sums the slices in split order and adds the
+  sum to C, or stores it, in C's dtype;
 - BatchNorm statistics from the GEMM / convolution epilogue (``stats_flush`` / ``stats_finalize``) and the
   stand-alone BatchNorm reductions (``block_reduce_to_global``): every CTA writes its own slot and the last
   CTA sums the slots in CTA order.
 
 The tests below check that order exactly (a split-K result must equal the per-split partials of the same
-kernel summed in split order, for any grid size), that results are independent of the grid, that fp32
-outputs lie within a rigorous per-element bound of a float64 reference of the same operation, and that a
-whole ResNet training step repeats bit for bit.
+kernel summed in split order, for any grid size), that results are independent of the grid, that the add /
+store modes write in bf16 or fp32 exactly the bits of adding into a zeroed fp32 buffer and converting that,
+that fp32 outputs lie within a rigorous per-element bound of a float64 reference of the same operation, and
+that a whole ResNet training step repeats bit for bit.
 
 Not covered on purpose: ViT and LSTM training are not reproducible run to run.  The LayerNorm parameter
 gradients (``elementwise.cu``), the attention dQ accumulation (``attn_sm90.cu``) and the LSTM ``dW_hh``
@@ -219,6 +220,65 @@ def test_gemm_splitk_on_side_streams():
             assert torch.equal(outs[i][r], ref[i]), (i, r)
 
 
+# ------------------------------------------------------------------------------------------------ add / store modes
+
+def _assert_same_bits(out, ref, what):
+    """Bit patterns, not values: torch.equal treats -0.0 == +0.0."""
+    itype = torch.int16 if out.dtype == torch.bfloat16 else torch.int32
+    diff = out.contiguous().view(itype) != ref.contiguous().view(itype)
+    if bool(diff.any()):
+        i = int(diff.reshape(-1).nonzero()[0])
+        raise AssertionError(f"{what}: {int(diff.sum())} element(s) differ from the two-stage bits, first: "
+                             f"out={float(out.reshape(-1)[i])!r} ref={float(ref.reshape(-1)[i])!r}")
+
+
+def _two_stage(add_into_zeros, prior, acc):
+    """What the add (``acc``) / store modes must write: the same kernel adds into a zeroed fp32 buffer, and
+    (prior + buffer), or the buffer alone, is rounded once to the prior's dtype.  A -0 sum thus comes out +0."""
+    buf = torch.zeros(prior.shape, device="cuda", dtype=torch.float32)
+    add_into_zeros(buf)
+    return ((prior.float() + buf) if acc else buf).to(prior.dtype)
+
+
+@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float32])
+@pytest.mark.parametrize("a_mn,b_mn,M,N,K,block_n,splits,alpha,extra", SPLITK_CASES)
+def test_gemm_add_store_match_two_stage_bits(a_mn, b_mn, M, N, K, block_n, splits, alpha, extra, dtype):
+    """out_mode 1 (add) and 2 (store) into a bf16 or fp32 C, split-K and one split, for every grid cap.
+    Rows 0..7 of A are zero against an all-negative B, so whole rows of the product are signed zeros, and
+    the prior contents there are -0."""
+    g = _gemm()
+    A, B, a, b = _operands(M, N, K, a_mn, b_mn, seed=K + N + 1)
+    B.abs_().neg_()
+    A[:8] = 0
+    a = A.t().contiguous() if a_mn else A
+    b = B.t().contiguous() if b_mn else B
+    ldc = N + extra
+    prior_big = torch.randn(M, ldc, device="cuda").to(dtype)
+    prior_big[:8] = -0.0
+    prior = prior_big[:, :N]
+    for s in (splits, 1):
+        def add_into_zeros(buf):
+            g.gemm(a, b, buf, M, N, K, a_mn=a_mn, b_mn=b_mn, out_mode=1, splits=s, alpha=alpha, block_n=block_n)
+        for acc in (False, True):
+            ref = _two_stage(add_into_zeros, prior, acc)
+            for max_ctas in (0, 1, 3, 7):
+                big = prior_big.clone() if acc else torch.full_like(prior_big, float("nan"))
+                g.gemm(a, b, big[:, :N], M, N, K, a_mn=a_mn, b_mn=b_mn, out_mode=1 if acc else 2, splits=s,
+                       alpha=alpha, block_n=block_n, max_ctas=max_ctas)
+                torch.cuda.synchronize()
+                _assert_same_bits(big[:, :N], ref, f"splits={s} acc={acc} max_ctas={max_ctas}")
+                if extra:
+                    _assert_same_bits(big[:, N:], prior_big[:, N:] if acc else torch.full_like(big[:, N:], float("nan")),
+                                      "columns past N")
+    # the crafted rows do reach the epilogue as -0 for one sign of alpha (the bf16 store keeps the sign)
+    raw = torch.empty(M, N, device="cuda", dtype=torch.bfloat16)
+    neg_zero = False
+    for al in (1.0, -1.0):
+        g.gemm(a, b, raw, M, N, K, a_mn=a_mn, b_mn=b_mn, alpha=al, block_n=block_n)
+        neg_zero |= bool((raw[:8].view(torch.int16) == -32768).any())
+    assert neg_zero
+
+
 # ------------------------------------------------------------------------------------------------ conv wgrad
 
 CONV_CASES = [
@@ -251,7 +311,9 @@ def _wgrad_ref(x, dy, R, stride, pad):
 
 
 @pytest.mark.parametrize("N,Cin,H,W,Cout,R,stride", CONV_CASES)
-def test_conv_wgrad_grid_invariant_and_bounded(N, Cin, H, W, Cout, R, stride):
+def test_conv_wgrad_fp32_store_add_grid_invariant_and_bounded(N, Cin, H, W, Cout, R, stride):
+    """The weight gradient written to an fp32 dw: stored for every split count and grid, then added onto a
+    prior; grid-invariant bits, and within the fp64 bound."""
     lib = _conv_lib()
     gen = torch.Generator(device="cuda").manual_seed(N * H + Cout)
     pad = (R - 1) // 2
@@ -265,7 +327,7 @@ def test_conv_wgrad_grid_invariant_and_bounded(N, Cin, H, W, Cout, R, stride):
         buf = torch.zeros(Cout, R, R, Cin, device="cuda", dtype=torch.float32) if prefill is None \
             else prefill.clone()
         rc = lib.b200dp_conv_wgrad(dy.data_ptr(), x.data_ptr(), buf.data_ptr(), N, H, W, Cin, Cout, R, R,
-                                   stride, pad, splits, 0, max_ctas, _stream())
+                                   stride, pad, splits, 0, max_ctas, int(prefill is not None), 0, _stream())
         assert rc == 0, lib.b200dp_conv_last_error()
         torch.cuda.synchronize()
         return buf
@@ -280,6 +342,37 @@ def test_conv_wgrad_grid_invariant_and_bounded(N, Cin, H, W, Cout, R, stride):
     pre = torch.randn(Cout, R, R, Cin, device="cuda", generator=gen)
     acc = run(0, 0, prefill=pre)
     _assert_within_bound(acc, pre.double() + ref64, pre.double().abs() + mag64, n_terms + 1, group="conv wgrad")
+
+
+@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float32])
+@pytest.mark.parametrize("N,Cin,H,W,Cout,R,stride", CONV_CASES)
+def test_conv_wgrad_add_store_match_two_stage_bits(N, Cin, H, W, Cout, R, stride, dtype):
+    """The weight gradient written in bf16 or fp32, added (onto a prior whose output channel 0 is -0) or
+    stored, for every split count.  dy channel 0 is zero against an all-negative x, so dw[0] is a sum of
+    signed zeros."""
+    lib = _conv_lib()
+    gen = torch.Generator(device="cuda").manual_seed(N * H + Cout + 1)
+    pad = (R - 1) // 2
+    OH, OW = H // stride, W // stride
+    x = _nhwc(-torch.randn(N, Cin, H, W, device="cuda", generator=gen).abs())
+    dy = torch.randn(N, Cout, OH, OW, device="cuda", generator=gen)
+    dy[:, 0] = 0
+    dy = _nhwc(dy)
+    prior = torch.randn(Cout, R, R, Cin, device="cuda", generator=gen).to(dtype)
+    prior[0] = -0.0
+
+    def run(buf, splits, acc):
+        rc = lib.b200dp_conv_wgrad(dy.data_ptr(), x.data_ptr(), buf.data_ptr(), N, H, W, Cin, Cout, R, R, stride,
+                                   pad, splits, 0, 0, int(acc), int(buf.dtype == torch.bfloat16), _stream())
+        assert rc == 0, lib.b200dp_conv_last_error()
+
+    for splits in (1, 2, 3, 7, 0):
+        for acc in (False, True):
+            ref = _two_stage(lambda buf: run(buf, splits, True), prior, acc)
+            out = prior.clone() if acc else torch.full_like(prior, float("nan"))
+            run(out, splits, acc)
+            torch.cuda.synchronize()
+            _assert_same_bits(out, ref, f"splits={splits} acc={acc}")
 
 
 # ------------------------------------------------------------------------------------------------ BN statistics
@@ -528,8 +621,7 @@ def test_resnet_step_reproducible_across_processes(tmp_path):
 
 def test_resnet_step_reproducible_in_one_process(hvd_single, monkeypatch):
     """Two models built from the same seed and trained for 3 steps in the same process end bit-identical:
-    no state (persistent BatchNorm statistics accumulators, per-weight split-K workspaces, reduction slots)
-    leaks from one run into the next."""
+    no state (persistent BatchNorm statistics accumulators, reduction slots) leaks from one run into the next."""
     monkeypatch.setenv("B200DP_FUSED_SINGLE", "1")
     hvd = hvd_single
     from distributed_torch_horovod_gcp_b200.models import resnet50

@@ -1,8 +1,7 @@
-"""CPU tests of the autograd hand-off protocols in ops/grad_sink.py (no kernels involved): the GradBox
-producer/consumer ordering rules and the deferred-cast queue's no-op behaviour outside a backward pass."""
+"""CPU tests of the autograd hand-off protocol in ops/grad_sink.py (no kernels involved): the GradBox
+producer/consumer ordering rules."""
 import torch
 
-from distributed_torch_horovod_gcp_b200.ops import grad_sink
 from distributed_torch_horovod_gcp_b200.ops.grad_sink import GradBox
 
 
@@ -40,18 +39,3 @@ def test_gradbox_fresh_per_forward():
     a.park(torch.ones(1))
     assert b.dres is None and not b.armed and not b.consumed and not b.want_mask and b.ext_mask is None
 
-
-def test_deferred_cast_is_refused_outside_backward():
-    """defer_cast registers an end-of-backward callback; outside a backward pass (or without the multi-tensor
-    kernel) it must refuse so that the caller converts immediately."""
-    class _NoLib:
-        pass
-    ws, dst = torch.zeros(8), torch.zeros(8, dtype=torch.bfloat16)
-    assert not grad_sink.defer_cast(_NoLib(), ws, dst, 8, False)
-
-    class _Lib:
-        def b200dp_multi_cast_acc_zero(self, *a):
-            raise AssertionError("must not be called")
-    assert not grad_sink.defer_cast(_Lib(), ws, dst, 8, False)      # not inside backward -> RuntimeError path
-    assert not grad_sink._pending_casts
-    grad_sink.flush_casts()                                          # empty queue: no-op
