@@ -62,6 +62,11 @@ def parse_args(argv=None):
                    help="capture the whole training step (fwd+bwd+fused allreduce/update) in one "
                         "CUDA graph; H100-first answer for the launch-bound LSTM config")
     p.add_argument("--data", default=env("B200DP_DATA", "data_es.csv"))
+    p.add_argument("--lstm-layers", type=int, default=int(env("B200DP_LSTM_LAYERS", "1")),
+                   help="stacked LSTM layers of the lstm model (the reference uses 1)")
+    p.add_argument("--bidirectional", action="store_true",
+                   default=env("B200DP_BIDIRECTIONAL", "0") == "1",
+                   help="bidirectional LSTM for the lstm model (the reference is unidirectional)")
     return p.parse_args(argv)
 
 
@@ -131,7 +136,7 @@ if __name__ == "__main__":
                                      shuffle=True, pin_memory=use_cuda, num_workers=nw)
 
         model = LSTM(n_features=23, window_size=window_length, output_size=1, h_size=256,
-                     device=_DEVICE)
+                     n_layers=args.lstm_layers, bidirectional=args.bidirectional, device=_DEVICE)
         optimizer = torch.optim.Adam(model.parameters(), lr=args.lr)
         loss_fn = nn.MSELoss(reduction="mean")
     else:

@@ -159,17 +159,23 @@ __global__ void __launch_bounds__(256) lstm_xproj_kernel(const float* __restrict
 // ---------------------------------------------------------------------------------------------------
 // forward recurrence
 // ---------------------------------------------------------------------------------------------------
-struct RecFwdParams {
+struct RecFwdParams {   // one direction
   const float* w_hh;    // [1024][256]
   const float* xp;      // [T][B][1024]
   const float* h0;      // [B][256]
   const float* c0;      // [B][256]
-  float* seq;           // [B][T][256]
+  float* seq;           // [B][T][ld], this direction's 256 columns (pointer already at its column offset)
   float* hT;            // [B][256]
   float* cT;            // [B][256]
   float* gates;         // [T][B][1024] post-activation i,f,g,o   (nullptr: inference, nothing saved)
   float* cs;            // [T][B][256]  c_t                       (nullptr: inference)
-  int B, T;
+  int reverse;          // walk t = T-1 .. 0
+};
+// The directions of a layer are independent chains: clusters [d * cpd, (d + 1) * cpd) run direction d
+// (cpd = clusters per direction), so every cluster loads one W_hh once and no cluster waits on another.
+struct RecFwdLaunch {
+  RecFwdParams d[2];
+  int ndir, B, T, ld;   // ld: row stride of seq (256 * ndir)
 };
 
 constexpr int FW_A_BYTES = 128 * 1024;               // 8 chunks x [128 rows x 128 B]
@@ -177,7 +183,7 @@ constexpr int FW_B_BYTES = 32 * 1024;                // 8 chunks x [32 rows x 12
 constexpr int FW_G_BYTES = 16 * 1024;                // gate exchange [4][32][32] fp32
 constexpr int FW_SMEM = FW_A_BYTES + 2 * FW_B_BYTES + FW_G_BYTES + IMG_BYTES + 1024;
 
-__global__ void __launch_bounds__(LTHREADS, 1) lstm_rec_fwd_kernel(const RecFwdParams p) {
+__global__ void __launch_bounds__(LTHREADS, 1) lstm_rec_fwd_kernel(const RecFwdLaunch L) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
@@ -188,7 +194,11 @@ __global__ void __launch_bounds__(LTHREADS, 1) lstm_rec_fwd_kernel(const RecFwdP
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const uint32_t c = my_cluster_rank();
-  const int cluster_id = blockIdx.x / CL, num_clusters = gridDim.x / CL;
+  const int cpd = gridDim.x / CL / L.ndir;
+  const int dir = (int)(blockIdx.x / CL) / cpd;
+  const int cluster_id = (int)(blockIdx.x / CL) - dir * cpd, num_clusters = cpd;
+  const RecFwdParams p = dir ? L.d[1] : L.d[0];
+  const int B = L.B, T = L.T;
 
   // ---- resident A operand: W_hh rows {g*256 + 32c + j}, K-major tf32, 128B swizzle.  Loads are issued in
   // batches of 8 independent 128-bit requests per thread before any store (latency-bound otherwise).
@@ -216,14 +226,14 @@ __global__ void __launch_bounds__(LTHREADS, 1) lstm_rec_fwd_kernel(const RecFwdP
   fence_proxy_async_all();
   __syncthreads();
 
-  const int num_tiles = (p.B + NB - 1) / NB;
+  const int num_tiles = (B + NB - 1) / NB;
   for (int tile = cluster_id; tile < num_tiles; tile += num_clusters) {
     const int b0 = tile * NB;
     // ---- h_{-1} = h0 into B buffer 0 (every CTA needs all 256 hidden units); c0 into registers
     for (int i = tid; i < NB * 64; i += LTHREADS) {
       const int b = i >> 6, k4 = i & 63;
       float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (b0 + b < p.B) v = *reinterpret_cast<const float4*>(p.h0 + (size_t)(b0 + b) * LH + k4 * 4);
+      if (b0 + b < B) v = *reinterpret_cast<const float4*>(p.h0 + (size_t)(b0 + b) * LH + k4 * 4);
       sts_v4(smem_u32(sB) + sw_off(b, k4 * 4, NB), v.x, v.y, v.z, v.w);
     }
     float cstate[8], hlast[8];
@@ -232,14 +242,15 @@ __global__ void __launch_bounds__(LTHREADS, 1) lstm_rec_fwd_kernel(const RecFwdP
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       const int b = b0 + bb + i;
-      cstate[i] = (b < p.B) ? p.c0[(size_t)b * LH + c * LU + ju] : 0.f;
+      cstate[i] = (b < B) ? p.c0[(size_t)b * LH + c * LU + ju] : 0.f;
       hlast[i] = 0.f;
     }
     fence_proxy_async_all();
     cluster_barrier();                         // nobody writes into a peer's buffers before it finished the last tile
 
-    for (int t = 0; t < p.T; ++t) {
-      const int cur = t & 1, nxt = cur ^ 1;
+    for (int s = 0; s < T; ++s) {
+      const int t = p.reverse ? T - 1 - s : s;
+      const int cur = s & 1, nxt = cur ^ 1;
       {
         // gate pre-activations h_{t-1} W_slice^T: two m64 halves of the 128 gate rows
         float d0[16], d1[16];
@@ -262,7 +273,7 @@ __global__ void __launch_bounds__(LTHREADS, 1) lstm_rec_fwd_kernel(const RecFwdP
         float xv[NB];
 #pragma unroll
         for (int b = 0; b < NB; ++b)                       // fetch the input projection while the MMAs run
-          xv[b] = (b0 + b < p.B) ? __ldg(p.xp + ((size_t)t * p.B + b0 + b) * LG + grow) : 0.f;
+          xv[b] = (b0 + b < B) ? __ldg(p.xp + ((size_t)t * B + b0 + b) * LG + grow) : 0.f;
         wg_wait<0>();
         wg_fence_operands<16>(d0);
         wg_fence_operands<16>(d1);
@@ -280,7 +291,7 @@ __global__ void __launch_bounds__(LTHREADS, 1) lstm_rec_fwd_kernel(const RecFwdP
         if (p.gates != nullptr) {
 #pragma unroll
           for (int b = 0; b < NB; ++b)
-            if (b0 + b < p.B) p.gates[((size_t)t * p.B + b0 + b) * LG + grow] = v[b];
+            if (b0 + b < B) p.gates[((size_t)t * B + b0 + b) * LG + grow] = v[b];
         }
         const uint32_t gx = smem_u32(sG);
 #pragma unroll
@@ -309,12 +320,12 @@ __global__ void __launch_bounds__(LTHREADS, 1) lstm_rec_fwd_kernel(const RecFwdP
           cstate[i] = gf[i] * cstate[i] + gi[i] * gg[i];
           hlast[i] = go[i] * tanhf_fast(cstate[i]);
           const int b = b0 + bb + i;
-          if (b < p.B) {
-            p.seq[((size_t)b * p.T + t) * LH + kglob] = hlast[i];
-            if (p.cs != nullptr) p.cs[((size_t)t * p.B + b) * LH + kglob] = cstate[i];
+          if (b < B) {
+            p.seq[((size_t)b * T + t) * L.ld + kglob] = hlast[i];
+            if (p.cs != nullptr) p.cs[((size_t)t * B + b) * LH + kglob] = cstate[i];
           }
         }
-        if (t + 1 < p.T) {
+        if (s + 1 < T) {
           // h_t -> chunk `c` of the next step's B operand in ALL 8 CTAs (swizzled K-major rows = batch)
           const uint32_t base = smem_u32(sB + nxt * FW_B_BYTES);
 #pragma unroll
@@ -332,7 +343,7 @@ __global__ void __launch_bounds__(LTHREADS, 1) lstm_rec_fwd_kernel(const RecFwdP
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       const int b = b0 + bb + i;
-      if (b < p.B) {
+      if (b < B) {
         p.hT[(size_t)b * LH + c * LU + ju] = hlast[i];
         p.cT[(size_t)b * LH + c * LU + ju] = cstate[i];
       }
@@ -344,25 +355,29 @@ __global__ void __launch_bounds__(LTHREADS, 1) lstm_rec_fwd_kernel(const RecFwdP
 // ---------------------------------------------------------------------------------------------------
 // backward recurrence
 // ---------------------------------------------------------------------------------------------------
-struct RecBwdParams {
+struct RecBwdParams {   // one direction
   const float* __restrict__ w_hh;    // [1024][256]
   const float* __restrict__ gates;   // [T][B][1024]
   const float* __restrict__ cs;      // [T][B][256]
   const float* __restrict__ c0;      // [B][256]
-  const float* __restrict__ dseq;    // [B][T][256]   (may be nullptr)
+  const float* __restrict__ dseq;    // [B][T][ld] at this direction's column offset (may be nullptr)
   const float* __restrict__ dhT;     // [B][256]      (may be nullptr)
   const float* __restrict__ dcT;     // [B][256]      (may be nullptr)
   float* __restrict__ dgates;        // [T][B][1024]
   float* dh0;           // [B][256]
   float* dc0;           // [B][256]
-  int B, T;
+  int reverse;          // the forward walked t = T-1 .. 0, so this walks t = 0 .. T-1
+};
+struct RecBwdLaunch {   // clusters are split between the directions as in RecFwdLaunch
+  RecBwdParams d[2];
+  int ndir, B, T, ld;
 };
 constexpr int BW_A_BYTES = 128 * 1024;               // W_slice^T: 4 chunks x [256 rows (k) x 128 B (32 gate rows)]
 constexpr int BW_B_BYTES = 16 * 1024;                // dgates: 4 chunks x [32 rows (b) x 128 B]
 constexpr int BW_R_BYTES = 32 * 1024;                // partial dh from 8 sources [8][32 j][32 b], double buffered
 constexpr int BW_SMEM = BW_A_BYTES + BW_B_BYTES + 2 * BW_R_BYTES + IMG_BYTES + 1024;
 
-__global__ void __launch_bounds__(LTHREADS, 1) lstm_rec_bwd_kernel(const RecBwdParams p) {
+__global__ void __launch_bounds__(LTHREADS, 1) lstm_rec_bwd_kernel(const RecBwdLaunch L) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
@@ -373,7 +388,11 @@ __global__ void __launch_bounds__(LTHREADS, 1) lstm_rec_bwd_kernel(const RecBwdP
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const uint32_t c = my_cluster_rank();
-  const int cluster_id = blockIdx.x / CL, num_clusters = gridDim.x / CL;
+  const int cpd = gridDim.x / CL / L.ndir;
+  const int dir = (int)(blockIdx.x / CL) / cpd;
+  const int cluster_id = (int)(blockIdx.x / CL) - dir * cpd, num_clusters = cpd;
+  const RecBwdParams p = dir ? L.d[1] : L.d[0];
+  const int B = L.B, T = L.T;
 
   // ---- resident A operand: (W_slice)^T, rows = k (256), K = local gate row r (128), K-major, swizzled.
   // W rows are read coalesced (128-bit, 8 requests in flight per thread) and scattered transposed.
@@ -407,7 +426,7 @@ __global__ void __launch_bounds__(LTHREADS, 1) lstm_rec_bwd_kernel(const RecBwdP
   fence_proxy_async_all();
   __syncthreads();
 
-  const int num_tiles = (p.B + NB - 1) / NB;
+  const int num_tiles = (B + NB - 1) / NB;
   for (int tile = cluster_id; tile < num_tiles; tile += num_clusters) {
     const int b0 = tile * NB;
     const int ju = lane, bb = warp * 8;
@@ -416,13 +435,15 @@ __global__ void __launch_bounds__(LTHREADS, 1) lstm_rec_bwd_kernel(const RecBwdP
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       const int b = b0 + bb + i;
-      dc_next[i] = (p.dcT != nullptr && b < p.B) ? p.dcT[(size_t)b * LH + kglob] : 0.f;
-      dh_rec[i] = (p.dhT != nullptr && b < p.B) ? p.dhT[(size_t)b * LH + kglob] : 0.f;
+      dc_next[i] = (p.dcT != nullptr && b < B) ? p.dcT[(size_t)b * LH + kglob] : 0.f;
+      dh_rec[i] = (p.dhT != nullptr && b < B) ? p.dhT[(size_t)b * LH + kglob] : 0.f;
     }
     cluster_barrier();
 
-    for (int t = p.T - 1; t >= 0; --t) {
-      const int cur = (p.T - 1 - t) & 1;        // reduce buffer written during this step
+    for (int s = 0; s < T; ++s) {
+      const int t = p.reverse ? s : T - 1 - s;
+      const int tp = p.reverse ? t + 1 : t - 1;  // the step that produced c_{t-1} / h_{t-1}
+      const int cur = s & 1;                     // reduce buffer written during this step
       {
         // ---- dgates for (unit ju, batch bb..bb+7)
         const uint32_t sB_u = smem_u32(sB);
@@ -431,24 +452,24 @@ __global__ void __launch_bounds__(LTHREADS, 1) lstm_rec_bwd_kernel(const RecBwdP
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
           const int b = b0 + bb + i;
-          const bool ok = b < p.B;
-          const size_t gbase = ((size_t)t * p.B + (ok ? b : 0)) * LG + kglob;
+          const bool ok = b < B;
+          const size_t gbase = ((size_t)t * B + (ok ? b : 0)) * LG + kglob;
           gi[i] = ok ? __ldg(p.gates + gbase) : 0.f;
           gf[i] = ok ? __ldg(p.gates + gbase + LH) : 0.f;
           gg[i] = ok ? __ldg(p.gates + gbase + 2 * LH) : 0.f;
           go[i] = ok ? __ldg(p.gates + gbase + 3 * LH) : 0.f;
-          ct[i] = ok ? __ldg(p.cs + ((size_t)t * p.B + b) * LH + kglob) : 0.f;
+          ct[i] = ok ? __ldg(p.cs + ((size_t)t * B + b) * LH + kglob) : 0.f;
           cprev[i] = !ok ? 0.f
-                         : ((t > 0) ? __ldg(p.cs + ((size_t)(t - 1) * p.B + b) * LH + kglob)
+                         : ((s + 1 < T) ? __ldg(p.cs + ((size_t)tp * B + b) * LH + kglob)
                                     : __ldg(p.c0 + (size_t)b * LH + kglob));
-          dsq[i] = (ok && p.dseq != nullptr) ? __ldg(p.dseq + ((size_t)b * p.T + t) * LH + kglob) : 0.f;
+          dsq[i] = (ok && p.dseq != nullptr) ? __ldg(p.dseq + ((size_t)b * T + t) * L.ld + kglob) : 0.f;
         }
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
           const int b = b0 + bb + i;
           float di = 0.f, df = 0.f, dg = 0.f, dob = 0.f;
-          if (b < p.B) {
-            const size_t gbase = ((size_t)t * p.B + b) * LG + kglob;
+          if (b < B) {
+            const size_t gbase = ((size_t)t * B + b) * LG + kglob;
             const float dh = dh_rec[i] + dsq[i];
             const float tc = tanhf_fast(ct[i]);
             const float dc = dc_next[i] + dh * go[i] * (1.0f - tc * tc);
@@ -518,9 +539,9 @@ __global__ void __launch_bounds__(LTHREADS, 1) lstm_rec_bwd_kernel(const RecBwdP
 #pragma unroll
         for (int i = 0; i < 8; ++i) dh_rec[i] = 0.f;
 #pragma unroll
-        for (int s = 0; s < CL; ++s) {
-          const float4 v0 = lds_v4(red + (uint32_t)(((s * 32 + ju) * 32 + bb) * 4));
-          const float4 v1 = lds_v4(red + (uint32_t)(((s * 32 + ju) * 32 + bb + 4) * 4));
+        for (int src = 0; src < CL; ++src) {
+          const float4 v0 = lds_v4(red + (uint32_t)(((src * 32 + ju) * 32 + bb) * 4));
+          const float4 v1 = lds_v4(red + (uint32_t)(((src * 32 + ju) * 32 + bb + 4) * 4));
           dh_rec[0] += v0.x; dh_rec[1] += v0.y; dh_rec[2] += v0.z; dh_rec[3] += v0.w;
           dh_rec[4] += v1.x; dh_rec[5] += v1.y; dh_rec[6] += v1.z; dh_rec[7] += v1.w;
         }
@@ -529,7 +550,7 @@ __global__ void __launch_bounds__(LTHREADS, 1) lstm_rec_bwd_kernel(const RecBwdP
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       const int b = b0 + bb + i;
-      if (b < p.B) {
+      if (b < B) {
         if (p.dh0 != nullptr) p.dh0[(size_t)b * LH + kglob] = dh_rec[i];
         if (p.dc0 != nullptr) p.dc0[(size_t)b * LH + kglob] = dc_next[i];
       }
@@ -540,14 +561,18 @@ __global__ void __launch_bounds__(LTHREADS, 1) lstm_rec_bwd_kernel(const RecBwdP
 
 // ---------------------------------------------------------------------------------------------------
 // weight / bias / input gradients: sums over (t, b), off the serial chain -> all SMs, fp32 SIMT
-//   dW_hh[r][k] = sum dG[t][b][r] * hprev[t][b][k]     (hprev[0] = h0, hprev[t] = seq[:, t-1])
-//   dW_ih[r][f] = sum dG[t][b][r] * x[b][t][f],   db[r] = sum dG[t][b][r]
-//   dx[b][t][f] = sum_r dG[t][b][r] * W_ih[r][f]                                   (optional)
+//   dW_hh[r][k] = sum dG[t][b][r] * hprev[t][b][k]     (hprev[0] = h0, hprev[t] = seq[:, t-1]; a reverse
+//                                                       direction: hprev[T-1] = h0, hprev[t] = seq[:, t+1])
+//   dW_ih[r][f] = sum dG[t][b][r] * x[b][t][f],   db[r] = sum dG[t][b][r]              (F <= 32)
+//   dx[b][t][f] = sum_r dG[t][b][r] * W_ih[r][f]                          (optional, one direction)
+// One launch per direction.  For F > 32 the dW_ih / db blocks are not launched and for two directions no dx
+// blocks are: lstm_ih_wgrad_kernel / lstm_dx_kernel compute those.
 // ---------------------------------------------------------------------------------------------------
 struct WgParams {
   const float* dG; const float* seq; const float* h0; const float* x; const float* w_ih;
   float* dW_hh; float* dW_ih; float* db_ih; float* db_hh; float* dx;
   int B, T, F, ksplit;
+  int ld, reverse;      // row stride of seq (at this direction's column offset); direction
 };
 constexpr int WG_TR = 64, WG_TK = 64, WG_KC = 16;
 
@@ -573,7 +598,9 @@ __global__ void __launch_bounds__(256) lstm_wgrad_kernel(const WgParams p) {
         float hv = 0.f;
         if (qq < q1) {
           const int t = qq / p.B, b = qq % p.B;
-          hv = (t == 0) ? p.h0[(size_t)b * LH + k0 + rr] : p.seq[((size_t)b * p.T + (t - 1)) * LH + k0 + rr];
+          const int tp = p.reverse ? t + 1 : t - 1;
+          hv = (tp < 0 || tp == p.T) ? p.h0[(size_t)b * LH + k0 + rr]
+                                     : p.seq[((size_t)b * p.T + tp) * p.ld + k0 + rr];
         }
         sH[kk][rr] = hv;
       }
@@ -657,6 +684,197 @@ __global__ void __launch_bounds__(256) lstm_wgrad_kernel(const WgParams p) {
   }
 }
 
+// ---------------------------------------------------------------------------------------------------
+// input-side products for inputs wider than the register-array paths above (F > 32: the layers above the
+// first see 256 or 512 features), and dx of a layer with two directions.  Each is a [T*B] x F x 1024 product
+// on tf32 wgmma with fp32 accumulation, the numerics of the recurrence:
+//   xp[t][b][r]  = sum_f x[b][t][f] W_ih[r][f] + (b_ih[r] + b_hh[r])      MODE_XPROJ  M = (t,b), N = r, K = f
+//   dW_ih[r][f]  = sum_(t,b) dG[t][b][r] x[b][t][f]                         MODE_WGRAD  M = r, N = f, K = (t,b)
+//   db[r]        = sum_(t,b) dG[t][b][r]     (column N = F of the same product, against a column of ones)
+//   dx[b][t][f]  = sum_r dG_fwd W_ih_fwd  (+ sum_r dG_rev W_ih_rev)        MODE_DX     M = (t,b), N = f, K = r
+// One warpgroup per CTA, a 128 x 64 output tile (two m64 halves x two n32 halves), K staged 32 at a time into
+// 128B-swizzled K-major shared memory.  tf32 wgmma has no transposed-operand mode, so operands that are
+// MN-major in memory (dG and x for dW_ih, W_ih for dx) are read along MN (coalesced) and transposed by the
+// shared-memory store; the next chunk's loads are in flight while the current chunk's MMAs run.
+// Every sum has a fixed order and no atomics: a CTA owns the whole K of its tile, except that dW_ih / db split
+// (t, b) into ranges whose partial tiles go to their own workspace slices, summed in split order by
+// lstm_ih_wgrad_finish_kernel.  dx of two directions is (forward sum) + (reverse sum), in that order.
+// ---------------------------------------------------------------------------------------------------
+struct IhDir {          // one direction's input-side operands
+  const float* w_ih; const float* b_ih; const float* b_hh; float* xp;   // forward
+  const float* dG; float* dW_ih; float* db_ih; float* db_hh;            // backward
+};
+constexpr int XPROJ_SIMT_MAX_F = 32;   // F up to this uses lstm_xproj_kernel / the lstm_wgrad_kernel branches
+constexpr int IM = 128, IN = 64, IK = 32;
+constexpr int MODE_XPROJ = 0, MODE_WGRAD = 1, MODE_DX = 2;
+
+struct InMmaArgs {
+  IhDir d0, d1;
+  const float* x;       // layer input [B][T][F]
+  float* out;           // MODE_DX: dx [B][T][F];  MODE_WGRAD: workspace [ndir][splits][1024][F + 1]
+  int B, T, F, ndir, splits, per;   // per: (t, b) rows of one dW_ih split (a multiple of IK)
+};
+
+// Stage ROWS x 32 fp32 of an operand into K-major swizzled shared memory: element (row, k) of the chunk.
+// K_CONTIG: consecutive k are adjacent in memory (a warp reads one row); otherwise consecutive rows are (a warp
+// reads 32 rows of one k and the store transposes them).
+template <int ROWS, bool K_CONTIG, typename Get>
+__device__ __forceinline__ void stage(uint32_t s, Get get) {
+#pragma unroll 4
+  for (int u = 0; u < ROWS * IK / 128; ++u) {
+    const int i = threadIdx.x + 128 * u;
+    const int row = K_CONTIG ? i / IK : i % ROWS, k = K_CONTIG ? i % IK : i / ROWS;
+    sts_f32(s + sw_off(row, k, ROWS), get(row, k));
+  }
+}
+
+constexpr int IBUF = (IM + IN) * IK * 4;   // one stage: A [128 x 32] + B [64 x 32] fp32
+
+// acc[mh][nq] += A[128 x K] B[64 x K]^T over chunks [0, nk) of K.  Two stages: the loads and stores of chunk
+// kc + 1 run while the MMAs of chunk kc do.
+template <bool A_K, bool B_K, typename GetA, typename GetB>
+__device__ __forceinline__ void in_mma_loop(float (&acc)[2][2][16], uint32_t smem, int nk, GetA ga, GetB gb) {
+  for (int kc = 0; kc < nk; ++kc) {
+    const uint32_t sA = smem + (kc & 1) * IBUF, sB = sA + IM * IK * 4;
+    const int k0 = kc * IK;
+    stage<IM, A_K>(sA, [&](int r, int k) { return ga(r, k0 + k); });
+    stage<IN, B_K>(sB, [&](int r, int k) { return gb(r, k0 + k); });
+    fence_proxy_async_all();
+    __syncthreads();
+    const uint64_t da = make_desc_base(16, 1024) + desc_addr(sA);
+    const uint64_t db = make_desc_base(16, 1024) + desc_addr(sB);
+    wg_fence();
+#pragma unroll
+    for (int ks = 0; ks < IK / 8; ++ks)
+#pragma unroll
+      for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+        for (int nq = 0; nq < 2; ++nq)
+          wgmma_tf32_n32(acc[mh][nq], da + (uint64_t)((mh * 64 * 128 + ks * 32) >> 4),
+                         db + (uint64_t)((nq * 32 * 128 + ks * 32) >> 4), 1u);
+    wg_commit();
+    wg_wait<1>();                                        // chunk kc - 1 is done: its stage is free again
+  }
+  wg_wait<0>();
+#pragma unroll
+  for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+    for (int nq = 0; nq < 2; ++nq) wg_fence_operands<16>(acc[mh][nq]);
+  __syncthreads();                                       // the stages may be restaged by a following loop
+}
+
+// element (m, n) of the tile held by this thread: fragment value acc[mh][nq][4 j + 2 h + e]
+template <typename Put>
+__device__ __forceinline__ void in_mma_epilogue(const float (&acc)[2][2][16], Put put) {
+  const int t = threadIdx.x;
+#pragma unroll
+  for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+    for (int nq = 0; nq < 2; ++nq)
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+            put(mh * 64 + (t >> 5) * 16 + ((t & 31) >> 2) + 8 * h, nq * 32 + 8 * j + 2 * (t & 3) + e,
+                acc[mh][nq][4 * j + 2 * h + e]);
+}
+
+template <int MODE>
+__global__ void __launch_bounds__(128, 1) lstm_in_mma_kernel(const InMmaArgs a) {
+  __shared__ __align__(1024) uint8_t smem_raw[2 * IBUF];
+  const uint32_t smem = smem_u32(smem_raw);
+  const int B = a.B, T = a.T, F = a.F, TB = T * B;
+  const int m0 = blockIdx.x * IM, n0 = blockIdx.y * IN;
+  // x row of (t, b) index q (x is [B][T][F])
+  auto xrow = [&](int q) { return a.x + ((size_t)(q % B) * T + q / B) * F; };
+  float acc[2][2][16];
+#pragma unroll
+  for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+    for (int nq = 0; nq < 2; ++nq)
+#pragma unroll
+      for (int i = 0; i < 16; ++i) acc[mh][nq][i] = 0.f;
+
+  if constexpr (MODE == MODE_XPROJ) {
+    const IhDir d = blockIdx.z ? a.d1 : a.d0;
+    in_mma_loop<true, true>(
+        acc, smem, (F + IK - 1) / IK,
+        [&](int r, int k) { const int q = m0 + r; return (q < TB && k < F) ? __ldg(xrow(q) + k) : 0.f; },
+        [&](int r, int k) { return k < F ? __ldg(d.w_ih + (size_t)(n0 + r) * F + k) : 0.f; });
+    in_mma_epilogue(acc, [&](int m, int n, float v) {
+      const int q = m0 + m, r = n0 + n;
+      if (q < TB) d.xp[(size_t)q * LG + r] = v + (d.b_ih[r] + d.b_hh[r]);
+    });
+  } else if constexpr (MODE == MODE_WGRAD) {
+    const int dir = blockIdx.z / a.splits, split = blockIdx.z % a.splits;
+    const IhDir d = dir ? a.d1 : a.d0;
+    const int q0 = split * a.per, q1 = min(q0 + a.per, TB);
+    in_mma_loop<false, false>(
+        acc, smem, (q1 - q0 + IK - 1) / IK,
+        [&](int r, int k) { const int q = q0 + k; return q < q1 ? __ldg(d.dG + (size_t)q * LG + m0 + r) : 0.f; },
+        [&](int r, int k) {
+          const int q = q0 + k, f = n0 + r;
+          if (q >= q1 || f > F) return 0.f;
+          return f == F ? 1.f : __ldg(xrow(q) + f);
+        });
+    float* ws = a.out + ((size_t)dir * a.splits + split) * LG * (F + 1);
+    in_mma_epilogue(acc, [&](int m, int n, float v) {
+      if (n0 + n <= F) ws[(size_t)(m0 + m) * (F + 1) + n0 + n] = v;
+    });
+  } else {
+    in_mma_loop<true, false>(
+        acc, smem, LG / IK,
+        [&](int r, int k) { const int q = m0 + r; return q < TB ? __ldg(a.d0.dG + (size_t)q * LG + k) : 0.f; },
+        [&](int r, int k) { const int f = n0 + r; return f < F ? __ldg(a.d0.w_ih + (size_t)k * F + f) : 0.f; });
+    in_mma_epilogue(acc, [&](int m, int n, float v) {
+      const int q = m0 + m, f = n0 + n;
+      if (q < TB && f < F) a.out[((size_t)(q % B) * T + q / B) * F + f] = v;
+    });
+    if (a.ndir == 2) {                                   // + the reverse direction's sum, read back by its writer
+#pragma unroll
+      for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+        for (int nq = 0; nq < 2; ++nq)
+#pragma unroll
+          for (int i = 0; i < 16; ++i) acc[mh][nq][i] = 0.f;
+      in_mma_loop<true, false>(
+          acc, smem, LG / IK,
+          [&](int r, int k) { const int q = m0 + r; return q < TB ? __ldg(a.d1.dG + (size_t)q * LG + k) : 0.f; },
+          [&](int r, int k) { const int f = n0 + r; return f < F ? __ldg(a.d1.w_ih + (size_t)k * F + f) : 0.f; });
+      in_mma_epilogue(acc, [&](int m, int n, float v) {
+        const int q = m0 + m, f = n0 + n;
+        if (q < TB && f < F) {
+          float* o = a.out + ((size_t)(q % B) * T + q / B) * F + f;
+          *o = *o + v;
+        }
+      });
+    }
+  }
+}
+
+// dW_ih / db of every direction: the split slices of each element summed in split order
+__global__ void __launch_bounds__(256) lstm_ih_wgrad_finish_kernel(const InMmaArgs a) {
+  const int F1 = a.F + 1;
+  const size_t per_dir = (size_t)LG * F1;
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= per_dir * a.ndir) return;
+  const int dir = (int)(i / per_dir);
+  const size_t e = i % per_dir;
+  const float* ws = a.out + (size_t)dir * a.splits * per_dir + e;
+  float s = ws[0];
+  for (int k = 1; k < a.splits; ++k) s += ws[(size_t)k * per_dir];
+  const IhDir d = dir ? a.d1 : a.d0;
+  const int r = (int)(e / F1), f = (int)(e % F1);
+  if (f < a.F) {
+    d.dW_ih[(size_t)r * a.F + f] = s;
+  } else {
+    d.db_ih[r] = s;
+    d.db_hh[r] = s;
+  }
+}
+
 int g_sms = 0;
 int sms() {
   if (!g_sms) {
@@ -689,50 +907,122 @@ int launch_cluster(K kern, const P& p, int clusters, int smem_bytes, cudaStream_
   return 0;
 }
 
+constexpr int MAX_F = 512;   // widest input: the 512 outputs of a bidirectional layer
+
+int cluster_split(int B, int ndir) {   // clusters per direction
+  const int tiles = (B + NB - 1) / NB;
+  int cpd = sms() / CL / ndir;
+  if (cpd > tiles) cpd = tiles;
+  if (cpd < 1) cpd = 1;
+  return cpd;
+}
+
+int check_shape(int ndir, int B, int T, int F) {
+  if (F < 1 || F > MAX_F || ndir < 1 || ndir > 2 || B < 1 || T < 1)
+    return lfail("unsupported LSTM shape: H=256 needs F in 1..512, 1 or 2 directions, B >= 1, T >= 1", F);
+  return 0;
+}
+
+enum { FW_W_IH, FW_W_HH, FW_B_IH, FW_B_HH, FW_H0, FW_C0, FW_XP, FW_GATES, FW_CS, FW_HT, FW_CT, FW_NPTR };
+enum { BW_W_IH, BW_W_HH, BW_H0, BW_C0, BW_GATES, BW_CS, BW_DHT, BW_DCT, BW_DGATES, BW_DH0, BW_DC0, BW_DW_IH,
+       BW_DW_HH, BW_DB_IH, BW_DB_HH, BW_NPTR };
+
+// dW_ih / db of one layer on tf32 wgmma: the (t, b) sum is split so that the tiles fill the GPU; each split's
+// partial tile goes to its own workspace slice (allocated on the stream, so CUDA graphs capture it) and the
+// finish kernel sums the slices in split order.
+int launch_ih_wgrad(InMmaArgs a, cudaStream_t st) {
+  const int TB = a.T * a.B;
+  const int tiles = (LG / IM) * ((a.F + 1 + IN - 1) / IN) * a.ndir;
+  int splits = (2 * sms() + tiles - 1) / tiles;
+  const int max_splits = (TB + 4 * IK - 1) / (4 * IK);          // at least 128 (t, b) rows per split
+  if (splits > max_splits) splits = max_splits;
+  if (splits < 1) splits = 1;
+  a.per = ((TB + splits - 1) / splits + IK - 1) / IK * IK;
+  a.splits = (TB + a.per - 1) / a.per;
+  const size_t n = (size_t)a.ndir * a.splits * LG * (a.F + 1);
+  cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&a.out), n * sizeof(float), st);
+  if (e != cudaSuccess) return lfail(cudaGetErrorString(e), (int)e);
+  lstm_in_mma_kernel<MODE_WGRAD><<<dim3(LG / IM, (a.F + 1 + IN - 1) / IN, a.ndir * a.splits), 128, 0, st>>>(a);
+  const size_t outs = (size_t)a.ndir * LG * (a.F + 1);
+  lstm_ih_wgrad_finish_kernel<<<(unsigned)((outs + 255) / 256), 256, 0, st>>>(a);
+  e = cudaFreeAsync(a.out, st);
+  if (e != cudaSuccess) return lfail(cudaGetErrorString(e), (int)e);
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
 
 const char* b200dp_lstm_rec_last_error() { return g_lerr; }
 
-int b200dp_lstm_rec_supported(int H, int F) { return (H == LH && F >= 1 && F <= 32) ? 1 : 0; }
+// Hidden size 256; input widths 1..512 (layer 0 of a model, or 256 / 512 above a one- / two-direction layer).
+int b200dp_lstm_rec_supported(int H, int F) { return (H == LH && F >= 1 && F <= MAX_F) ? 1 : 0; }
 
-// Forward: x [B][T][F], h0/c0 [B][256], weights in PyTorch layout; outputs seq [B][T][256], hT/cT [B][256].
-// xp_ws: [T][B][1024] workspace.  gates/cs: saved for backward ([T][B][1024] / [T][B][256]) or null.
-int b200dp_lstm_rec_fwd(const float* x, const float* h0, const float* c0, const float* w_ih, const float* w_hh,
-                        const float* b_ih, const float* b_hh, float* xp_ws, float* seq, float* hT, float* cT,
-                        float* gates, float* cs, int B, int T, int F, unsigned long long stream) {
-  if (!b200dp_lstm_rec_supported(LH, F)) return lfail("unsupported LSTM shape");
+// One layer, one or both directions (direction 1 is the reverse one).  x [B][T][F]; seq [B][T][256 * ndir],
+// direction d writes columns [256 d, 256 d + 256).  `dir_ptrs` holds FW_NPTR pointers per direction, in the
+// order of the FW_* enum: weights in PyTorch layout, h0/c0/hT/cT [B][256] (slices of the [layers * ndir][B][256]
+// state), the xp workspace [T][B][1024], and gates/cs saved for backward ([T][B][1024] / [T][B][256]) or null.
+int b200dp_lstm_rec_fwd(const float* x, float* seq, const void* const* dir_ptrs, int ndir, int B, int T, int F,
+                        unsigned long long stream) {
+  if (check_shape(ndir, B, T, F)) return -1;
   cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
   const int rows = T * B;
-  lstm_xproj_kernel<<<(rows + 7) / 8, 256, 8 * F * sizeof(float), st>>>(x, w_ih, b_ih, b_hh, xp_ws, B, T, F);
-  RecFwdParams p{w_hh, xp_ws, h0, c0, seq, hT, cT, gates, cs, B, T};
-  const int tiles = (B + NB - 1) / NB;
-  int clusters = sms() / CL;
-  if (clusters > tiles) clusters = tiles;
-  if (clusters < 1) clusters = 1;
-  return launch_cluster(lstm_rec_fwd_kernel, p, clusters, FW_SMEM, st);
+  RecFwdLaunch L{};
+  IhDir ih[2] = {};
+  L.ndir = ndir; L.B = B; L.T = T; L.ld = LH * ndir;
+  for (int d = 0; d < ndir; ++d) {
+    const float* const* v = reinterpret_cast<const float* const*>(dir_ptrs) + d * FW_NPTR;
+    float* xp = const_cast<float*>(v[FW_XP]);
+    if (F <= XPROJ_SIMT_MAX_F)
+      lstm_xproj_kernel<<<(rows + 7) / 8, 256, 8 * F * sizeof(float), st>>>(x, v[FW_W_IH], v[FW_B_IH], v[FW_B_HH],
+                                                                            xp, B, T, F);
+    ih[d].w_ih = v[FW_W_IH]; ih[d].b_ih = v[FW_B_IH]; ih[d].b_hh = v[FW_B_HH]; ih[d].xp = xp;
+    L.d[d] = RecFwdParams{v[FW_W_HH], xp, v[FW_H0], v[FW_C0], seq + d * LH, const_cast<float*>(v[FW_HT]),
+                          const_cast<float*>(v[FW_CT]), const_cast<float*>(v[FW_GATES]),
+                          const_cast<float*>(v[FW_CS]), d};
+  }
+  if (F > XPROJ_SIMT_MAX_F) {
+    const InMmaArgs a{ih[0], ih[ndir - 1], x, nullptr, B, T, F, ndir, 1, 0};
+    lstm_in_mma_kernel<MODE_XPROJ><<<dim3((rows + IM - 1) / IM, LG / IN, ndir), 128, 0, st>>>(a);
+  }
+  return launch_cluster(lstm_rec_fwd_kernel, L, cluster_split(B, ndir) * ndir, FW_SMEM, st);
 }
 
-// Backward of the recurrence + all parameter gradients.  dW_hh [1024][256] must be ZERO on entry (split-K
-// atomics); dW_ih / db_ih / db_hh are overwritten; dx may be null.
-int b200dp_lstm_rec_bwd(const float* x, const float* h0, const float* c0, const float* w_ih, const float* w_hh,
-                        const float* seq, const float* gates, const float* cs, const float* dseq, const float* dhT,
-                        const float* dcT, float* dgates_ws, float* dh0, float* dc0, float* dW_ih, float* dW_hh,
-                        float* db_ih, float* db_hh, float* dx, int B, int T, int F, unsigned long long stream) {
-  if (!b200dp_lstm_rec_supported(LH, F)) return lfail("unsupported LSTM shape");
+// Backward of one layer + all its parameter gradients.  seq / dseq [B][T][256 * ndir] as in the forward (dseq
+// may be null); dx [B][T][F] or null; with two directions dx is the sum of both.  `dir_ptrs` holds BW_NPTR
+// pointers per direction in the order of the BW_* enum (dhT/dcT/dh0/dc0 may be null).  dW_hh [1024][256] must be
+// ZERO on entry (split-K atomics); dW_ih / db_ih / db_hh are overwritten.
+int b200dp_lstm_rec_bwd(const float* x, const float* seq, const float* dseq, float* dx, const void* const* dir_ptrs,
+                        int ndir, int B, int T, int F, unsigned long long stream) {
+  if (check_shape(ndir, B, T, F)) return -1;
   cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
-  RecBwdParams p{w_hh, gates, cs, c0, dseq, dhT, dcT, dgates_ws, dh0, dc0, B, T};
-  const int tiles = (B + NB - 1) / NB;
-  int clusters = sms() / CL;
-  if (clusters > tiles) clusters = tiles;
-  if (clusters < 1) clusters = 1;
-  if (launch_cluster(lstm_rec_bwd_kernel, p, clusters, BW_SMEM, st)) return -1;
-  WgParams w{dgates_ws, seq, h0, x, w_ih, dW_hh, dW_ih, db_ih, db_hh, dx, B, T, F, 4};
   const int TB = T * B;
-  if (TB < 256) w.ksplit = 2;
-  const int blocks = (LG / WG_TR) * (LH / WG_TK) * w.ksplit + LG / 8 + (dx != nullptr ? (TB + 7) / 8 : 0);
-  lstm_wgrad_kernel<<<blocks, 256, 0, st>>>(w);
+  RecBwdLaunch L{};
+  WgParams w[2] = {};
+  IhDir ih[2] = {};
+  L.ndir = ndir; L.B = B; L.T = T; L.ld = LH * ndir;
+  const bool ih_simt = F <= XPROJ_SIMT_MAX_F;
+  const bool dx_simt = ih_simt && ndir == 1 && dx != nullptr;
+  for (int d = 0; d < ndir; ++d) {
+    const float* const* v = reinterpret_cast<const float* const*>(dir_ptrs) + d * BW_NPTR;
+    float* dG = const_cast<float*>(v[BW_DGATES]);
+    L.d[d] = RecBwdParams{v[BW_W_HH], v[BW_GATES], v[BW_CS], v[BW_C0], dseq != nullptr ? dseq + d * LH : nullptr,
+                          v[BW_DHT], v[BW_DCT], dG, const_cast<float*>(v[BW_DH0]), const_cast<float*>(v[BW_DC0]), d};
+    w[d] = WgParams{dG, seq + d * LH, v[BW_H0], x, v[BW_W_IH], const_cast<float*>(v[BW_DW_HH]),
+                    const_cast<float*>(v[BW_DW_IH]), const_cast<float*>(v[BW_DB_IH]), const_cast<float*>(v[BW_DB_HH]),
+                    dx_simt ? dx : nullptr, B, T, F, TB < 256 ? 2 : 4, LH * ndir, d};
+    ih[d] = IhDir{v[BW_W_IH], nullptr, nullptr, nullptr, dG, const_cast<float*>(v[BW_DW_IH]),
+                  const_cast<float*>(v[BW_DB_IH]), const_cast<float*>(v[BW_DB_HH])};
+  }
+  if (launch_cluster(lstm_rec_bwd_kernel, L, cluster_split(B, ndir) * ndir, BW_SMEM, st)) return -1;
+  const int blocks = (LG / WG_TR) * (LH / WG_TK) * w[0].ksplit + (ih_simt ? LG / 8 : 0) + (dx_simt ? (TB + 7) / 8 : 0);
+  for (int d = 0; d < ndir; ++d) lstm_wgrad_kernel<<<blocks, 256, 0, st>>>(w[d]);
+  if (!ih_simt && launch_ih_wgrad(InMmaArgs{ih[0], ih[ndir - 1], x, nullptr, B, T, F, ndir, 1, 0}, st)) return -1;
+  if (dx != nullptr && !dx_simt) {
+    const InMmaArgs a{ih[0], ih[ndir - 1], x, dx, B, T, F, ndir, 1, 0};
+    lstm_in_mma_kernel<MODE_DX><<<dim3((TB + IM - 1) / IM, (F + IN - 1) / IN), 128, 0, st>>>(a);
+  }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return lfail(cudaGetErrorString(e), (int)e);
   return 0;

@@ -91,24 +91,32 @@ def available(model, x: torch.Tensor) -> bool:
 _warned_cudnn = False
 
 
-def forward(model, x, hidden):
-    """Persistent recurrence kernel (K5, ops/lstm_rec.py; cuDNN only for shapes it does not cover)
-    + fused head (K6)."""
+def recurrence(model, x, hidden):
+    """The model's nn.LSTM on the persistent recurrence kernels (K5, ops/lstm_rec.py) for every shape they
+    cover; cuDNN only for the others (hidden size != 256, > 512 input features, dropout, projections,
+    non-fp32 weights)."""
     from . import lstm_rec
     lstm = model.lstm
-    if model.n_layers == 1 and lstm_rec.supported(x, lstm.weight_hh_l0):
-        seq, model.hidden = lstm_rec.lstm_recurrent(x, hidden[0], hidden[1], lstm.weight_ih_l0,
-                                                    lstm.weight_hh_l0, lstm.bias_ih_l0, lstm.bias_hh_l0)
-    else:
-        global _warned_cudnn
-        if not _warned_cudnn:
-            _warned_cudnn = True
-            import logging
-            logging.getLogger("b200dp").warning(
-                "LSTM shape (layers=%d, hidden=%d, features=%d, bidirectional=%s) is outside the persistent "
-                "recurrence kernel (1 layer, H=256, F<=32): using the cuDNN RNN for this module",
-                model.n_layers, model.h_size, model.n_features, model.directions == 2)
-        seq, model.hidden = lstm(x, hidden)
+    if lstm_rec.stack_supported(lstm, x):
+        return lstm_rec.lstm_stack(x, hidden[0], hidden[1], [w for ws in lstm.all_weights for w in ws],
+                                   lstm.num_layers, lstm.bidirectional)
+    global _warned_cudnn
+    if not _warned_cudnn:
+        _warned_cudnn = True
+        import logging
+        logging.getLogger("b200dp").warning(
+            "LSTM shape (layers=%d, hidden=%d, features=%d, bidirectional=%s, dropout=%g, proj_size=%d, "
+            "dtype=%s) is outside the persistent recurrence kernels (hidden size 256, 1..512 features, fp32, "
+            "no dropout or projection): using the cuDNN RNN for this module",
+            model.n_layers, model.h_size, model.n_features, model.directions == 2, lstm.dropout,
+            getattr(lstm, "proj_size", 0), lstm.weight_hh_l0.dtype)
+    return lstm(x, hidden)
+
+
+def forward(model, x, hidden):
+    """Persistent recurrence kernels (K5, ops/lstm_rec.py; cuDNN only for shapes they do not cover)
+    + fused head (K6)."""
+    seq, model.hidden = recurrence(model, x, hidden)
     if not seq.is_contiguous():
         seq = seq.contiguous()
     return _HeadFn.apply(seq, model.window_size - 1, model.linear.weight, model.linear.bias,

@@ -1,11 +1,20 @@
 """K5 — persistent LSTM recurrence binding (csrc/lstm_rec_sm90.cu).
 
-``lstm_recurrent(x, h0, c0, w_ih, w_hh, b_ih, b_hh) -> (seq, (hT, cT))`` is a drop-in for a
-single-layer unidirectional ``nn.LSTM(batch_first=True)`` call with hidden size 256 (the reference
-model, reference app/torch_train.py:121-122,195) in fp32: forward = x-projection kernel + ONE
-cluster kernel for all timesteps, backward = ONE cluster kernel + ONE gradient kernel.  Weight
-gradients go straight into the gradient-bucket slots when the parameters carry a grad sink
-(ops/grad_sink.py).  cuDNN is not involved.
+``lstm_stack(x, h0, c0, weights, num_layers, bidirectional) -> (seq, (h_n, c_n))`` has the semantics of
+``nn.LSTM(batch_first=True)`` with hidden size 256 in fp32, for any number of layers, one or two
+directions and 1..512 input features: ``weights`` are the module's parameters in ``nn.LSTM`` order
+(``lstm.all_weights`` flattened), ``h0``/``c0`` are ``[layers * directions, B, 256]`` and ``seq`` is
+``[B, T, directions * 256]``.  Per layer, forward = x-projection kernel(s) + ONE cluster kernel that runs
+both directions as separate clusters of the same launch; backward = ONE cluster kernel + the gradient
+kernels, the last of which writes ``dx``, i.e. the ``dseq`` of the layer below.  The directions write their
+halves of ``seq`` / ``dseq`` and their slices of ``h_n``/``c_n``/``dh0``/``dc0`` in place.
+
+``lstm_recurrent(x, h0, c0, w_ih, w_hh, b_ih, b_hh) -> (seq, (hT, cT))`` is the one-layer unidirectional
+case (the reference model, reference app/torch_train.py:121-122,195).
+
+Weight gradients go straight into the gradient-bucket slots when the parameters carry a grad sink
+(ops/grad_sink.py).  cuDNN is not involved.  Nothing synchronises with the host and every workspace comes
+from the caching allocator, so the whole path can be captured in a CUDA graph.
 """
 from __future__ import annotations
 
@@ -18,6 +27,9 @@ from . import grad_sink
 
 _lib = None
 
+H = 256
+_SIMT_MAX_F = 32            # inputs up to this width use the register-array x-projection / dW_ih kernels
+
 
 def register(lib, have):
     global _lib
@@ -25,8 +37,8 @@ def register(lib, have):
         return
     _lib = lib
     vp, i, u64 = ctypes.c_void_p, ctypes.c_int, ctypes.c_uint64
-    lib.b200dp_lstm_rec_fwd.argtypes = [vp] * 13 + [i, i, i, u64]
-    lib.b200dp_lstm_rec_bwd.argtypes = [vp] * 19 + [i, i, i, u64]
+    lib.b200dp_lstm_rec_fwd.argtypes = [vp, vp, vp, i, i, i, i, u64]
+    lib.b200dp_lstm_rec_bwd.argtypes = [vp, vp, vp, vp, vp, i, i, i, i, u64]
     lib.b200dp_lstm_rec_supported.argtypes = [i, i]
     lib.b200dp_lstm_rec_last_error.restype = ctypes.c_char_p
     have["lstm_recurrent"] = True
@@ -39,86 +51,144 @@ def _ck(rc):
 
 def supported(x: torch.Tensor, w_hh: torch.Tensor) -> bool:
     return (_lib is not None and x.is_cuda and x.dtype == torch.float32 and w_hh.dtype == torch.float32
-            and x.dim() == 3 and w_hh.shape[1] == 256 and w_hh.shape[0] == 1024
-            and bool(_lib.b200dp_lstm_rec_supported(256, x.shape[2])))
+            and x.dim() == 3 and w_hh.shape[1] == H and w_hh.shape[0] == 4 * H
+            and bool(_lib.b200dp_lstm_rec_supported(H, x.shape[2])))
+
+
+def stack_supported(lstm: torch.nn.LSTM, x: torch.Tensor) -> bool:
+    """Whether ``lstm(x, (h0, c0))`` can run on the kernels: hidden size 256, fp32, batch_first, biases,
+    1..512 input features, no dropout and no projection."""
+    return (isinstance(lstm, torch.nn.LSTM) and lstm.hidden_size == H and lstm.batch_first and lstm.bias
+            and lstm.dropout == 0 and getattr(lstm, "proj_size", 0) == 0 and x.dim() == 3
+            and x.shape[2] == lstm.input_size and x.shape[0] >= 1 and x.shape[1] >= 1
+            and all(p.dtype == torch.float32 for p in lstm.parameters())
+            and supported(x, lstm.weight_hh_l0))
 
 
 def _p(t):
     return t.data_ptr() if t is not None else None
 
 
-class _LSTMRecFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, x, h0, c0, w_ih, w_hh, b_ih, b_hh):
-        B, T, F = x.shape
-        H = w_hh.shape[1]
-        dev = x.device
-        x = x.contiguous()
-        h0 = h0.reshape(B, H).contiguous()
-        c0 = c0.reshape(B, H).contiguous()
-        need = any(ctx.needs_input_grad)
-        seq = torch.empty((B, T, H), dtype=torch.float32, device=dev)
-        hT = torch.empty((B, H), dtype=torch.float32, device=dev)
-        cT = torch.empty((B, H), dtype=torch.float32, device=dev)
-        xp = torch.empty((T, B, 4 * H), dtype=torch.float32, device=dev)
-        gates = torch.empty((T, B, 4 * H), dtype=torch.float32, device=dev) if need else None
-        cs = torch.empty((T, B, H), dtype=torch.float32, device=dev) if need else None
-        st = torch.cuda.current_stream(dev).cuda_stream
-        _ck(_lib.b200dp_lstm_rec_fwd(x.data_ptr(), h0.data_ptr(), c0.data_ptr(), w_ih.data_ptr(),
-                                     w_hh.data_ptr(), b_ih.data_ptr(), b_hh.data_ptr(), xp.data_ptr(),
-                                     seq.data_ptr(), hT.data_ptr(), cT.data_ptr(), _p(gates), _p(cs),
-                                     B, T, F, st))
-        counters.bump("lstm_rec_fwd", 2)
-        if need:
-            ctx.save_for_backward(x, h0, c0, w_ih, w_hh, seq, gates, cs)
-            ctx.params = (w_ih, w_hh, b_ih, b_hh)
-            for prm, ng in zip(ctx.params, ctx.needs_input_grad[3:]):
-                if ng:
-                    grad_sink.note_forward(prm)
-        return seq, hT.view(1, B, H), cT.view(1, B, H)
+def _ptr_array(tensors):
+    return (ctypes.c_void_p * len(tensors))(*[_p(t) for t in tensors])
+
+
+class _LSTMStackFn(torch.autograd.Function):
+    """One node for the whole stack.  ``weights``: 4 tensors (w_ih, w_hh, b_ih, b_hh) per (layer, direction),
+    in nn.LSTM order."""
 
     @staticmethod
-    def backward(ctx, dseq, dhT, dcT):
-        x, h0, c0, w_ih, w_hh, seq, gates, cs = ctx.saved_tensors
-        B, T, F = x.shape
-        H = w_hh.shape[1]
+    def forward(ctx, L, D, x, h0, c0, *weights):
+        B, T, _ = x.shape
         dev = x.device
-        dseq = dseq.contiguous() if dseq is not None else None
-        dhT = dhT.reshape(B, H).contiguous() if dhT is not None else None
-        dcT = dcT.reshape(B, H).contiguous() if dcT is not None else None
-        dG = torch.empty((T, B, 4 * H), dtype=torch.float32, device=dev)
-        ni = ctx.needs_input_grad
-        dh0 = torch.empty((B, H), dtype=torch.float32, device=dev) if ni[1] else None
-        dc0 = torch.empty((B, H), dtype=torch.float32, device=dev) if ni[2] else None
-        dx = torch.empty_like(x) if ni[0] else None
-        # parameter gradients: into the gradient buckets when possible (first pass of the step only:
-        # the kernels overwrite / atomically add onto zero)
-        sinks = [grad_sink.begin(prm) for prm in ctx.params]
-        direct = all(s[0] is not None and not s[1] for s in sinks) and \
-            all(s[0].is_contiguous() for s in sinks)
-        if direct:
-            dW_ih, dW_hh, db_ih, db_hh = [s[0] for s in sinks]
-            dW_hh.zero_()
-        else:
-            dW_ih = torch.empty_like(w_ih)
-            dW_hh = torch.zeros_like(w_hh)
-            db_ih = torch.empty(4 * H, dtype=torch.float32, device=dev)
-            db_hh = torch.empty(4 * H, dtype=torch.float32, device=dev)
+        x = x.contiguous()
+        h0_shape, c0_shape = h0.shape, c0.shape
+        h0 = h0.reshape(L * D, B, H).contiguous()
+        c0 = c0.reshape(L * D, B, H).contiguous()
+        need = any(ctx.needs_input_grad)
+        hN = torch.empty((L * D, B, H), dtype=torch.float32, device=dev)
+        cN = torch.empty((L * D, B, H), dtype=torch.float32, device=dev)
         st = torch.cuda.current_stream(dev).cuda_stream
-        _ck(_lib.b200dp_lstm_rec_bwd(x.data_ptr(), h0.data_ptr(), c0.data_ptr(), w_ih.data_ptr(),
-                                     w_hh.data_ptr(), seq.data_ptr(), gates.data_ptr(), cs.data_ptr(),
-                                     _p(dseq), _p(dhT), _p(dcT), dG.data_ptr(), _p(dh0), _p(dc0),
-                                     dW_ih.data_ptr(), dW_hh.data_ptr(), db_ih.data_ptr(), db_hh.data_ptr(),
-                                     _p(dx), B, T, F, st))
-        counters.bump("lstm_rec_bwd", 2)
-        if direct:
-            for s in sinks:
-                s[2]()
-            dW_ih = dW_hh = db_ih = db_hh = None
-        return (dx, dh0.view(1, B, H) if dh0 is not None else None,
-                dc0.view(1, B, H) if dc0 is not None else None, dW_ih, dW_hh, db_ih, db_hh)
+        inp, seqs, gates, cs = x, [], [], []
+        for l in range(L):
+            F = inp.shape[2]
+            seq = torch.empty((B, T, D * H), dtype=torch.float32, device=dev)
+            ptrs, g_l, c_l = [], [], []
+            for d in range(D):
+                i = l * D + d
+                w_ih, w_hh, b_ih, b_hh = weights[4 * i:4 * i + 4]
+                xp = torch.empty((T, B, 4 * H), dtype=torch.float32, device=dev)
+                g = torch.empty((T, B, 4 * H), dtype=torch.float32, device=dev) if need else None
+                c = torch.empty((T, B, H), dtype=torch.float32, device=dev) if need else None
+                g_l.append(g)
+                c_l.append(c)
+                # per-direction pointer group, in the order of the FW_* enum of csrc/lstm_rec_sm90.cu
+                ptrs += [w_ih, w_hh, b_ih, b_hh, h0[i], c0[i], xp, g, c, hN[i], cN[i]]
+            _ck(_lib.b200dp_lstm_rec_fwd(inp.data_ptr(), seq.data_ptr(), _ptr_array(ptrs), D, B, T, F, st))
+            counters.bump("lstm_rec_fwd", (D if F <= _SIMT_MAX_F else 1) + 1)
+            seqs.append(seq)
+            gates.append(g_l)
+            cs.append(c_l)
+            inp = seq
+        if need:
+            ctx.save_for_backward(x, h0, c0, *seqs, *[t for g_l in gates for t in g_l],
+                                  *[t for c_l in cs for t in c_l], *weights)
+            ctx.L, ctx.D, ctx.h0_shape, ctx.c0_shape = L, D, h0_shape, c0_shape
+            for prm, ng in zip(weights, ctx.needs_input_grad[5:]):
+                if ng:
+                    grad_sink.note_forward(prm)
+        return seqs[-1], hN, cN
+
+    @staticmethod
+    def backward(ctx, dseq, dhN, dcN):
+        L, D = ctx.L, ctx.D
+        saved = ctx.saved_tensors
+        x, h0, c0 = saved[:3]
+        seqs = saved[3:3 + L]
+        gates = saved[3 + L:3 + L + L * D]
+        cs = saved[3 + L + L * D:3 + L + 2 * L * D]
+        weights = saved[3 + L + 2 * L * D:]
+        B, T, _ = x.shape
+        dev = x.device
+        ni = ctx.needs_input_grad
+        dcur = dseq.contiguous() if dseq is not None else None
+        dhN = dhN.contiguous() if dhN is not None else None
+        dcN = dcN.contiguous() if dcN is not None else None
+        dh0 = torch.empty((L * D, B, H), dtype=torch.float32, device=dev) if ni[3] else None
+        dc0 = torch.empty((L * D, B, H), dtype=torch.float32, device=dev) if ni[4] else None
+        grads = [None] * len(weights)
+        st = torch.cuda.current_stream(dev).cuda_stream
+        for l in reversed(range(L)):
+            inp = x if l == 0 else seqs[l - 1]
+            F = inp.shape[2]
+            dx = torch.empty_like(inp) if (l > 0 or ni[2]) else None
+            ptrs, fire = [], []
+            for d in range(D):
+                i = l * D + d
+                prm = weights[4 * i:4 * i + 4]
+                # parameter gradients: into the gradient buckets when possible (first pass of the step only:
+                # the kernels overwrite / atomically add onto zero)
+                sinks = [grad_sink.begin(p) for p in prm]
+                if all(s[0] is not None and not s[1] and s[0].is_contiguous() for s in sinks):
+                    dW_ih, dW_hh, db_ih, db_hh = [s[0] for s in sinks]
+                    dW_hh.zero_()
+                    fire += [s[2] for s in sinks]
+                else:
+                    dW_ih = torch.empty_like(prm[0])
+                    dW_hh = torch.zeros_like(prm[1])
+                    db_ih = torch.empty(4 * H, dtype=torch.float32, device=dev)
+                    db_hh = torch.empty(4 * H, dtype=torch.float32, device=dev)
+                    grads[4 * i:4 * i + 4] = [dW_ih, dW_hh, db_ih, db_hh]
+                dG = torch.empty((T, B, 4 * H), dtype=torch.float32, device=dev)
+                # per-direction pointer group, in the order of the BW_* enum of csrc/lstm_rec_sm90.cu
+                ptrs += [prm[0], prm[1], h0[i], c0[i], gates[i], cs[i],
+                         dhN[i] if dhN is not None else None, dcN[i] if dcN is not None else None, dG,
+                         dh0[i] if dh0 is not None else None, dc0[i] if dc0 is not None else None,
+                         dW_ih, dW_hh, db_ih, db_hh]
+            _ck(_lib.b200dp_lstm_rec_bwd(inp.data_ptr(), seqs[l].data_ptr(), _p(dcur), _p(dx), _ptr_array(ptrs),
+                                         D, B, T, F, st))
+            simt = F <= _SIMT_MAX_F
+            counters.bump("lstm_rec_bwd", 1 + D + (0 if simt else 2) + (1 if dx is not None and not (simt and D == 1)
+                                                                        else 0))
+            for f in fire:
+                f()
+            dcur = dx
+        return (None, None, dcur if ni[2] else None,
+                dh0.view(ctx.h0_shape) if dh0 is not None else None,
+                dc0.view(ctx.c0_shape) if dc0 is not None else None, *grads)
+
+
+def lstm_stack(x, h0, c0, weights, num_layers: int, bidirectional: bool):
+    """``nn.LSTM(batch_first=True)`` forward on the K5 kernels (see the module docstring)."""
+    D = 2 if bidirectional else 1
+    weights = list(weights)
+    if len(weights) != 4 * num_layers * D:
+        raise ValueError(f"expected {4 * num_layers * D} weight tensors (w_ih, w_hh, b_ih, b_hh per layer and "
+                         f"direction), got {len(weights)}")
+    seq, hN, cN = _LSTMStackFn.apply(num_layers, D, x, h0, c0, *weights)
+    return seq, (hN, cN)
 
 
 def lstm_recurrent(x, h0, c0, w_ih, w_hh, b_ih, b_hh):
-    seq, hT, cT = _LSTMRecFn.apply(x, h0, c0, w_ih, w_hh, b_ih, b_hh)
+    seq, hT, cT = _LSTMStackFn.apply(1, 1, x, h0, c0, w_ih, w_hh, b_ih, b_hh)
     return seq, (hT, cT)

@@ -56,5 +56,8 @@ from distributed_torch_horovod_gcp_b200.models import LSTM
 m = LSTM(23, 20, 1, 256, device=torch.device(dev)).to(dev)
 xs = torch.randn(8, 20, 23, device=dev)
 m(xs).sum().backward()
+# stacked bidirectional: reverse direction, strided halves of seq, F > 32 input products with a tail
+m2 = LSTM(40, 5, 1, 256, n_layers=2, bidirectional=True, device=torch.device(dev)).to(dev)
+m2(torch.randn(7, 5, 40, device=dev)).sum().backward()
 torch.cuda.synchronize()
 print("all ok")
