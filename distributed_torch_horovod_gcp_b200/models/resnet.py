@@ -60,19 +60,7 @@ class Bottleneck(nn.Module):
         self.stride = stride
 
     def forward(self, x):
-        # The block input feeds conv1 AND the skip branch: instead of autograd summing two activation-sized
-        # gradients with a stand-alone add, the skip gradient is parked in a GradBox and conv1's dgrad
-        # epilogue adds it (identity block: bn3's unmasked dy + the ReLU sign bits; projection block: the
-        # downsample conv's dgrad, while bn3 hands its sign bits to the downsample BN through a second box).
-        box = F2.new_grad_box(x)
-        out = F2.conv_bn_act(x, self.conv1, self.bn1, relu=True, input_box=box)
-        out = F2.conv_bn_act(out, self.conv2, self.bn2, relu=True)
-        if self.downsample is None:
-            return F2.conv_bn_act(out, self.conv3, self.bn3, relu=True, residual=x, skip_box=box)
-        mbox = F2.new_grad_box(x)
-        identity = F2.conv_bn_act(x, self.downsample[0], self.downsample[1], relu=False, park_box=box,
-                                  skip_box=mbox)
-        return F2.conv_bn_act(out, self.conv3, self.bn3, relu=True, residual=identity, skip_box=mbox)
+        return F2.bottleneck(x, self)
 
 
 class ResNet(nn.Module):

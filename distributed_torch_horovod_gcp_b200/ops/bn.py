@@ -70,114 +70,110 @@ def bn_supported(x: torch.Tensor, C: int) -> bool:
     return _lib is not None and _nhwc_ok(x) and bool(_lib.b200dp_bn_supported(C))
 
 
+def _cl(t: torch.Tensor) -> torch.Tensor:
+    return t if t.is_contiguous(memory_format=torch.channels_last) else t.contiguous(memory_format=torch.channels_last)
+
+
+def bn_forward(x, bn: torch.nn.BatchNorm2d, residual, relu: bool, stats_in=None, grads=(True, True)):
+    """Training-mode BN(+residual)(+ReLU) of an NHWC bf16 ``x``; updates the running statistics and
+    ``num_batches_tracked``.  ``stats_in``: the per-channel sums of ``x`` accumulated by the producing GEMM /
+    conv epilogue (persistent buffer).  ``grads``: whether γ and β need gradients (their grad sinks count
+    this use).  Returns ``(y, mask, ws)``: the ReLU sign bits (None without ReLU) and the per-channel
+    ``(mean, invstd, a)`` that ``bn_backward`` reads."""
+    N, C, H, W = x.shape
+    M = N * H * W
+    dev = x.device
+    gamma, beta = bn.weight, bn.bias
+    nbt = bn.num_batches_tracked if (bn.track_running_stats and bn.num_batches_tracked is not None
+                                     and bn.num_batches_tracked.is_cuda) else None   # += 1 inside bn_finalize
+    mom = bn.momentum if bn.momentum is not None else 0.1
+    y = torch.empty_like(x, memory_format=torch.channels_last)
+    ws = torch.empty(6 * C, dtype=torch.float32, device=dev)
+    stats, mean, invstd, a, b = ws[:2 * C], ws[2 * C:3 * C], ws[3 * C:4 * C], ws[4 * C:5 * C], ws[5 * C:]
+    if stats_in is not None:
+        stats = stats_in
+    pbf16 = int(gamma.dtype == torch.bfloat16)
+    # ReLU sign bits, 1 byte per 8 channels: the backward reads 1/16th of what y would cost
+    mask = torch.empty(M * (C // 8), dtype=torch.uint8, device=dev) if relu else None
+    st = torch.cuda.current_stream(dev).cuda_stream
+    _ck(_lib.b200dp_bn_fwd(x.data_ptr(), residual.data_ptr() if residual is not None else None,
+                           y.data_ptr(), gamma.data_ptr(), beta.data_ptr(), stats.data_ptr(),
+                           mean.data_ptr(), invstd.data_ptr(), a.data_ptr(), b.data_ptr(),
+                           bn.running_mean.data_ptr() if bn.running_mean is not None else None,
+                           bn.running_var.data_ptr() if bn.running_var is not None else None,
+                           M, C, float(bn.eps), float(mom), int(relu), pbf16,
+                           2 if stats_in is not None else 0,
+                           mask.data_ptr() if mask is not None else None,
+                           nbt.data_ptr() if nbt is not None else None, st))
+    counters.bump("bn_fwd", 2 if stats_in is not None else 3)
+    if grads[0]:
+        grad_sink.note_forward(gamma)
+    if grads[1]:
+        grad_sink.note_forward(beta)
+    return y, mask, (mean, invstd, a)
+
+
+def bn_backward(dy, bn: torch.nn.BatchNorm2d, x, mask, ws, write_dres: bool = False):
+    """Backward of ``bn_forward`` for a channels_last ``dy``.  ``mask``: ReLU sign bits applied to ``dy``
+    (None: no ReLU).  ``write_dres``: also write the masked ``dy``, the gradient of the residual input.
+    Returns ``(dx, dgamma, dbeta, dres)``; dgamma and dbeta are None when they went straight into the
+    gradient buckets."""
+    mean, invstd, a = ws
+    N, C, H, W = x.shape
+    M = N * H * W
+    dx = torch.empty_like(x, memory_format=torch.channels_last)
+    dres = torch.empty_like(x, memory_format=torch.channels_last) if write_dres else None
+    sums = torch.empty(2 * C, dtype=torch.float32, device=x.device)
+    # dgamma / dbeta: straight into the gradient-bucket slots when both parameters offer a sink
+    gamma, beta = bn.weight, bn.bias
+    gd, ga, gdone = grad_sink.begin(gamma)
+    bd, ba, bdone = grad_sink.begin(beta)
+    direct = gd is not None and bd is not None and not ga and not ba
+    if direct:
+        dg_ptr, db_ptr = gd.data_ptr(), bd.data_ptr()
+    else:
+        dgb = torch.empty(2 * C, dtype=gamma.dtype, device=x.device)
+        dg_ptr, db_ptr = dgb.data_ptr(), dgb.data_ptr() + C * dgb.element_size()
+    st = torch.cuda.current_stream(x.device).cuda_stream
+    _ck(_lib.b200dp_bn_bwd(dy.data_ptr(), x.data_ptr(), mask.data_ptr() if mask is not None else None,
+                           dx.data_ptr(), dres.data_ptr() if dres is not None else None,
+                           a.data_ptr(), mean.data_ptr(), invstd.data_ptr(), sums.data_ptr(),
+                           dg_ptr, db_ptr,
+                           int(gamma.dtype == torch.bfloat16), M, C, int(mask is not None), st))
+    counters.bump("bn_bwd", 2)
+    if direct:
+        gdone()
+        bdone()
+        return dx, None, None, dres
+    return dx, dgb[:C], dgb[C:], dres                   # written by the kernel in the param dtype
+
+
 class _BNActFn(torch.autograd.Function):
     """Training-mode BN over NHWC bf16 with fused residual add and ReLU."""
 
     @staticmethod
-    def forward(ctx, x, gamma, beta, running_mean, running_var, residual, relu, eps, momentum,
-                stats_in=None, box=None, nbt=None):
-        N, C, H, W = x.shape
-        M = N * H * W
-        dev = x.device
-        y = torch.empty_like(x, memory_format=torch.channels_last)
-        ws = torch.empty(6 * C, dtype=torch.float32, device=dev)
-        stats, mean, invstd, a, b = ws[:2 * C], ws[2 * C:3 * C], ws[3 * C:4 * C], ws[4 * C:5 * C], ws[5 * C:]
-        if stats_in is not None:
-            stats = stats_in              # accumulated by the producing GEMM / conv epilogue (persistent buffer)
-        pbf16 = int(gamma.dtype == torch.bfloat16)
-        # ReLU sign bits, 1 byte per 8 channels: the backward reads 1/16th of what y would cost
-        mask = torch.empty(M * (C // 8), dtype=torch.uint8, device=dev) if relu else None
-        st = torch.cuda.current_stream(dev).cuda_stream
-        _ck(_lib.b200dp_bn_fwd(x.data_ptr(), residual.data_ptr() if residual is not None else None,
-                               y.data_ptr(), gamma.data_ptr(), beta.data_ptr(), stats.data_ptr(),
-                               mean.data_ptr(), invstd.data_ptr(), a.data_ptr(), b.data_ptr(),
-                               running_mean.data_ptr() if running_mean is not None else None,
-                               running_var.data_ptr() if running_var is not None else None,
-                               M, C, float(eps), float(momentum), int(relu), pbf16,
-                               2 if stats_in is not None else 0,
-                               mask.data_ptr() if mask is not None else None,
-                               nbt.data_ptr() if nbt is not None else None, st))
-        counters.bump("bn_fwd", 2 if stats_in is not None else 3)
-        ctx.save_for_backward(x, mask, mean, invstd, a)
-        ctx.relu, ctx.has_res, ctx.pdtype = relu, residual is not None, gamma.dtype
-        ctx.affine = (gamma, beta)
-        ctx.box = box
-        if box is not None and residual is None and not relu and ctx.needs_input_grad[0]:
-            box.armed = box.want_mask = True      # consumer role (see backward)
-        if ctx.needs_input_grad[1]:
-            grad_sink.note_forward(gamma)
-        if ctx.needs_input_grad[2]:
-            grad_sink.note_forward(beta)
+    def forward(ctx, x, gamma, beta, residual, relu, stats_in, bn):
+        y, mask, ws = bn_forward(x, bn, residual, relu, stats_in, ctx.needs_input_grad[1:3])
+        ctx.save_for_backward(x, mask, *ws)
+        ctx.bn, ctx.has_res = bn, residual is not None
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        x, mask, mean, invstd, a = ctx.saved_tensors
-        N, C, H, W = x.shape
-        M = N * H * W
-        if not dy.is_contiguous(memory_format=torch.channels_last):
-            dy = dy.contiguous(memory_format=torch.channels_last)
-        dx = torch.empty_like(x, memory_format=torch.channels_last)
-        box = ctx.box
-        relu = ctx.relu
-        if box is not None and not ctx.has_res and not relu and box.ext_mask is not None:
-            # downsample BN of a projection block: ``dy`` is the block-output gradient BEFORE the block's
-            # final ReLU mask, whose sign bits the block's BN+add+ReLU backward left in the box
-            ext_mask, box.ext_mask = box.ext_mask, None
-            assert ext_mask.numel() == M * (C // 8)
-            mask, relu = ext_mask, True
-        # the masked skip gradient is only materialised when nobody downstream applies the sign bits itself
-        hand_off = ctx.has_res and ctx.relu and box is not None and box.armed and not box.consumed
-        dres = torch.empty_like(x, memory_format=torch.channels_last) if (ctx.has_res and ctx.relu and not hand_off) \
-            else None
-        sums = torch.empty(2 * C, dtype=torch.float32, device=x.device)
-        # dgamma / dbeta: straight into the gradient-bucket slots when both parameters offer a sink
-        gamma, beta = ctx.affine
-        gd, ga, gdone = grad_sink.begin(gamma)
-        bd, ba, bdone = grad_sink.begin(beta)
-        direct = gd is not None and bd is not None and not ga and not ba
-        if direct:
-            dg_ptr, db_ptr = gd.data_ptr(), bd.data_ptr()
-        else:
-            dgb = torch.empty(2 * C, dtype=ctx.pdtype, device=x.device)
-            dg_ptr, db_ptr = dgb.data_ptr(), dgb.data_ptr() + C * dgb.element_size()
-        st = torch.cuda.current_stream(x.device).cuda_stream
-        _ck(_lib.b200dp_bn_bwd(dy.data_ptr(), x.data_ptr(), mask.data_ptr() if mask is not None else None,
-                               dx.data_ptr(), dres.data_ptr() if dres is not None else None,
-                               a.data_ptr(), mean.data_ptr(), invstd.data_ptr(), sums.data_ptr(),
-                               dg_ptr, db_ptr,
-                               int(ctx.pdtype == torch.bfloat16), M, C, int(relu), st))
-        counters.bump("bn_bwd", 2)
-        if direct:
-            dgamma = dbeta = None
-            gdone()
-            bdone()
-        else:
-            dgamma, dbeta = dgb[:C], dgb[C:]              # written by the kernel in the param dtype
-        if hand_off:
-            if box.want_mask:
-                box.ext_mask = mask         # projection block: the downsample BN backward masks dy itself
-                dres = dy
-            else:
-                box.park(dy, mask)          # identity block: conv1's dgrad epilogue adds mask(dy)
-                dres = None
-        elif ctx.has_res and dres is None:
+        x, mask, *ws = ctx.saved_tensors
+        dy = _cl(dy)
+        dx, dgamma, dbeta, dres = bn_backward(dy, ctx.bn, x, mask, ws, write_dres=ctx.has_res and mask is not None)
+        if ctx.has_res and dres is None:
             dres = dy                       # no ReLU: the residual branch gets dy unchanged
-            if box is not None and not box.want_mask and box.park(dres):
-                dres = None
-        return dx, dgamma, dbeta, None, None, dres, None, None, None, None, None, None
+        return dx, dgamma, dbeta, dres, None, None, None
 
 
 def bn_act(x, bn: torch.nn.BatchNorm2d, relu: bool, residual: Optional[torch.Tensor] = None,
-           stats: Optional[torch.Tensor] = None, box=None):
-    if residual is not None and not residual.is_contiguous(memory_format=torch.channels_last):
-        residual = residual.contiguous(memory_format=torch.channels_last)
+           stats: Optional[torch.Tensor] = None):
+    if residual is not None:
+        residual = _cl(residual)
     if bn.training:
-        nbt = bn.num_batches_tracked if (bn.track_running_stats and bn.num_batches_tracked is not None
-                                         and bn.num_batches_tracked.is_cuda) else None   # += 1 inside bn_finalize
-        mom = bn.momentum if bn.momentum is not None else 0.1
-        return _BNActFn.apply(x, bn.weight, bn.bias, bn.running_mean, bn.running_var, residual,
-                              relu, bn.eps, mom, stats, box, nbt)
+        return _BNActFn.apply(x, bn.weight, bn.bias, residual, relu, stats, bn)
     # inference: frozen statistics -> one fused apply pass
     a = (bn.weight.float() * torch.rsqrt(bn.running_var.float() + bn.eps))
     b = bn.bias.float() - bn.running_mean.float() * a
@@ -253,7 +249,7 @@ def _is_stem_conv(x, conv) -> bool:
 _FUSE_STATS = os.environ.get("B200DP_BN_STATS_IN_EPILOGUE", "1") == "1"
 
 
-def conv2d(x, conv: torch.nn.Conv2d, box=None, stats=None, park=None):
+def conv2d(x, conv: torch.nn.Conv2d, stats=None):
     """Convolution of an NHWC bf16 activation; 1x1/stride-1 and the 7x7 stem -> wgmma GEMM, 3x3 and
     strided 1x1 -> implicit-GEMM kernel.  Returns ``(y, stats_filled)``: when ``stats`` (fp32 [2*Cout]
     accumulator) is given and the kernel that ran supports it, its epilogue has added the output's
@@ -262,13 +258,13 @@ def conv2d(x, conv: torch.nn.Conv2d, box=None, stats=None, park=None):
     if _is_gemm_conv(x, conv):
         N, C, H, W = x.shape
         x2 = x.permute(0, 2, 3, 1).reshape(N * H * W, C)             # view: NHWC rows
-        y2 = _gemm.linear(x2, w.reshape(w.shape[0], C), owner=w, box=box, stats=stats, park=park)     # [M, Cout]
+        y2 = _gemm.linear(x2, w.reshape(w.shape[0], C), owner=w, stats=stats)     # [M, Cout]
         return y2.view(N, H, W, w.shape[0]).permute(0, 3, 1, 2), stats is not None   # logical NCHW, NHWC memory
     if _is_stem_conv(x, conv):
         return _StemConvFn.apply(x, w, stats), stats is not None
     from . import conv as _conv
     if conv.bias is None and _conv.supported(x, w, conv.stride, conv.padding, conv.dilation, conv.groups):
-        return _conv.conv2d(x, w, conv.stride[0], conv.padding[0], stats, park), stats is not None
+        return _conv.conv2d(x, w, conv.stride[0], conv.padding[0], stats), stats is not None
     return F.conv2d(x, w, conv.bias, conv.stride, conv.padding, conv.dilation, conv.groups), False
 
 
@@ -281,22 +277,22 @@ def _stats_buffer(bn, C: int, device):
     return buf
 
 
-def conv_bn_act(x, conv, bn, relu: bool, residual=None, skip_box=None, input_box=None, park_box=None):
-    """``input_box``: this conv consumes the block input whose skip gradient will arrive through the
-    box; ``skip_box``: this BN's residual IS that block input, or (projection block) this BN is the
-    downsample BN / the block's last BN exchanging the ReLU sign bits; ``park_box``: this conv's input
-    gradient is handed to the box's consumer instead of being returned (grad_sink.GradBox)."""
+def fused_stats(bn, C: int, device) -> Optional[torch.Tensor]:
+    """The accumulator the producing conv / GEMM epilogue fills with the batch statistics of the BatchNorm
+    that follows (no separate pass over its input), or None where that is not done."""
+    return _stats_buffer(bn, C, device) if _FUSE_STATS and bn.training and C <= 2048 else None
+
+
+def conv_bn_act(x, conv, bn, relu: bool, residual=None):
     C = conv.out_channels
     fused_bn = _lib is not None and bn.weight is not None and bool(_lib.b200dp_bn_supported(C)) and \
         (residual is None or residual.dtype == torch.bfloat16)
-    # batch statistics come out of the conv / GEMM epilogue (no separate pass over y)
-    want_stats = _FUSE_STATS and fused_bn and bn.training and C <= 2048 and x.dtype == torch.bfloat16
-    stats = _stats_buffer(bn, C, x.device) if want_stats else None
-    y, filled = conv2d(x, conv, box=input_box, stats=stats, park=park_box)
+    stats = fused_stats(bn, C, x.device) if fused_bn and x.dtype == torch.bfloat16 else None
+    y, filled = conv2d(x, conv, stats=stats)
     if stats is not None and not filled:
         stats = None
     if fused_bn and bn_supported(y, C):
-        return bn_act(y, bn, relu, residual, stats=stats, box=skip_box)
+        return bn_act(y, bn, relu, residual, stats=stats)
     if stats is not None:
         stats.zero_()          # filled but not consumed by the fused BN: keep the accumulator clean
     y = bn(y)

@@ -118,9 +118,8 @@ def conv_wgrad(dy, x, weight, stride: int, pad: int) -> Optional[torch.Tensor]:
 
 class _ConvFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, weight, stride, pad, stats=None, park=None):
+    def forward(ctx, x, weight, stride, pad, stats=None):
         w = _krsc(weight)
-        ctx.park = park if ctx.needs_input_grad[0] else None
         if ctx.needs_input_grad[1]:
             grad_sink.note_forward(weight)
         y = conv_fprop(x, w, stride, pad, stats)
@@ -137,21 +136,18 @@ class _ConvFn(torch.autograd.Function):
         dx = dw = None
         if ctx.needs_input_grad[0]:
             dx = conv_dgrad(dy, w, x.shape, ctx.stride, ctx.pad)
-            if ctx.park is not None and ctx.park.park(dx):
-                dx = None          # grad_sink.GradBox: the block's first conv adds it in its dgrad epilogue
         if ctx.needs_input_grad[1]:
             dw = conv_wgrad(dy, x, ctx.weight, ctx.stride, ctx.pad)
-        return dx, dw, None, None, None, None
+        return dx, dw, None, None, None
 
 
-def conv2d(x: torch.Tensor, weight: torch.Tensor, stride: int = 1, padding: Optional[int] = None, stats=None,
-           park=None):
+def conv2d(x: torch.Tensor, weight: torch.Tensor, stride: int = 1, padding: Optional[int] = None, stats=None):
     """``F.conv2d`` for NHWC bf16 activations on the sm_90a implicit-GEMM kernel.  ``stats`` (fp32
     [2*Cout], zero on entry): the kernel's epilogue adds the per-channel sum / sum of squares of the
     output to it — the batch statistics of the BatchNorm that follows."""
     if padding is None:
         padding = (weight.shape[2] - 1) // 2
-    return _ConvFn.apply(x, weight, int(stride), int(padding), stats, park)
+    return _ConvFn.apply(x, weight, int(stride), int(padding), stats)
 
 
 def conv3x3(x, weight, stride: int = 1):

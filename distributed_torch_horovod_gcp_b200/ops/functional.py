@@ -37,22 +37,27 @@ def conv_bn_act_reference(x, conv: nn.Conv2d, bn: nn.BatchNorm2d, relu: bool,
 
 
 def conv_bn_act(x, conv: nn.Conv2d, bn: nn.BatchNorm2d, relu: bool = True,
-                residual: Optional[torch.Tensor] = None, skip_box=None, input_box=None, park_box=None):
-    """``skip_box`` / ``input_box`` (kernel path only): see ``ops.grad_sink.GradBox`` — the block's last
-    BN parks the skip-connection gradient, the block's first conv adds it in its dgrad epilogue."""
+                residual: Optional[torch.Tensor] = None):
     k = _kernels(x)
     if k is not None and k.has("conv_bn_act"):
-        return k.conv_bn_act(x, conv, bn, relu, residual, skip_box=skip_box, input_box=input_box,
-                             park_box=park_box)
+        return k.conv_bn_act(x, conv, bn, relu, residual)
     return conv_bn_act_reference(x, conv, bn, relu, residual)
 
 
-def new_grad_box(x: torch.Tensor):
-    """A GradBox when ``x`` takes the kernel path and needs a gradient, else ``None``."""
-    if _kernels(x) is None or not x.requires_grad or not torch.is_grad_enabled():
-        return None
-    from .grad_sink import GradBox
-    return GradBox()
+def bottleneck(x, block):
+    """ResNet bottleneck block (``models.resnet.Bottleneck``).  Kernel path: one autograd node whose
+    backward adds the skip-connection gradient in conv1's dgrad epilogue (ops/bottleneck.py).  Otherwise
+    (CPU, eval mode, shapes that node does not cover) the per-op chain, where autograd adds it."""
+    k = _kernels(x)
+    if k is not None and k.has("conv_bn_act"):
+        from . import bottleneck as _bt
+        if _bt.supported(x, block):
+            return _bt.bottleneck(x, block)
+    out = conv_bn_act(x, block.conv1, block.bn1, relu=True)
+    out = conv_bn_act(out, block.conv2, block.bn2, relu=True)
+    identity = x if block.downsample is None else \
+        conv_bn_act(x, block.downsample[0], block.downsample[1], relu=False)
+    return conv_bn_act(out, block.conv3, block.bn3, relu=True, residual=identity)
 
 
 def max_pool_3x3_s2(x):

@@ -126,15 +126,24 @@ def bias_grad(dz: torch.Tensor, N: int, M: int, dtype) -> torch.Tensor:
     return acc[:, 0].to(dtype)
 
 
+def dgrad(dz: torch.Tensor, weight: torch.Tensor, residual: Optional[torch.Tensor] = None,
+          res_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """dx[M,K] = dz[M,N] @ W[N,K] (+ ``residual`` [M,K], kept only where the bits of ``res_mask`` are set:
+    ReLU sign bits, 1 byte per 8 columns)."""
+    M, (N, K) = dz.shape[0], weight.shape
+    if res_mask is not None and (K % 64):      # kernel limit: apply the sign bits here
+        bits = (res_mask.view(M, K // 8, 1) >> torch.arange(8, device=dz.device, dtype=torch.uint8)) & 1
+        residual = residual * bits.view(M, K).to(residual.dtype)
+        res_mask = None
+    dx = torch.empty((M, K), dtype=torch.bfloat16, device=dz.device)
+    return gemm(dz, weight, dx, M, K, N, b_mn=True, residual=residual, res_mask=res_mask)
+
+
 class _LinearFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, weight, bias, act, residual, owner=None, box=None, stats=None, park=None):
+    def forward(ctx, x, weight, bias, act, residual, owner=None, stats=None):
         K = weight.shape[1]
         ctx.owner = owner if owner is not None else weight
-        ctx.box = box if (box is not None and ctx.needs_input_grad[0]) else None
-        ctx.park = park if ctx.needs_input_grad[0] else None
-        if ctx.box is not None:
-            ctx.box.armed = True
         if ctx.needs_input_grad[1]:
             grad_sink.note_forward(ctx.owner)
         N = weight.shape[0]
@@ -172,30 +181,12 @@ class _LinearFn(torch.autograd.Function):
             dz = dy2
         dx = dw = db = None
         if ctx.needs_input_grad[0]:
-            dx = torch.empty((M, K), dtype=torch.bfloat16, device=dy.device)
-            skip = skip_mask = None
-            if ctx.box is not None:
-                skip, skip_mask = ctx.box.take()    # skip-connection gradient of the same block input
-            if skip is not None:
-                if skip.dim() == 4:                 # NHWC activation -> its [M, C] matrix (a view)
-                    skip = skip.permute(0, 2, 3, 1).reshape(M, K)
-                else:
-                    skip = skip.reshape(M, K)
-                if not skip.is_contiguous():
-                    skip = skip.contiguous()
-                if skip_mask is not None and (K % 64):      # kernel limit: apply the sign bits here
-                    bits = (skip_mask.view(M, K // 8, 1) >> torch.arange(8, device=skip.device, dtype=torch.uint8)) & 1
-                    skip = skip * bits.view(M, K).to(skip.dtype)
-                    skip_mask = None
-            gemm(dz, weight, dx, M, K, N, b_mn=True, residual=skip, res_mask=skip_mask)   # dx = dz @ W (+ skip)
-            dx = dx.view(ctx.x_shape)
-            if ctx.park is not None and ctx.park.park(dx):
-                dx = None                           # the block's first conv adds it in its dgrad epilogue
+            dx = dgrad(dz, weight).view(ctx.x_shape)                       # dx = dz @ W
         if ctx.needs_input_grad[1]:
             dw = wgrad(dz, x2, N, K, M, weight.dtype, owner=ctx.owner)     # dW = dz^T @ x
         if ctx.has_bias and ctx.needs_input_grad[2]:
             db = bias_grad(dz, N, M, ctx.bias_dtype)
-        return dx, dw, db, None, dres, None, None, None, None
+        return dx, dw, db, None, dres, None, None
 
 
 def act_backward(dy2: torch.Tensor, z: torch.Tensor, act: int) -> torch.Tensor:
@@ -324,10 +315,7 @@ def qkv_proj(x, weight, bias):
     return _QKVFn.apply(x, weight, bias)
 
 
-def linear(x, weight, bias=None, act: Optional[str] = None, residual=None, owner=None, box=None, stats=None,
-           park=None):
+def linear(x, weight, bias=None, act: Optional[str] = None, residual=None, owner=None, stats=None):
     """``owner``: the parameter whose storage ``weight`` is a 2D view of (a 1x1 conv weight), so the
-    weight gradient can be written into its gradient-bucket slot directly.  ``box``: a
-    ``grad_sink.GradBox`` through which a later node hands this layer the skip-connection gradient of
-    the same input (added in the dgrad epilogue)."""
-    return _LinearFn.apply(x, weight, bias, ACT[act], residual, owner, box, stats, park)
+    weight gradient can be written into its gradient-bucket slot directly."""
+    return _LinearFn.apply(x, weight, bias, ACT[act], residual, owner, stats)

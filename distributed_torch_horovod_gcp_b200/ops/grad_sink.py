@@ -77,42 +77,9 @@ def begin(weight, krsc: bool = False) -> Tuple[Optional[torch.Tensor], bool, Opt
 
 
 class GradBox:
-    """Hand-off of a residual-branch gradient between two autograd nodes of one block.
+    """Removed.  The name stays importable so that code written against the former cross-node hand-off of
+    skip-connection gradients fails where it uses it, with this pointer, rather than at import."""
 
-    In a residual block the block input ``x`` feeds the first convolution AND the skip connection, so
-    autograd sums two activation-sized gradients with a stand-alone ``add`` kernel (16 of them per
-    ResNet-50 step, ~1.1 ms).  With a box, the node that produces the skip gradient (the fused
-    BN+add+ReLU backward) parks it here instead of returning it, and the first convolution's dgrad GEMM
-    adds it in its epilogue (``C = A B + residual``) — the returned input gradient is already the sum.
-    The consumer arms the box in ITS forward (which runs first), so a producer never withholds a
-    gradient nobody will pick up; it marks the box ``consumed`` in its backward, so a producer that has
-    no data dependency on the consumer (the downsample convolution of a projection block) only parks
-    its gradient while the consumer is still to come.
-
-    ``mask``: optional ReLU sign bits (1 byte / 8 channels) that the consumer's epilogue applies to
-    ``dres`` — the BN+add+ReLU backward then parks the UNMASKED incoming gradient and does not write a
-    masked copy at all.  ``ext_mask``: the same bits handed to the downsample BatchNorm of a projection
-    block, whose incoming gradient is that unmasked tensor."""
-    __slots__ = ("armed", "consumed", "dres", "mask", "ext_mask", "want_mask")
-
-    def __init__(self):
-        self.armed = False
-        self.consumed = False
-        self.want_mask = False       # the consumer is a BatchNorm backward that applies ``ext_mask`` to its dy
-        self.dres = None
-        self.mask = None
-        self.ext_mask = None
-
-    def park(self, grad, mask=None) -> bool:
-        """Producer side: hand ``grad`` to the consumer if it is armed and still to run."""
-        if not self.armed or self.consumed or self.dres is not None:
-            return False
-        self.dres, self.mask = grad, mask
-        return True
-
-    def take(self):
-        """Consumer side (its backward): the parked (gradient, mask) or (None, None)."""
-        self.consumed = True
-        g, m = self.dres, self.mask
-        self.dres = self.mask = None
-        return g, m
+    def __init__(self, *args, **kwargs):
+        raise RuntimeError("GradBox was removed: a ResNet bottleneck block runs as one autograd node "
+                           "(ops/bottleneck.py) that adds the skip gradient in conv1's dgrad itself")

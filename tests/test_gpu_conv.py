@@ -161,16 +161,17 @@ def test_grad_sink_matches_autograd_path():
 
 
 @pytest.mark.parametrize("kind", ["identity", "projection_s1", "projection_s2"])
-def test_bottleneck_skip_gradient_goes_through_dgrad_epilogue(kind):
+def test_bottleneck_node_skip_gradient_goes_through_dgrad_epilogue(kind):
     """The block input feeds conv1 and the skip branch; its second gradient is added by conv1's dgrad GEMM
-    epilogue (ops.grad_sink.GradBox) — identity block: bn3's unmasked dy + ReLU sign bits; projection block:
-    the downsample conv's dgrad, with the sign bits handed to the downsample BN.  Oracle: the same kernels
-    with the boxes disabled (autograd's stand-alone add, masked copy written by the BN backward), plus a
-    loose check against the fp32 reference composition."""
+    epilogue inside the block's one autograd node (ops/bottleneck.py) — identity block: bn3's unmasked dy +
+    ReLU sign bits; projection block: the downsample conv's dgrad, with the sign bits applied by the
+    downsample BN.  Oracle: the per-op conv_bn_act chain on the same kernels (autograd's stand-alone add,
+    masked copy written by the BN backward), plus a loose check against the fp32 reference composition.
+    No state outlives a forward, so a repeated run is bit-identical."""
     import copy
     import torch.nn as nn
     from distributed_torch_horovod_gcp_b200.models.resnet import Bottleneck
-    from distributed_torch_horovod_gcp_b200.ops import functional as F2
+    from distributed_torch_horovod_gcp_b200.ops import bottleneck, functional as F2
     _kern()
     torch.manual_seed(4)
     if kind == "identity":
@@ -185,22 +186,27 @@ def test_bottleneck_skip_gradient_goes_through_dgrad_epilogue(kind):
     with torch.no_grad():
         oshape = blk(x0).shape
     g = torch.randn(oshape, device="cuda").to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
+    assert bottleneck.supported(x0, blk)
+
+    def per_op(x):
+        out = F2.conv_bn_act(x, blk.conv1, blk.bn1, relu=True)
+        out = F2.conv_bn_act(out, blk.conv2, blk.bn2, relu=True)
+        identity = x if blk.downsample is None else \
+            F2.conv_bn_act(x, blk.downsample[0], blk.downsample[1], relu=False)
+        return F2.conv_bn_act(out, blk.conv3, blk.bn3, relu=True, residual=identity)
+
     grads, wgrads = [], []
-    real_box = F2.new_grad_box
-    for use_box in (True, False, True):
-        F2.new_grad_box = real_box if use_box else (lambda t: None)
-        try:
-            # x is an intermediate (as in the network), so that a withheld gradient would go missing
-            leaf = x0.clone().requires_grad_(True)
-            x = leaf * 1.0
-            blk.zero_grad()
-            blk(x).backward(g)
-            grads.append(leaf.grad.float().clone())
-            wgrads.append(blk.conv1.weight.grad.float().clone())
-        finally:
-            F2.new_grad_box = real_box
+    for fwd in (blk, per_op, blk):
+        # x is an intermediate (as in the network), so that a withheld gradient would go missing
+        leaf = x0.clone().requires_grad_(True)
+        x = leaf * 1.0
+        blk.zero_grad()
+        fwd(x).backward(g)
+        grads.append(leaf.grad.float().clone())
+        wgrads.append(blk.conv1.weight.grad.float().clone())
     assert _rel(grads[0], grads[1]) < 1e-2          # fused add == stand-alone add
-    assert _rel(grads[2], grads[1]) < 1e-2          # the box is per-forward state: second use is clean
+    assert torch.equal(grads[2], grads[0])          # no per-forward state: the second use is bit-identical
+    assert torch.equal(wgrads[2], wgrads[0])
     assert _rel(wgrads[0], wgrads[1]) < 1e-2
     xr = x0.detach().float().requires_grad_(True)
     F2._FORCE_REFERENCE = True
