@@ -67,6 +67,9 @@ def parse_args(argv=None):
     p.add_argument("--bidirectional", action="store_true",
                    default=env("B200DP_BIDIRECTIONAL", "0") == "1",
                    help="bidirectional LSTM for the lstm model (the reference is unidirectional)")
+    p.add_argument("--clip-grad-norm", type=float, default=float(env("B200DP_CLIP_GRAD_NORM", "0")),
+                   help="clip the averaged gradient by its global L2 norm to at most this value before "
+                        "each update (DistributedOptimizer max_grad_norm=; 0 = off, the reference)")
     return p.parse_args(argv)
 
 
@@ -169,7 +172,8 @@ if __name__ == "__main__":
 
     if args.cuda_graph and use_cuda:
         os.environ.setdefault("B200DP_FUSED_SINGLE", "1")    # graph capture needs the fused update
-    optimizer = hvd.DistributedOptimizer(optimizer, named_parameters=model.named_parameters())
+    optimizer = hvd.DistributedOptimizer(optimizer, named_parameters=model.named_parameters(),
+                                         max_grad_norm=args.clip_grad_norm or None)
 
     model.to(_DEVICE)
     train_times = []

@@ -94,6 +94,18 @@ struct CollArgs {
   int pad_;
 };
 
+// Global-norm gradient clipping on the one-shot path (max_grad_norm=).  The per-bucket kernel is split in
+// three: K1c reduces into the fp32 arena `r` and writes one sum-of-squares slot per CTA, K8 folds every
+// slot into the norm and the clip coefficient, K9 scales `r` by the coefficient and runs the K7 epilogue.
+struct ClipArgs {
+  float* r;                // fp32 reduced gradient of this bucket (scale * sum), n elements
+  float* slots;            // K1c: this bucket's B200DP_MAX_BLOCKS slots; K8: the first slot of all buckets
+  float* norm;             // device scalar: total L2 norm before clipping (K8 writes it)
+  float* coef;             // device scalar: min(max_norm / (norm + 1e-6), 1) (K8 writes, K9 reads)
+  float max_norm;
+  int nslots;              // K8: number of slots (buckets * B200DP_MAX_BLOCKS)
+};
+
 struct BcastArgs {
   void* buf[B200DP_MAX_RANKS];
   void* buf_mc;
@@ -449,6 +461,120 @@ __global__ void __launch_bounds__(512) allreduce_oneshot_kernel(CommCtx c, ARArg
   finish_step(a);
 }
 
+// ------------------------------------------------------------------ K1c / K8 / K9: clip by global norm
+// Fixed-shape block sum of one fp32 value per thread (warp butterfly, then warp 0 over the warp partials):
+// the same inputs give the same bits on every rank and every run.
+__device__ __forceinline__ float block_sum_fixed(float v) {
+  __shared__ float s_part[32];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (lane == 0) s_part[warp] = v;
+  __syncthreads();
+  float t = 0.0f;
+  if (warp == 0) {
+    t = lane < (int)(blockDim.x >> 5) ? s_part[lane] : 0.0f;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+  }
+  return t;  // valid in thread 0
+}
+
+// K1c: K1's reduction (same fixed rank order, same `scale * sum`), but the result goes to the fp32 arena
+// `k.r` instead of through the optimizer epilogue, and each CTA stores the sum of squares of the values it
+// wrote in slot `k.slots[blockIdx.x]`.  Every rank reduces the whole bucket, so every rank holds the same
+// bits of `r` and of the slots, and hence computes the same norm.  Step counters are not touched.
+template <typename T>
+__global__ void __launch_bounds__(512) allreduce_oneshot_clip_kernel(CommCtx c, ARArgs a, ClipArgs k) {
+  constexpr int VN = Vec<T>::N;
+  const size_t nvec = a.n / VN;
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  const size_t start = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+
+  if (!rank_barrier(c, a.channel)) return;
+  float sq = 0.0f;
+  for (size_t v = start; v < nvec; v += stride) {
+    uint4 raw[B200DP_MAX_RANKS];
+#pragma unroll
+    for (int r = 0; r < B200DP_MAX_RANKS; ++r)
+      if (r < c.world) raw[r] = ld_peer_v4(reinterpret_cast<const uint4*>(a.in[r]) + v);
+    float acc[VN], f[VN];
+#pragma unroll
+    for (int i = 0; i < VN; ++i) acc[i] = 0.0f;
+#pragma unroll
+    for (int r = 0; r < B200DP_MAX_RANKS; ++r) {
+      if (r < c.world) {
+        Vec<T>::unpack(raw[r], f);
+#pragma unroll
+        for (int i = 0; i < VN; ++i) acc[i] += f[i];
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < VN; ++i) {
+      acc[i] *= a.scale;
+      sq = fmaf(acc[i], acc[i], sq);
+    }
+#pragma unroll
+    for (int i = 0; i < VN; i += 4)
+      *reinterpret_cast<float4*>(k.r + v * VN + i) = make_float4(acc[i], acc[i + 1], acc[i + 2], acc[i + 3]);
+  }
+  const float total = block_sum_fixed(sq);
+  if (threadIdx.x == 0) k.slots[blockIdx.x] = total;  // a CTA without elements writes 0
+  rank_barrier(c, a.channel);  // every peer has finished reading my gradients
+  if (a.zero_input) {
+    uint4* mine = reinterpret_cast<uint4*>(const_cast<void*>(a.in[c.rank]));
+    for (size_t v = start; v < nvec; v += stride) mine[v] = make_uint4(0, 0, 0, 0);
+  }
+}
+
+// K8: one CTA.  Thread t adds slots t, t + blockDim, ... in double, then a fixed tree in shared memory
+// combines the threads, so the order of every addition is fixed.  The coefficient follows
+// torch.nn.utils.clip_grad_norm_ in fp32: (1 / (norm + 1e-6)) * max_norm, clamped to at most 1 (NaN stays NaN).
+__global__ void __launch_bounds__(256) clip_finalize_kernel(ClipArgs k) {
+  __shared__ double s[256];
+  double acc = 0.0;
+  for (int i = threadIdx.x; i < k.nslots; i += blockDim.x) acc += (double)k.slots[i];
+  s[threadIdx.x] = acc;
+  __syncthreads();
+  for (int w = blockDim.x >> 1; w > 0; w >>= 1) {
+    if ((int)threadIdx.x < w) s[threadIdx.x] += s[threadIdx.x + w];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    const float norm = (float)sqrt(s[0]);
+    const float c = __frcp_rn(norm + 1e-6f) * k.max_norm;
+    *k.norm = norm;
+    *k.coef = c > 1.0f ? 1.0f : c;
+  }
+}
+
+// K9: purely local.  g = r * coef, then the K7 epilogue with a.scale == 1 (the scale is already in r), so
+// with coef == 1 the update is bit-identical to K1's.  Output and state are this rank's own copies.
+template <typename T>
+__global__ void __launch_bounds__(512) clip_apply_kernel(CommCtx c, ARArgs a, ClipArgs k) {
+  constexpr int VN = Vec<T>::N;
+  const size_t nvec = a.n / VN;
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  const size_t start = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const StepInfo s = make_step(a);
+  const float coef = *k.coef;
+  T* out = reinterpret_cast<T*>(a.out[c.rank]);
+  for (size_t v = start; v < nvec; v += stride) {
+    float g[VN];
+#pragma unroll
+    for (int i = 0; i < VN; i += 4) {
+      const float4 x = *reinterpret_cast<const float4*>(k.r + v * VN + i);
+      g[i] = x.x; g[i + 1] = x.y; g[i + 2] = x.z; g[i + 3] = x.w;
+    }
+#pragma unroll
+    for (int i = 0; i < VN; ++i) g[i] *= coef;
+    float o[VN];
+    epilogue<T, VN>(a, s, v * VN, g, out, o);
+    reinterpret_cast<uint4*>(out)[v] = Vec<T>::pack(o);
+  }
+  finish_step(a);
+}
+
 // ------------------------------------------------------------------ K2: two-shot (P2P) and K3: NVLS
 template <typename T, bool kNVLS>
 __global__ void __launch_bounds__(512) allreduce_sliced_kernel(CommCtx c, ARArgs a) {
@@ -663,6 +789,14 @@ cudaError_t launch_ar(const CommCtx& c, const ARArgs& a, int algo, int blocks, i
   return cudaGetLastError();
 }
 
+template <typename T>
+cudaError_t launch_clip(const CommCtx& c, const ARArgs& a, const ClipArgs& k, bool apply, int blocks,
+                        int threads, cudaStream_t st) {
+  if (apply) clip_apply_kernel<T><<<blocks, threads, 0, st>>>(c, a, k);
+  else allreduce_oneshot_clip_kernel<T><<<blocks, threads, 0, st>>>(c, a, k);
+  return cudaGetLastError();
+}
+
 }  // namespace
 
 extern "C" {
@@ -678,6 +812,42 @@ int b200dp_comm_limits(int* max_ranks, int* max_blocks, int* channels, int* ctx_
   *ctx_bytes = (int)sizeof(CommCtx);
   *ar_bytes = (int)sizeof(ARArgs);
   *bc_bytes = (int)sizeof(BcastArgs);
+  return 0;
+}
+
+int b200dp_comm_clip_bytes() { return (int)sizeof(ClipArgs); }
+
+// phase: 0 reduce into k.r + norm slots (K1c), 1 clip + optimizer update from k.r (K9).  dtype as in
+// b200dp_comm_allreduce: the dtype of the gradient bucket on the wire and of the parameter output.
+int b200dp_comm_clip_bucket(const CommCtx* ctx, const ARArgs* args, const ClipArgs* clip, int phase, int dtype,
+                            int blocks, int threads, unsigned long long stream) {
+  if (blocks < 1 || blocks > B200DP_MAX_BLOCKS || threads < 32 || threads > 512 || (threads & 31) ||
+      ctx->world > B200DP_MAX_RANKS || args->channel < 0 || args->channel >= B200DP_NUM_CHANNELS ||
+      phase < 0 || phase > 1) {
+    snprintf(g_comm_err, sizeof(g_comm_err), "bad clip launch config blocks=%d threads=%d world=%d ch=%d phase=%d",
+             blocks, threads, ctx->world, args->channel, phase);
+    return -1;
+  }
+  cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
+  cudaError_t e;
+  if (dtype == 0) e = launch_clip<float>(*ctx, *args, *clip, phase == 1, blocks, threads, st);
+  else if (dtype == 1) e = launch_clip<__nv_bfloat16>(*ctx, *args, *clip, phase == 1, blocks, threads, st);
+  else if (dtype == 2) e = launch_clip<__half>(*ctx, *args, *clip, phase == 1, blocks, threads, st);
+  else e = cudaErrorInvalidValue;
+  if (e != cudaSuccess) {
+    snprintf(g_comm_err, sizeof(g_comm_err), "clip launch: %s", cudaGetErrorString(e));
+    return -1;
+  }
+  return 0;
+}
+
+int b200dp_comm_clip_finalize(const ClipArgs* clip, unsigned long long stream) {
+  clip_finalize_kernel<<<1, 256, 0, (cudaStream_t)(uintptr_t)stream>>>(*clip);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    snprintf(g_comm_err, sizeof(g_comm_err), "clip finalize launch: %s", cudaGetErrorString(e));
+    return -1;
+  }
   return 0;
 }
 

@@ -16,6 +16,14 @@ Memory plan (per dtype arena, same element layout in every arena):
   P  parameters     symmetric   p.data are views        (peers push updated slices)
   M  fp32 master    local       only when dtype != fp32
   S0 momentum | exp_avg,  S1 exp_avg_sq   local fp32    (sharded by slice for K2/K3)
+  R  fp32 reduced gradient                local         clip mode only (max_grad_norm=)
+
+Clip mode (``max_grad_norm=``) splits each bucket's kernel in two phases, because a global norm needs
+every bucket reduced before any bucket is updated: the bucket-ready hook launches a one-shot reduction
+into R that also leaves one sum-of-squares slot per CTA (K1c); ``wait_all`` then launches one kernel
+that folds all slots into the norm and the clip coefficient (K8) and one local update per bucket that
+scales R by it and runs the unchanged K7 epilogue (K9).  One-shot everywhere means every rank holds the
+same bits of R, so every rank computes the same norm without a further exchange.
 """
 from __future__ import annotations
 
@@ -69,7 +77,8 @@ class FusedEngine:
     fuses_update = True
 
     @staticmethod
-    def try_create(opt, buckets: List[Bucket], wire_dtype) -> Optional["FusedEngine"]:
+    def try_create(opt, buckets: List[Bucket], wire_dtype,
+                   max_grad_norm: Optional[float] = None) -> Optional["FusedEngine"]:
         rt = _state.runtime()
         kind = _classify(opt)
         ok_dtypes = all(b.dtype in (torch.float32, torch.bfloat16, torch.float16) for b in buckets)
@@ -92,10 +101,11 @@ class FusedEngine:
             symm = LocalRuntime.get()
             if symm is None:
                 return None
-        return FusedEngine(opt, buckets, symm, kind, wire_dtype)
+        return FusedEngine(opt, buckets, symm, kind, wire_dtype, max_grad_norm)
 
     # ------------------------------------------------------------------ construction
-    def __init__(self, opt, buckets: List[Bucket], symm, kind: str, wire_dtype=None):
+    def __init__(self, opt, buckets: List[Bucket], symm, kind: str, wire_dtype=None,
+                 max_grad_norm: Optional[float] = None):
         from ..runtime import symm as S
         self.S = S
         self.opt, self.buckets, self.symm, self.kind = weakref.proxy(opt), buckets, symm, kind
@@ -113,6 +123,8 @@ class FusedEngine:
         # the wire dtype (keeps fp16 in range), the fused kernel applies f/N after the fp32 sum.  Without
         # wire compression the sum is fp32 end to end and (1/f)(f/N) == 1/N exactly, so nothing changes.
         self.predivide = float(getattr(opt, "_gradient_predivide_factor", 1.0) or 1.0)
+        self.max_grad_norm = None if max_grad_norm is None else float(max_grad_norm)
+        self.clip = self.max_grad_norm is not None
         self.arenas: Dict[torch.dtype, dict] = {}
         for (dtype, device), n in arena_sizes(buckets).items():
             if self.wire is not None:
@@ -144,6 +156,8 @@ class FusedEngine:
                 "S0": torch.zeros(n, dtype=torch.float32, device=device),
                 "S1": torch.zeros(n, dtype=torch.float32, device=device) if kind != "sgd" else None,
             }
+        for (dtype, device), n in arena_sizes(buckets).items():
+            self.arenas[dtype]["R"] = torch.zeros(n, dtype=torch.float32, device=device) if self.clip else None
         # re-home parameters and gradients into the arenas
         with torch.no_grad():
             for b in buckets:
@@ -160,6 +174,20 @@ class FusedEngine:
         self._algo: Dict[int, int] = {}
         for b in buckets:
             self._args[b.index], self._algo[b.index] = self._make_args(b)
+        self.grad_norm: Optional[torch.Tensor] = None
+        if self.clip:
+            # per-bucket slots of the reduce phase; a bucket's grid never changes, so slots past it stay 0
+            self.slots = torch.zeros(nb * S.MAX_BLOCKS, dtype=torch.float32, device=self.device)
+            self.grad_norm = torch.zeros((), dtype=torch.float32, device=self.device)
+            self.coef = torch.ones((), dtype=torch.float32, device=self.device)
+            self._clip_args: Dict[int, object] = {}
+            self._apply_args: Dict[int, object] = {}
+            for b in buckets:
+                self._clip_args[b.index], self._apply_args[b.index] = self._make_clip_args(b)
+            fin = S.ClipArgs()
+            fin.slots, fin.nslots = self.slots.data_ptr(), self.slots.numel()
+            fin.norm, fin.coef, fin.max_norm = self.grad_norm.data_ptr(), self.coef.data_ptr(), self.max_grad_norm
+            self._fin_args = fin
         self._done = torch.cuda.Event()
         self.steps = 0
         self.rehomed = 0
@@ -226,8 +254,8 @@ class FusedEngine:
             a.inp[r], a.out[r] = gp[r], pp[r]
         both_mc = ar["G"].mc_ptr != 0 and ar["P"].mc_ptr != 0
         algo = symm.pick_algo(nbytes, need_mc=both_mc)
-        if self.wire is not None:
-            algo = S.ALGO_ONESHOT            # every rank must hold the full fp32 update (see __init__)
+        if self.wire is not None or self.clip:
+            algo = S.ALGO_ONESHOT            # every rank must hold the full fp32 update / gradient (see __init__)
         if algo == S.ALGO_NVLS and not both_mc:
             algo = S.ALGO_TWOSHOT
         if algo == S.ALGO_NVLS:
@@ -248,6 +276,19 @@ class FusedEngine:
         a.channel = S.CH_ENGINE
         a.zero_input, a.copy_back = 1, 0
         return a, algo
+
+    def _make_clip_args(self, b: Bucket):
+        """(reduce-phase ClipArgs, apply-phase ARArgs) of a bucket in clip mode.  The apply phase reads the
+        already scaled R, so its ``scale`` is 1; everything else (outputs, master, state, step counter) is the
+        bucket's ordinary one-shot argument block."""
+        S, ar = self.S, self.arenas[b.dtype]
+        k = S.ClipArgs()
+        k.r = ar["R"].data_ptr() + 4 * b.flat_offset
+        k.slots = self.slots.data_ptr() + 4 * S.MAX_BLOCKS * b.index
+        k.norm, k.coef, k.max_norm = self.grad_norm.data_ptr(), self.coef.data_ptr(), self.max_grad_norm
+        ap = S.ARArgs.from_buffer_copy(self._args[b.index])
+        ap.scale = 1.0
+        return k, ap
 
     # ------------------------------------------------------------------ hot path
     def _fill_hyper(self, a, group: dict):
@@ -294,7 +335,10 @@ class FusedEngine:
                       f"{b.nbytes / 2**20:.1f}MB")
         kdtype = self.wire if self.wire is not None else b.dtype
         kbytes = b.numel * torch.empty((), dtype=kdtype).element_size()
-        self.symm.launch_allreduce(a, self._algo[b.index], kdtype, kbytes, self.side)
+        if self.clip:
+            self.symm.launch_clip_bucket(a, self._clip_args[b.index], self.S.CLIP_REDUCE, kdtype, kbytes, self.side)
+        else:
+            self.symm.launch_allreduce(a, self._algo[b.index], kdtype, kbytes, self.side)
         nvtx.pop()
         self.kernel_launches += 1
         if tl is not None:
@@ -305,9 +349,36 @@ class FusedEngine:
         return True
 
     def wait_all(self, launched):
+        if self.clip:
+            self._clip_and_update()
         self._done.record(self.side)
         torch.cuda.current_stream(self.device).wait_event(self._done)
         self.symm.check_errors()
+
+    def _clip_and_update(self):
+        """Clip mode, after every bucket's reduce phase: the global norm and the clip coefficient (one
+        launch), then the optimizer update of every bucket from R (one launch each), all on the side stream."""
+        tl = _state.runtime().timeline
+        if tl is not None:
+            s_ev, e_ev = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            s_ev.record(self.side)
+        nvtx.push("CLIP_FINALIZE_APPLY")
+        self.symm.launch_clip_finalize(self._fin_args, self.side)
+        self.kernel_launches += 1
+        lr_scale = self.lr_scale.data_ptr() if self.lr_scale is not None else 0
+        for b in self.buckets:
+            ap = self._apply_args[b.index]
+            self._fill_hyper(ap, self.opt.param_groups[b.group_index])
+            ap.lr_scale = lr_scale
+            kdtype = self.wire if self.wire is not None else b.dtype
+            kbytes = b.numel * torch.empty((), dtype=kdtype).element_size()
+            self.symm.launch_clip_bucket(ap, self._clip_args[b.index], self.S.CLIP_APPLY, kdtype, kbytes, self.side)
+            self.kernel_launches += 1
+        nvtx.pop()
+        if tl is not None:
+            e_ev.record(self.side)
+            tl.cuda_span("optimizer", "CLIP_FINALIZE_APPLY", s_ev, e_ev,
+                         bytes=sum(b.numel for b in self.buckets) * 4)
 
     def after_step(self):
         self.steps += 1
@@ -429,7 +500,7 @@ class FusedEngine:
                     except Exception:  # noqa: BLE001
                         pass
             ar["g"] = ar["p"] = ar["G"] = ar["P"] = None
-            ar["gw"] = None
+            ar["gw"] = ar["R"] = None
         self._args.clear()
 
     def algorithms(self) -> Dict[int, str]:

@@ -84,6 +84,8 @@ class LocalRuntime:
         return int(max(1, min((nbytes + per_block - 1) // per_block, self.max_blocks or 128)))
 
     launch_allreduce = S.SymmRuntime.launch_allreduce
+    launch_clip_bucket = S.SymmRuntime.launch_clip_bucket
+    launch_clip_finalize = S.SymmRuntime.launch_clip_finalize
 
     def allreduce_(self, t, prescale=1.0, postscale=1.0, algo=None):
         if prescale * postscale != 1.0:

@@ -54,6 +54,14 @@ class ARArgs(ctypes.Structure):
                 ("zero_input", ctypes.c_int), ("copy_back", ctypes.c_int), ("h", OptHyper)]
 
 
+class ClipArgs(ctypes.Structure):
+    _fields_ = [("r", ctypes.c_uint64), ("slots", ctypes.c_uint64), ("norm", ctypes.c_uint64),
+                ("coef", ctypes.c_uint64), ("max_norm", ctypes.c_float), ("nslots", ctypes.c_int)]
+
+
+CLIP_REDUCE, CLIP_APPLY = 0, 1
+
+
 class BcastArgs(ctypes.Structure):
     _fields_ = [("buf", ctypes.c_uint64 * MAX_RANKS), ("buf_mc", ctypes.c_uint64),
                 ("nbytes", ctypes.c_uint64), ("root", ctypes.c_int), ("channel", ctypes.c_int),
@@ -226,15 +234,17 @@ class SymmRuntime:
         L.b200dp_can_access_peer.argtypes = [i, i]
         L.b200dp_comm_allreduce.argtypes = [P(CommCtx), P(ARArgs), i, i, i, i, u64]
         L.b200dp_comm_broadcast.argtypes = [P(CommCtx), P(BcastArgs), i, i, u64]
+        L.b200dp_comm_clip_bucket.argtypes = [P(CommCtx), P(ARArgs), P(ClipArgs), i, i, i, i, u64]
+        L.b200dp_comm_clip_finalize.argtypes = [P(ClipArgs), u64]
         if hasattr(L, "b200dp_comm_collective"):
             L.b200dp_comm_collective.argtypes = [P(CommCtx), P(CollArgs), i, i, i, i, u64]
             if L.b200dp_comm_coll_bytes() != ctypes.sizeof(CollArgs):
                 raise RuntimeError("ctypes/C struct layout mismatch: CollArgs")
         lim = [ctypes.c_int() for _ in range(6)]
         L.b200dp_comm_limits(*[ctypes.byref(x) for x in lim])
-        got = tuple(x.value for x in lim)
+        got = tuple(x.value for x in lim) + (L.b200dp_comm_clip_bytes(),)
         want = (MAX_RANKS, MAX_BLOCKS, NUM_CHANNELS, ctypes.sizeof(CommCtx), ctypes.sizeof(ARArgs),
-                ctypes.sizeof(BcastArgs))
+                ctypes.sizeof(BcastArgs), ctypes.sizeof(ClipArgs))
         if got != want:
             raise RuntimeError(f"ctypes/C struct layout mismatch: C={got} python={want}")
 
@@ -377,6 +387,25 @@ class SymmRuntime:
         blocks = blocks or self.pick_blocks(algo, nbytes)
         rc = self.lib.b200dp_comm_allreduce(ctypes.byref(self.ctx), ctypes.byref(args), algo,
                                             _DTYPE_CODE[dtype], blocks, 512, stream.cuda_stream)
+        if rc != 0:
+            raise RuntimeError((self.lib.b200dp_comm_last_error() or b"").decode())
+        self.launches += 1
+
+    def launch_clip_bucket(self, args: ARArgs, clip: ClipArgs, phase: int, dtype: torch.dtype, nbytes: int,
+                           stream: torch.cuda.Stream):
+        """One bucket of the clip-mode engine: ``CLIP_REDUCE`` (one-shot reduction into ``clip.r`` plus the
+        per-CTA norm slots) or ``CLIP_APPLY`` (scale ``clip.r`` by the clip coefficient, optimizer update).
+        Both phases of a bucket use the same grid, so the reduce phase fills the same slots every step."""
+        blocks = self.pick_blocks(ALGO_ONESHOT, nbytes)
+        rc = self.lib.b200dp_comm_clip_bucket(ctypes.byref(self.ctx), ctypes.byref(args), ctypes.byref(clip),
+                                              phase, _DTYPE_CODE[dtype], blocks, 512, stream.cuda_stream)
+        if rc != 0:
+            raise RuntimeError((self.lib.b200dp_comm_last_error() or b"").decode())
+        self.launches += 1
+
+    def launch_clip_finalize(self, clip: ClipArgs, stream: torch.cuda.Stream):
+        """Sum every bucket's norm slots (fixed order) into the global norm and the clip coefficient."""
+        rc = self.lib.b200dp_comm_clip_finalize(ctypes.byref(clip), stream.cuda_stream)
         if rc != 0:
             raise RuntimeError((self.lib.b200dp_comm_last_error() or b"").decode())
         self.launches += 1

@@ -23,9 +23,16 @@ H100-first design (vs Horovod's per-tensor ``allreduce_async_`` + host ``synchro
 When ``size() == 1`` no hooks are registered and the object behaves as the plain
 optimizer (Horovod parity), unless ``B200DP_FUSED_SINGLE=1`` asks for the fused update
 kernel on one GPU.
+
+``max_grad_norm=`` clips the reduced gradient by its global L2 norm before the update, with the
+semantics of ``torch.nn.utils.clip_grad_norm_(params, max_grad_norm)``.  The fused engine does it on
+the device between its reduce and update phases (``parallel/fused_engine.py``); every other path calls
+``clip_grad_norm_`` once per step on the reduced gradients, right before the wrapped ``step()``.
 """
 from __future__ import annotations
 
+import math
+import numbers
 import os
 import warnings
 from contextlib import contextmanager
@@ -48,7 +55,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
 
     def __init__(self, params, named_parameters, compression, backward_passes_per_step, op,
                  gradient_predivide_factor, groups, num_groups, sparse_as_dense, process_set,
-                 bucket_bytes, fused):
+                 bucket_bytes, fused, max_grad_norm=None):
         super(self.__class__, self).__init__(params)
         self._compression = compression
         self._op = op
@@ -93,6 +100,11 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         self._num_groups = num_groups
         self._bucket_bytes = bucket_bytes
         self._fused_request = fused
+        self._max_grad_norm = max_grad_norm
+        self._grad_norm_out = None
+        if max_grad_norm is not None and all_params:
+            # fixed address: a captured graph and the host read the same tensor every step
+            self._grad_norm_out = torch.zeros((), dtype=torch.float32, device=all_params[0].device)
 
         rt = _state._require_init()
         self._world = mpi_ops._ps_size(process_set)
@@ -131,7 +143,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
             want_fused = os.environ.get("B200DP_FUSED", "1") == "1"
         if want_fused and on_cuda and self._process_set is None and self._op in (Average, Sum):
             from ..parallel.fused_engine import FusedEngine
-            self._engine = FusedEngine.try_create(self, self._buckets, wire)
+            self._engine = FusedEngine.try_create(self, self._buckets, wire, self._max_grad_norm)
             if self._engine is None and self._fused_request:
                 raise RuntimeError("fused=True requested but the fused sm_90a engine is "
                                    "unavailable: " + str(_state.runtime().symm_failed))
@@ -324,9 +336,24 @@ class _DistributedOptimizer(torch.optim.Optimizer):
                 self._passes[k] = 0
 
     # ------------------------------------------------------------------ step / zero_grad
+    def _clip_then_step(self, closure):
+        """Un-fused paths: clip the (reduced) gradients by their global norm, then the wrapped step."""
+        if self._max_grad_norm is None:
+            return super(self.__class__, self).step(closure)
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        params = [p for g in self.param_groups for p in g["params"]]
+        norm = torch.nn.utils.clip_grad_norm_(params, self._max_grad_norm)
+        if self._grad_norm_out is not None:
+            self._grad_norm_out.copy_(norm)
+        super(self.__class__, self).step()
+        return loss
+
     def step(self, closure=None):
         if not self._active:
-            return super(self.__class__, self).step(closure)
+            return self._clip_then_step(closure)
         tl = _state.runtime().timeline
         if tl is None:
             with nvtx.range("optimizer.step"):
@@ -345,7 +372,9 @@ class _DistributedOptimizer(torch.optim.Optimizer):
                 raise RuntimeError(
                     "skip_synchronize() requires the un-fused path: construct "
                     "DistributedOptimizer(..., fused=False) when gradients must be modified "
-                    "(e.g. clipped) between synchronize() and step().")
+                    "(e.g. clipped) between synchronize() and step().  To clip by global norm, "
+                    "pass DistributedOptimizer(..., max_grad_norm=X) instead: the fused engine "
+                    "then clips the reduced gradients itself.")
             loss = None
             if closure is not None:
                 with torch.enable_grad():
@@ -364,7 +393,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
                               "optimizer.synchronize() in your code.")
             self.synchronize()
         self._synchronized = False
-        return super(self.__class__, self).step(closure)
+        return self._clip_then_step(closure)
 
     def zero_grad(self, set_to_none: bool = True):
         """At size 1 this is the wrapped optimizer's ``zero_grad``.  When active, gradients are
@@ -416,6 +445,15 @@ class _DistributedOptimizer(torch.optim.Optimizer):
     def fused_engine(self):
         return self._engine
 
+    @property
+    def grad_norm(self):
+        """0-dim fp32 device tensor: the global L2 norm of the reduced gradients of the latest step, before
+        clipping (what ``clip_grad_norm_`` returns).  Same tensor every step, updated in place (also by
+        CUDA-graph replays); reading it does not synchronise.  ``None`` without ``max_grad_norm``."""
+        if self._engine is not None and getattr(self._engine, "grad_norm", None) is not None:
+            return self._engine.grad_norm
+        return self._grad_norm_out
+
     def bucket_plan(self) -> List[Bucket]:
         return list(self._buckets)
 
@@ -432,13 +470,20 @@ class _DistributedOptimizer(torch.optim.Optimizer):
 def DistributedOptimizer(optimizer, named_parameters=None, compression=Compression.none,
                          backward_passes_per_step=1, op=Average, gradient_predivide_factor=1.0,
                          num_groups=0, groups=None, sparse_as_dense=False, process_set=None,
-                         bucket_bytes=None, fused=None):
+                         bucket_bytes=None, fused=None, max_grad_norm=None):
     """Wrap ``optimizer`` so gradients are averaged across ranks before the update.
 
-    Arguments follow Horovod (SURVEY.md §2.3 A6); ``bucket_bytes`` and ``fused`` are
-    H100-runtime extensions (``fused=None`` → use the fused sm_90a kernel when the
-    optimizer is plain SGD(-momentum) / Adam / AdamW on CUDA with the symmetric runtime).
+    Arguments follow Horovod (SURVEY.md §2.3 A6); ``bucket_bytes``, ``fused`` and
+    ``max_grad_norm`` are H100-runtime extensions (``fused=None`` → use the fused sm_90a kernel
+    when the optimizer is plain SGD(-momentum) / Adam / AdamW on CUDA with the symmetric runtime;
+    ``max_grad_norm=X`` → clip the reduced gradient by its global L2 norm before every update, as
+    ``torch.nn.utils.clip_grad_norm_(params, X)`` would; the norm is ``optimizer.grad_norm``).
     """
+    if max_grad_norm is not None:
+        if isinstance(max_grad_norm, bool) or not isinstance(max_grad_norm, numbers.Real) or \
+                not math.isfinite(float(max_grad_norm)) or float(max_grad_norm) <= 0.0:
+            raise ValueError(f"max_grad_norm must be None or a finite number > 0, got {max_grad_norm!r}")
+        max_grad_norm = float(max_grad_norm)
     if op is Adasum:
         raise NotImplementedError("op=Adasum is not supported; use Average or Sum.")
     if gradient_predivide_factor != 1.0 and op is not Average:
@@ -457,4 +502,4 @@ def DistributedOptimizer(optimizer, named_parameters=None, compression=Compressi
     cls = type(optimizer.__class__.__name__, (optimizer.__class__,), body)
     return cls(optimizer.param_groups, named_parameters, compression, backward_passes_per_step,
                op, gradient_predivide_factor, groups, num_groups, sparse_as_dense, process_set,
-               bucket_bytes, fused)
+               bucket_bytes, fused, max_grad_norm)

@@ -4,7 +4,7 @@ Shapes are small (the tools slow kernels 10-100x) but cover: multi-tile persiste
 CTA are not reachable at these sizes on 132 SMs, so max_ctas is forced down where the API allows), the
 statistics / residual / masked-residual / split-K epilogues (per-CTA statistics slots, last-arriver split-K
 reduction, fp32 and bf16 add / store outputs), 3x3 / strided / 1x1 conv paths incl. split-K wgrad, BN, LN, pooling, attention and the LSTM
-recurrence."""
+recurrence, plus the fused engine's clip-by-global-norm kernels (reduce into R with norm slots, finalize, update)."""
 import os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from distributed_torch_horovod_gcp_b200.ops import kernels, gemm as G, conv as C, bn as B
@@ -60,4 +60,20 @@ m(xs).sum().backward()
 m2 = LSTM(40, 5, 1, 256, n_layers=2, bidirectional=True, device=torch.device(dev)).to(dev)
 m2(torch.randn(7, 5, 40, device=dev)).sum().backward()
 torch.cuda.synchronize()
+
+# fused engine in clip mode on one GPU: several buckets, bf16 parameters with fp32 masters, two steps
+os.environ["B200DP_FUSED_SINGLE"] = "1"
+import distributed_torch_horovod_gcp_b200.torch as hvd
+hvd.init()
+mlp = nn.Sequential(nn.Linear(32, 100), nn.ReLU(), nn.Linear(100, 7)).to(dev).to(bf)
+opt = hvd.DistributedOptimizer(torch.optim.Adam(mlp.parameters(), lr=1e-3), named_parameters=mlp.named_parameters(),
+                               bucket_bytes=4096, max_grad_norm=0.01)
+assert opt.fused_engine is not None and opt.fused_engine.clip
+for _ in range(2):
+    mlp(rnd(8, 32)).float().square().mean().backward()
+    opt.step()
+    opt.zero_grad()
+torch.cuda.synchronize()
+print("clip ok", float(opt.grad_norm))
+hvd.shutdown()
 print("all ok")
