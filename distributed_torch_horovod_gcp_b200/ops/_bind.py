@@ -33,5 +33,5 @@ def linear_supported(x, weight) -> bool:
     return _gemm.supported(x, weight)
 
 
-def layer_norm_supported(x, weight) -> bool:
-    return _ln.supported(x, weight)
+def layer_norm_supported(x, weight, bias) -> bool:
+    return _ln.supported(x, weight, bias)

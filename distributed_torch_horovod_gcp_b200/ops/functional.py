@@ -105,9 +105,9 @@ def mlp(x, w1, b1, w2, b2, residual=None):
 # ------------------------------------------------------------------ layer norm
 def layer_norm(x, weight, bias, eps: float = 1e-6):
     k = _kernels(x)
-    if k is not None and k.has("layer_norm") and k.layer_norm_supported(x, weight):
+    if k is not None and k.has("layer_norm") and k.layer_norm_supported(x, weight, bias):
         return k.layer_norm(x, weight, bias, eps)
-    return F.layer_norm(x, (x.shape[-1],), weight.to(x.dtype), bias.to(x.dtype), eps)
+    return F.layer_norm(x, (x.shape[-1],), weight.to(x.dtype), None if bias is None else bias.to(x.dtype), eps)
 
 
 # ------------------------------------------------------------------ attention

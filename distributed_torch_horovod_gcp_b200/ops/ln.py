@@ -23,10 +23,12 @@ def register(lib, have):
     have["layer_norm"] = True
 
 
-def supported(x: torch.Tensor, weight: torch.Tensor) -> bool:
+def supported(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor) -> bool:
+    """The kernels read gamma and beta in one dtype (``pbf16``), so both must have it."""
     C = x.shape[-1]
     return (_lib is not None and x.dtype == torch.bfloat16 and x.is_cuda
-            and weight.dtype in (torch.bfloat16, torch.float32) and bool(_lib.b200dp_ln_supported(C)))
+            and weight.dtype in (torch.bfloat16, torch.float32) and bias is not None
+            and bias.dtype == weight.dtype and bool(_lib.b200dp_ln_supported(C)))
 
 
 class _LayerNormFn(torch.autograd.Function):

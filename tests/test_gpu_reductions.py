@@ -18,7 +18,9 @@ that a whole ResNet training step repeats bit for bit.
 
 Not covered on purpose: ViT and LSTM training are not reproducible run to run.  The LayerNorm parameter
 gradients (``elementwise.cu``), the attention dQ accumulation (``attn_sm90.cu``) and the LSTM ``dW_hh``
-(``lstm_rec_sm90.cu``) still sum with fp32 atomics, in arrival order.
+(``lstm_rec_sm90.cu``) still sum with fp32 atomics, in arrival order, so their bits are not checked here.
+Their values are: ``test_gpu_vit_numerics.py`` bounds the LayerNorm and attention outputs and gradients
+against float64 with bounds that hold for any summation order.
 """
 import os
 import subprocess
@@ -29,45 +31,17 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from fp64_bounds import assert_within_bound, report_ratios
+
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-U32 = 2.0 ** -24          # unit roundoff of fp32
-U_BF16 = 2.0 ** -8        # relative rounding error of a bf16 store
-
-# worst err/bound ratio seen per test group (printed at the end of the module, e.g. with `pytest -s`)
-_WORST = {}
 
 
 @pytest.fixture(scope="module", autouse=True)
 def _report_ratios():
     yield
-    for k in sorted(_WORST):
-        print(f"\n[err/bound] {k}: max {_WORST[k]:.3e}", end="")
-    print()
-
-
-def _assert_within_bound(out, ref64, mag64, n_terms, out_bf16=False, group="misc"):
-    """|out - ref64| <= 2 * n_terms * 2^-24 * mag64 (+ 2^-8 * |ref64| for a bf16 output), elementwise.
-
-    ``ref64``: the operation in float64 on the bf16 inputs the kernel saw; ``mag64``: the same operation on
-    absolute values.  This bounds any fp32 summation order and rounding of ``n_terms`` terms, so it needs no
-    fitting and does not flake."""
-    out64 = out.double()
-    err = (out64 - ref64).abs()
-    bound = 2.0 * n_terms * U32 * mag64
-    if out_bf16:
-        bound = bound + U_BF16 * ref64.abs()
-    ratio = torch.where(bound > 0, err / bound.clamp_min(1e-300),
-                        torch.where(err > 0, torch.full_like(err, float("inf")), torch.zeros_like(err)))
-    worst = int(torch.argmax(ratio))
-    r = float(ratio.reshape(-1)[worst])
-    _WORST[group] = max(_WORST.get(group, 0.0), r)
-    if not bool((err <= bound).all()):
-        idx = np.unravel_index(worst, tuple(ratio.shape))
-        raise AssertionError(
-            f"{group}: {int((err > bound).sum())} element(s) outside the fp64 bound; worst at {tuple(map(int, idx))}: "
-            f"out={float(out64[idx]):.9g} ref={float(ref64[idx]):.9g} err/bound={r:.3g}")
+    report_ratios()
 
 
 def _gemm():
@@ -160,7 +134,7 @@ def test_gemm_splitk_sums_in_split_order(a_mn, b_mn, M, N, K, block_n, splits, a
             f"(max diff {float((out - expected).abs().max()):.3g})"
         if extra:
             assert torch.equal(big[:, N:], big0[:, N:]), "split-K wrote past column N of its output"
-        _assert_within_bound(out, ref64, mag64, K + s + 1, group="gemm split-K")
+        assert_within_bound(out, ref64, mag64, K + s + 1, group="gemm split-K")
 
 
 def test_gemm_bias_grad_shape_splitk():
@@ -184,7 +158,7 @@ def test_gemm_bias_grad_shape_splitk():
                max_ctas=max_ctas)
         torch.cuda.synchronize()
         assert torch.equal(out, expected), f"max_ctas={max_ctas}"
-        _assert_within_bound(out, ref64, mag64, rows + s + 1, group="gemm split-K")
+        assert_within_bound(out, ref64, mag64, rows + s + 1, group="gemm split-K")
     db = g.bias_grad(dz, C, rows, torch.float32)
     assert torch.equal(db, expected[:, 0])
 
@@ -338,10 +312,10 @@ def test_conv_wgrad_fp32_store_add_grid_invariant_and_bounded(N, Cin, H, W, Cout
             again = run(splits, max_ctas)
             assert torch.equal(again, first), \
                 f"splits={splits}: max_ctas={max_ctas} != default grid (max diff {float((again - first).abs().max()):.3g})"
-        _assert_within_bound(first, ref64, mag64, n_terms, group="conv wgrad")
+        assert_within_bound(first, ref64, mag64, n_terms, group="conv wgrad")
     pre = torch.randn(Cout, R, R, Cin, device="cuda", generator=gen)
     acc = run(0, 0, prefill=pre)
-    _assert_within_bound(acc, pre.double() + ref64, pre.double().abs() + mag64, n_terms + 1, group="conv wgrad")
+    assert_within_bound(acc, pre.double() + ref64, pre.double().abs() + mag64, n_terms + 1, group="conv wgrad")
 
 
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float32])
@@ -464,7 +438,7 @@ def test_gemm_epilogue_stats(M, N, K, bias):
         g.gemm(a, b, y, M, N, K, bias=bvec, stats=st, max_ctas=max_ctas)
         torch.cuda.synchronize()
         ref, mag = _stats_ref(y)
-        _assert_within_bound(st, ref, mag, M, group="gemm epilogue stats")
+        assert_within_bound(st, ref, mag, M, group="gemm epilogue stats")
         runs.append((y, st))
     _assert_repeats(runs)
     pre = torch.randn(2 * N, device="cuda", generator=gen).abs() * 10
@@ -473,7 +447,7 @@ def test_gemm_epilogue_stats(M, N, K, bias):
     g.gemm(a, b, y, M, N, K, bias=bvec, stats=st)
     torch.cuda.synchronize()
     ref, mag = _stats_ref(y, pre)
-    _assert_within_bound(st, ref, mag, M + 1, group="gemm epilogue stats")
+    assert_within_bound(st, ref, mag, M + 1, group="gemm epilogue stats")
 
 
 CONV_STATS_CASES = [
@@ -509,18 +483,18 @@ def test_conv_epilogue_stats(N, Cin, H, W, Cout, R, stride):
     for max_ctas in GRID_SEQUENCE:
         y, st = run(max_ctas)
         ref, mag = _stats_ref(y.permute(0, 2, 3, 1).reshape(-1, Cout))
-        _assert_within_bound(st, ref, mag, N * OH * OW, group="conv epilogue stats")
+        assert_within_bound(st, ref, mag, N * OH * OW, group="conv epilogue stats")
         runs.append((y, st))
     _assert_repeats(runs)
     # the output itself, against a float64 convolution of the same bf16 operands
     y = runs[0][0]
     y64 = F.conv2d(x.double(), w.double(), None, stride, pad)
     m64 = F.conv2d(x.double().abs(), w.double().abs(), None, stride, pad)
-    _assert_within_bound(y, y64, m64, Cin * R * R, out_bf16=True, group="conv fprop output")
+    assert_within_bound(y, y64, m64, Cin * R * R, out_bf16=True, group="conv fprop output")
     pre = torch.randn(2 * Cout, device="cuda", generator=gen)
     y, st = run(3, prefill=pre)
     ref, mag = _stats_ref(y.permute(0, 2, 3, 1).reshape(-1, Cout), pre)
-    _assert_within_bound(st, ref, mag, N * OH * OW + 1, group="conv epilogue stats")
+    assert_within_bound(st, ref, mag, N * OH * OW + 1, group="conv epilogue stats")
 
 
 BN_CHANNELS = [8, 16, 32, 64, 128, 256, 512, 1024, 2048]
@@ -554,7 +528,7 @@ def test_bn_standalone_reductions(C, M):
     st = stats()
     torch.cuda.synchronize()
     ref, mag = _stats_ref(x)
-    _assert_within_bound(st, ref, mag, M, group="bn stand-alone stats")
+    assert_within_bound(st, ref, mag, M, group="bn stand-alone stats")
     assert torch.equal(stats(), st)
     x64, m64 = x.double(), mean.double()
     for relu in (False, True):
@@ -564,7 +538,7 @@ def test_bn_standalone_reductions(C, M):
         xc = x64 - m64
         ref = torch.cat([dz.sum(0), (dz * xc).sum(0)])
         mag = torch.cat([dz.abs().sum(0), (dz.abs() * xc.abs()).sum(0)])
-        _assert_within_bound(s, ref, mag, M, group="bn stand-alone bwd reduce")
+        assert_within_bound(s, ref, mag, M, group="bn stand-alone bwd reduce")
         assert torch.equal(bwd(relu), s)
 
 
