@@ -67,6 +67,10 @@ def parse_args(argv=None):
     p.add_argument("--bidirectional", action="store_true",
                    default=env("B200DP_BIDIRECTIONAL", "0") == "1",
                    help="bidirectional LSTM for the lstm model (the reference is unidirectional)")
+    p.add_argument("--lstm-dropout", type=float, default=float(env("B200DP_LSTM_DROPOUT", "0")),
+                   help="dropout probability between stacked LSTM layers (nn.LSTM dropout=; 0 = off, the "
+                        "reference).  Like the reference, validation does not switch the model to eval mode, "
+                        "so with P > 0 the printed test_loss is computed with dropout on")
     p.add_argument("--clip-grad-norm", type=float, default=float(env("B200DP_CLIP_GRAD_NORM", "0")),
                    help="clip the averaged gradient by its global L2 norm to at most this value before "
                         "each update (DistributedOptimizer max_grad_norm=; 0 = off, the reference)")
@@ -139,7 +143,8 @@ if __name__ == "__main__":
                                      shuffle=True, pin_memory=use_cuda, num_workers=nw)
 
         model = LSTM(n_features=23, window_size=window_length, output_size=1, h_size=256,
-                     n_layers=args.lstm_layers, bidirectional=args.bidirectional, device=_DEVICE)
+                     n_layers=args.lstm_layers, bidirectional=args.bidirectional, device=_DEVICE,
+                     dropout=args.lstm_dropout)
         optimizer = torch.optim.Adam(model.parameters(), lr=args.lr)
         loss_fn = nn.MSELoss(reduction="mean")
     else:

@@ -6,9 +6,11 @@ For each (layers, directions, batch, steps) config, with F = 23 input features a
   * ``step_ms``: a whole training step of the reference model (LSTM + head + MSE +
     ``DistributedOptimizer(Adam)`` with the fused engine), captured in one CUDA graph and replayed.
 Both for K5 (the default path) and for cuDNN (``model._fused = False``, cuDNN's default TF32 on).
-Prints one JSON line per config with the card name and power limit read in the same run.
+``--dropout P`` also times every config with inter-layer dropout P (``nn.LSTM(dropout=P)``, training mode;
+one-layer configs have no layer to drop after and are timed at P = 0 only).
+Prints one JSON line per (config, dropout) with the card name and power limit read in the same run.
 
-    python benchmarks/lstm_bench.py [--iters 200] [--warmup 20]
+    python benchmarks/lstm_bench.py [--iters 200] [--warmup 20] [--dropout 0.2]
 """
 import argparse
 import copy
@@ -77,6 +79,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=200)
     ap.add_argument("--warmup", type=int, default=20)
+    ap.add_argument("--dropout", type=float, default=0.0, help="also time at this inter-layer dropout")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("lstm_bench needs a GPU")
@@ -87,13 +90,13 @@ def main():
     hvd.init()
     dev = torch.device("cuda", 0)
     name, power = card()
-    for L, D, B, T in CONFIGS:
+    for (L, D, B, T), p in [(c, p) for c in CONFIGS for p in sorted({0.0, args.dropout if c[0] > 1 else 0.0})]:
         torch.manual_seed(0)
-        base = LSTM(F, T, 1, 256, n_layers=L, bidirectional=D == 2, device=dev)
+        base = LSTM(F, T, 1, 256, n_layers=L, bidirectional=D == 2, device=dev, dropout=p)
         x = torch.randn(B, T, F, device=dev)
         y = torch.randn(B, 1, 1, device=dev)
         g = torch.randn(B, T, D * 256, device=dev)
-        res = {"layers": L, "directions": D, "batch": B, "steps": T, "features": F, "hidden": 256}
+        res = {"layers": L, "directions": D, "batch": B, "steps": T, "features": F, "hidden": 256, "dropout": p}
         for arm in ("k5", "cudnn"):
             m = copy.deepcopy(base)
             m._fused = False if arm == "cudnn" else None

@@ -23,7 +23,8 @@
 // core, reduce-scatter of the 8 partials through DSMEM.  dgates_t is also streamed to global memory and
 // the weight/bias/input gradients are ONE extra kernel over all SMs (they are sums over (t, b), not part
 // of the serial chain).  The x-projection (x_t W_ih^T + b_ih + b_hh for all t) is likewise hoisted out of
-// the recurrence into one small kernel.
+// the recurrence into one small kernel.  Inter-layer dropout is a keep-bit mask per dropped layer output, drawn
+// by a Philox kernel and applied by the next layer's input-side products (lstm_in_mma_kernel<MODE, true>).
 //
 // Replaces cuDNN's RNN kernels.
 #include <cuda.h>
@@ -713,7 +714,50 @@ struct InMmaArgs {
   const float* x;       // layer input [B][T][F]
   float* out;           // MODE_DX: dx [B][T][F];  MODE_WGRAD: workspace [ndir][splits][1024][F + 1]
   int B, T, F, ndir, splits, per;   // per: (t, b) rows of one dW_ih split (a multiple of IK)
+  // inter-layer dropout of x (read only by the DROP instantiations): one keep bit per element of x, element
+  // e = (b T + t) F + f at bit e % 32 of word e / 32; kept elements are multiplied by `scale` = 1 / (1 - p)
+  const uint32_t* keep;
+  float scale;
 };
+
+// ---------------------------------------------------------------------------------------------------
+// inter-layer dropout mask: keep[w] bit i = (element 32 w + i of the layer's output is kept), drawn with
+// Philox4x32-10 (Salmon et al., SC'11): key = seed[0], counter = (e / 4, seed[1]), output word e % 4,
+// kept when it is below `thr` = (1 - p) 2^32.  The seed lives in device memory (drawn by torch's CUDA
+// generator), so a replayed CUDA graph draws a fresh mask.
+// ---------------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint4 philox4x32_10(uint4 ctr, uint2 key) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    const uint32_t lo0 = 0xD2511F53u * ctr.x, hi0 = __umulhi(0xD2511F53u, ctr.x);
+    const uint32_t lo1 = 0xCD9E8D57u * ctr.z, hi1 = __umulhi(0xCD9E8D57u, ctr.z);
+    ctr = make_uint4(hi1 ^ ctr.y ^ key.x, lo1, hi0 ^ ctr.w ^ key.y, lo0);
+    key.x += 0x9E3779B9u;
+    key.y += 0xBB67AE85u;
+  }
+  return ctr;
+}
+
+__global__ void __launch_bounds__(256) lstm_dropout_mask_kernel(uint32_t* __restrict__ keep,
+                                                                const unsigned long long* __restrict__ seed,
+                                                                size_t words, uint32_t thr) {
+  const size_t w = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (w >= words) return;
+  const unsigned long long k = seed[0], off = seed[1];
+  const uint2 key = make_uint2((uint32_t)k, (uint32_t)(k >> 32));
+  uint32_t bits = 0;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const unsigned long long q = w * 8 + j;             // index of the element quad 4 q .. 4 q + 3
+    const uint4 u = philox4x32_10(make_uint4((uint32_t)q, (uint32_t)(q >> 32), (uint32_t)off, (uint32_t)(off >> 32)),
+                                  key);
+    bits |= ((uint32_t)(u.x < thr) | (uint32_t)(u.y < thr) << 1 | (uint32_t)(u.z < thr) << 2 |
+             (uint32_t)(u.w < thr) << 3) << (4 * j);
+  }
+  keep[w] = bits;
+}
+
+__device__ __forceinline__ bool kept(const uint32_t* keep, size_t e) { return (__ldg(keep + (e >> 5)) >> (e & 31)) & 1u; }
 
 // Stage ROWS x 32 fp32 of an operand into K-major swizzled shared memory: element (row, k) of the chunk.
 // K_CONTIG: consecutive k are adjacent in memory (a warp reads one row); otherwise consecutive rows are (a warp
@@ -781,7 +825,10 @@ __device__ __forceinline__ void in_mma_epilogue(const float (&acc)[2][2][16], Pu
                 acc[mh][nq][4 * j + 2 * h + e]);
 }
 
-template <int MODE>
+// DROP: x is the output of the layer below seen through inter-layer dropout (a.keep / a.scale): the x-projection
+// and dW_ih read x * keep * scale, and dx is stored as keep ? dx * scale : 0 (the gradient of the layer below's
+// output).
+template <int MODE, bool DROP>
 __global__ void __launch_bounds__(128, 1) lstm_in_mma_kernel(const InMmaArgs a) {
   __shared__ __align__(1024) uint8_t smem_raw[2 * IBUF];
   const uint32_t smem = smem_u32(smem_raw);
@@ -789,6 +836,17 @@ __global__ void __launch_bounds__(128, 1) lstm_in_mma_kernel(const InMmaArgs a) 
   const int m0 = blockIdx.x * IM, n0 = blockIdx.y * IN;
   // x row of (t, b) index q (x is [B][T][F])
   auto xrow = [&](int q) { return a.x + ((size_t)(q % B) * T + q / B) * F; };
+  // element f of that row, as the layer reads it
+  auto xval = [&](int q, int f) {
+    const float v = __ldg(xrow(q) + f);
+    if constexpr (DROP) return kept(a.keep, ((size_t)(q % B) * T + q / B) * F + f) ? v * a.scale : 0.f;
+    return v;
+  };
+  // dx element (q, f) as stored: masked for the layer below when DROP
+  auto dxval = [&](int q, int f, float v) {
+    if constexpr (DROP) return kept(a.keep, ((size_t)(q % B) * T + q / B) * F + f) ? v * a.scale : 0.f;
+    return v;
+  };
   float acc[2][2][16];
 #pragma unroll
   for (int mh = 0; mh < 2; ++mh)
@@ -801,7 +859,7 @@ __global__ void __launch_bounds__(128, 1) lstm_in_mma_kernel(const InMmaArgs a) 
     const IhDir d = blockIdx.z ? a.d1 : a.d0;
     in_mma_loop<true, true>(
         acc, smem, (F + IK - 1) / IK,
-        [&](int r, int k) { const int q = m0 + r; return (q < TB && k < F) ? __ldg(xrow(q) + k) : 0.f; },
+        [&](int r, int k) { const int q = m0 + r; return (q < TB && k < F) ? xval(q, k) : 0.f; },
         [&](int r, int k) { return k < F ? __ldg(d.w_ih + (size_t)(n0 + r) * F + k) : 0.f; });
     in_mma_epilogue(acc, [&](int m, int n, float v) {
       const int q = m0 + m, r = n0 + n;
@@ -817,7 +875,7 @@ __global__ void __launch_bounds__(128, 1) lstm_in_mma_kernel(const InMmaArgs a) 
         [&](int r, int k) {
           const int q = q0 + k, f = n0 + r;
           if (q >= q1 || f > F) return 0.f;
-          return f == F ? 1.f : __ldg(xrow(q) + f);
+          return f == F ? 1.f : xval(q, f);
         });
     float* ws = a.out + ((size_t)dir * a.splits + split) * LG * (F + 1);
     in_mma_epilogue(acc, [&](int m, int n, float v) {
@@ -830,7 +888,7 @@ __global__ void __launch_bounds__(128, 1) lstm_in_mma_kernel(const InMmaArgs a) 
         [&](int r, int k) { const int f = n0 + r; return f < F ? __ldg(a.d0.w_ih + (size_t)k * F + f) : 0.f; });
     in_mma_epilogue(acc, [&](int m, int n, float v) {
       const int q = m0 + m, f = n0 + n;
-      if (q < TB && f < F) a.out[((size_t)(q % B) * T + q / B) * F + f] = v;
+      if (q < TB && f < F) a.out[((size_t)(q % B) * T + q / B) * F + f] = (DROP && a.ndir == 1) ? dxval(q, f, v) : v;
     });
     if (a.ndir == 2) {                                   // + the reverse direction's sum, read back by its writer
 #pragma unroll
@@ -847,7 +905,7 @@ __global__ void __launch_bounds__(128, 1) lstm_in_mma_kernel(const InMmaArgs a) 
         const int q = m0 + m, f = n0 + n;
         if (q < TB && f < F) {
           float* o = a.out + ((size_t)(q % B) * T + q / B) * F + f;
-          *o = *o + v;
+          *o = dxval(q, f, *o + v);
         }
       });
     }
@@ -917,11 +975,27 @@ int cluster_split(int B, int ndir) {   // clusters per direction
   return cpd;
 }
 
-int check_shape(int ndir, int B, int T, int F) {
+// drop_in / drop_out: the layer's input / output goes through inter-layer dropout with probability p.  A dropped
+// input is the output of a layer below (256 or 512 features), which only the tf32 input products read.
+int check_shape(int ndir, int B, int T, int F, double p, bool drop_in, bool drop_out) {
   if (F < 1 || F > MAX_F || ndir < 1 || ndir > 2 || B < 1 || T < 1)
     return lfail("unsupported LSTM shape: H=256 needs F in 1..512, 1 or 2 directions, B >= 1, T >= 1", F);
+  if ((drop_in || drop_out) && !(p > 0.0 && p <= 1.0))
+    return lfail("unsupported LSTM dropout: a dropout mask needs 0 < p <= 1", (int)(p * 100));
+  if (drop_in && F <= XPROJ_SIMT_MAX_F)
+    return lfail("unsupported LSTM dropout: only the input of a layer above the first (F > 32) is dropped", F);
   return 0;
 }
+
+template <int MODE>
+void launch_in_mma(const InMmaArgs& a, dim3 grid, cudaStream_t st) {
+  if (a.keep != nullptr)
+    lstm_in_mma_kernel<MODE, true><<<grid, 128, 0, st>>>(a);
+  else
+    lstm_in_mma_kernel<MODE, false><<<grid, 128, 0, st>>>(a);
+}
+
+float dropout_scale(double p) { return p < 1.0 ? (float)(1.0 / (1.0 - p)) : 0.f; }
 
 enum { FW_W_IH, FW_W_HH, FW_B_IH, FW_B_HH, FW_H0, FW_C0, FW_XP, FW_GATES, FW_CS, FW_HT, FW_CT, FW_NPTR };
 enum { BW_W_IH, BW_W_HH, BW_H0, BW_C0, BW_GATES, BW_CS, BW_DHT, BW_DCT, BW_DGATES, BW_DH0, BW_DC0, BW_DW_IH,
@@ -942,7 +1016,7 @@ int launch_ih_wgrad(InMmaArgs a, cudaStream_t st) {
   const size_t n = (size_t)a.ndir * a.splits * LG * (a.F + 1);
   cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&a.out), n * sizeof(float), st);
   if (e != cudaSuccess) return lfail(cudaGetErrorString(e), (int)e);
-  lstm_in_mma_kernel<MODE_WGRAD><<<dim3(LG / IM, (a.F + 1 + IN - 1) / IN, a.ndir * a.splits), 128, 0, st>>>(a);
+  launch_in_mma<MODE_WGRAD>(a, dim3(LG / IM, (a.F + 1 + IN - 1) / IN, a.ndir * a.splits), st);
   const size_t outs = (size_t)a.ndir * LG * (a.F + 1);
   lstm_ih_wgrad_finish_kernel<<<(unsigned)((outs + 255) / 256), 256, 0, st>>>(a);
   e = cudaFreeAsync(a.out, st);
@@ -963,11 +1037,22 @@ int b200dp_lstm_rec_supported(int H, int F) { return (H == LH && F >= 1 && F <= 
 // direction d writes columns [256 d, 256 d + 256).  `dir_ptrs` holds FW_NPTR pointers per direction, in the
 // order of the FW_* enum: weights in PyTorch layout, h0/c0/hT/cT [B][256] (slices of the [layers * ndir][B][256]
 // state), the xp workspace [T][B][1024], and gates/cs saved for backward ([T][B][1024] / [T][B][256]) or null.
+// Inter-layer dropout with probability p (null pointers: none): `in_keep` is the keep-bit mask of x (the output
+// of the layer below, as drawn by its forward), which the x-projection applies; `out_keep` [B * T * ndir * 8]
+// words receives a fresh mask of seq drawn from `out_seed` (2 words in device memory: Philox key and offset).
 int b200dp_lstm_rec_fwd(const float* x, float* seq, const void* const* dir_ptrs, int ndir, int B, int T, int F,
+                        double p, const uint32_t* in_keep, const unsigned long long* out_seed, uint32_t* out_keep,
                         unsigned long long stream) {
-  if (check_shape(ndir, B, T, F)) return -1;
+  if (check_shape(ndir, B, T, F, p, in_keep != nullptr, out_keep != nullptr)) return -1;
+  if (out_keep != nullptr && out_seed == nullptr) return lfail("LSTM dropout: an output mask needs a seed");
   cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
   const int rows = T * B;
+  if (out_keep != nullptr) {
+    const size_t words = (size_t)rows * ndir * (LH / 32);
+    const double k = (1.0 - p) * 4294967296.0;        // keep when a 32-bit draw is below (1 - p) 2^32
+    const uint32_t thr = k >= 4294967295.0 ? 0xFFFFFFFFu : (uint32_t)k;
+    lstm_dropout_mask_kernel<<<(unsigned)((words + 255) / 256), 256, 0, st>>>(out_keep, out_seed, words, thr);
+  }
   RecFwdLaunch L{};
   IhDir ih[2] = {};
   L.ndir = ndir; L.B = B; L.T = T; L.ld = LH * ndir;
@@ -983,8 +1068,8 @@ int b200dp_lstm_rec_fwd(const float* x, float* seq, const void* const* dir_ptrs,
                           const_cast<float*>(v[FW_CS]), d};
   }
   if (F > XPROJ_SIMT_MAX_F) {
-    const InMmaArgs a{ih[0], ih[ndir - 1], x, nullptr, B, T, F, ndir, 1, 0};
-    lstm_in_mma_kernel<MODE_XPROJ><<<dim3((rows + IM - 1) / IM, LG / IN, ndir), 128, 0, st>>>(a);
+    const InMmaArgs a{ih[0], ih[ndir - 1], x, nullptr, B, T, F, ndir, 1, 0, in_keep, dropout_scale(p)};
+    launch_in_mma<MODE_XPROJ>(a, dim3((rows + IM - 1) / IM, LG / IN, ndir), st);
   }
   return launch_cluster(lstm_rec_fwd_kernel, L, cluster_split(B, ndir) * ndir, FW_SMEM, st);
 }
@@ -992,10 +1077,12 @@ int b200dp_lstm_rec_fwd(const float* x, float* seq, const void* const* dir_ptrs,
 // Backward of one layer + all its parameter gradients.  seq / dseq [B][T][256 * ndir] as in the forward (dseq
 // may be null); dx [B][T][F] or null; with two directions dx is the sum of both.  `dir_ptrs` holds BW_NPTR
 // pointers per direction in the order of the BW_* enum (dhT/dcT/dh0/dc0 may be null).  dW_hh [1024][256] must be
-// ZERO on entry (split-K atomics); dW_ih / db_ih / db_hh are overwritten.
+// ZERO on entry (split-K atomics); dW_ih / db_ih / db_hh are overwritten.  `in_keep` (or null) is the forward's
+// dropout mask of x with probability p: dW_ih reads the dropped x, and dx is the gradient of the undropped x
+// (the layer below's output), i.e. zero where x was dropped.
 int b200dp_lstm_rec_bwd(const float* x, const float* seq, const float* dseq, float* dx, const void* const* dir_ptrs,
-                        int ndir, int B, int T, int F, unsigned long long stream) {
-  if (check_shape(ndir, B, T, F)) return -1;
+                        int ndir, int B, int T, int F, double p, const uint32_t* in_keep, unsigned long long stream) {
+  if (check_shape(ndir, B, T, F, p, in_keep != nullptr, false)) return -1;
   cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
   const int TB = T * B;
   RecBwdLaunch L{};
@@ -1018,10 +1105,13 @@ int b200dp_lstm_rec_bwd(const float* x, const float* seq, const float* dseq, flo
   if (launch_cluster(lstm_rec_bwd_kernel, L, cluster_split(B, ndir) * ndir, BW_SMEM, st)) return -1;
   const int blocks = (LG / WG_TR) * (LH / WG_TK) * w[0].ksplit + (ih_simt ? LG / 8 : 0) + (dx_simt ? (TB + 7) / 8 : 0);
   for (int d = 0; d < ndir; ++d) lstm_wgrad_kernel<<<blocks, 256, 0, st>>>(w[d]);
-  if (!ih_simt && launch_ih_wgrad(InMmaArgs{ih[0], ih[ndir - 1], x, nullptr, B, T, F, ndir, 1, 0}, st)) return -1;
+  const float scale = dropout_scale(p);
+  if (!ih_simt &&
+      launch_ih_wgrad(InMmaArgs{ih[0], ih[ndir - 1], x, nullptr, B, T, F, ndir, 1, 0, in_keep, scale}, st))
+    return -1;
   if (dx != nullptr && !dx_simt) {
-    const InMmaArgs a{ih[0], ih[ndir - 1], x, dx, B, T, F, ndir, 1, 0};
-    lstm_in_mma_kernel<MODE_DX><<<dim3((TB + IM - 1) / IM, (F + IN - 1) / IN), 128, 0, st>>>(a);
+    const InMmaArgs a{ih[0], ih[ndir - 1], x, dx, B, T, F, ndir, 1, 0, in_keep, scale};
+    launch_in_mma<MODE_DX>(a, dim3((TB + IM - 1) / IM, (F + IN - 1) / IN), st);
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return lfail(cudaGetErrorString(e), (int)e);

@@ -1,7 +1,7 @@
 """LSTM regressor — the reference model (app/torch_train.py:107-206; SURVEY.md §2.1 C6).
 
 Architecture (parity): ``nn.LSTM(n_features -> h_size, n_layers, bidirectional?,
-batch_first)`` -> ``Linear(h*dirs -> h)`` -> ``Linear(h -> 64)`` -> ``Linear(64 -> 1)`` with
+batch_first, dropout)`` -> ``Linear(h*dirs -> h)`` -> ``Linear(h -> 64)`` -> ``Linear(64 -> 1)`` with
 NO activations between the linears (app/torch_train.py:199-205); fresh random ``(h0, c0)``
 every forward (app/torch_train.py:179-193); the last timestep is selected
 (app/torch_train.py:196); output shape ``[B, 1, 1]``.  ``state_dict`` keys are identical to
@@ -12,8 +12,8 @@ H100-first changes (SURVEY.md §2.6 S2/S4, §7.3):
   * ``(h0, c0)`` come from the device generator (no CPU randn + pageable H2D + sync per
     step), the last-step gather is a slice (no host-built index tensor);
   * on CUDA (fp32, hidden size 256, any number of layers, one or two directions, 1..512 input
-    features) forward/backward run on the persistent cluster LSTM kernels (K5: ``ops/lstm_rec.py``,
-    csrc/lstm_rec_sm90.cu — tf32 wgmma, W_hh resident in shared memory, h exchanged through
+    features, inter-layer dropout in [0, 1]) forward/backward run on the persistent cluster LSTM
+    kernels (K5: ``ops/lstm_rec.py``, csrc/lstm_rec_sm90.cu — tf32 wgmma, W_hh resident in shared memory, h exchanged through
     DSMEM; the two directions of a layer run as separate clusters of one launch) and, for batches
     up to 1024, the chained-GEMM head (K6: ``ops/lstm_fused.py``; larger batches use torch's
     linears).  Other hidden sizes, wider inputs and non-fp32 weights use cuDNN / cuBLAS, which is
@@ -33,7 +33,8 @@ class LSTM(nn.Module):
 
     def __init__(self, n_features, window_size, output_size, h_size, n_layers=1,
                  bidirectional=False, device=torch.device('cpu'),
-                 initializers: Optional[Sequence[Callable]] = None, fused: Optional[bool] = None):
+                 initializers: Optional[Sequence[Callable]] = None, fused: Optional[bool] = None,
+                 dropout: float = 0.0):
         super().__init__()
         self.n_features = n_features
         self.window_size = window_size
@@ -44,7 +45,7 @@ class LSTM(nn.Module):
         self.device = torch.device(device)
 
         self.lstm = nn.LSTM(input_size=n_features, hidden_size=h_size, num_layers=n_layers,
-                            bidirectional=bidirectional, batch_first=True)
+                            bidirectional=bidirectional, batch_first=True, dropout=dropout)
         self.hidden = None
         self.linear = nn.Linear(self.h_size * self.directions, self.h_size)
         self.linear2 = nn.Linear(self.h_size, 64)

@@ -93,22 +93,23 @@ _warned_cudnn = False
 
 def recurrence(model, x, hidden):
     """The model's nn.LSTM on the persistent recurrence kernels (K5, ops/lstm_rec.py) for every shape they
-    cover; cuDNN only for the others (hidden size != 256, > 512 input features, dropout, projections,
-    non-fp32 weights)."""
+    cover, inter-layer dropout included; cuDNN only for the others (hidden size != 256, > 512 input features,
+    projections, non-fp32 weights)."""
     from . import lstm_rec
     lstm = model.lstm
     if lstm_rec.stack_supported(lstm, x):
         return lstm_rec.lstm_stack(x, hidden[0], hidden[1], [w for ws in lstm.all_weights for w in ws],
-                                   lstm.num_layers, lstm.bidirectional)
+                                   lstm.num_layers, lstm.bidirectional,
+                                   dropout=lstm.dropout if lstm.training else 0.0)
     global _warned_cudnn
     if not _warned_cudnn:
         _warned_cudnn = True
         import logging
         logging.getLogger("b200dp").warning(
-            "LSTM shape (layers=%d, hidden=%d, features=%d, bidirectional=%s, dropout=%g, proj_size=%d, "
-            "dtype=%s) is outside the persistent recurrence kernels (hidden size 256, 1..512 features, fp32, "
-            "no dropout or projection): using the cuDNN RNN for this module",
-            model.n_layers, model.h_size, model.n_features, model.directions == 2, lstm.dropout,
+            "LSTM shape (layers=%d, hidden=%d, features=%d, bidirectional=%s, proj_size=%d, dtype=%s) is "
+            "outside the persistent recurrence kernels (hidden size 256, 1..512 features, fp32, no "
+            "projection): using the cuDNN RNN for this module",
+            model.n_layers, model.h_size, model.n_features, model.directions == 2,
             getattr(lstm, "proj_size", 0), lstm.weight_hh_l0.dtype)
     return lstm(x, hidden)
 

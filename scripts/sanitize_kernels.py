@@ -59,6 +59,9 @@ m(xs).sum().backward()
 # stacked bidirectional: reverse direction, strided halves of seq, F > 32 input products with a tail
 m2 = LSTM(40, 5, 1, 256, n_layers=2, bidirectional=True, device=torch.device(dev)).to(dev)
 m2(torch.randn(7, 5, 40, device=dev)).sum().backward()
+# inter-layer dropout: the mask kernel and the dropped-input products of the layers above the first
+m3 = LSTM(40, 5, 1, 256, n_layers=3, bidirectional=True, dropout=0.3, device=torch.device(dev)).to(dev)
+m3(torch.randn(7, 5, 40, device=dev)).sum().backward()
 torch.cuda.synchronize()
 
 # fused engine in clip mode on one GPU: several buckets, bf16 parameters with fp32 masters, two steps
