@@ -74,7 +74,27 @@ def parse_args(argv=None):
     p.add_argument("--clip-grad-norm", type=float, default=float(env("B200DP_CLIP_GRAD_NORM", "0")),
                    help="clip the averaged gradient by its global L2 norm to at most this value before "
                         "each update (DistributedOptimizer max_grad_norm=; 0 = off, the reference)")
-    return p.parse_args(argv)
+    p.add_argument("--optimizer", default=env("B200DP_OPTIMIZER", "default"), choices=["default", "lars", "lamb"],
+                   help="image models: 'default' = SGD momentum 0.9, wd 1e-4 (the LSTM always uses Adam); "
+                        "'lars' / 'lamb' = hvd.LARS / hvd.LAMB with biases and norm-layer parameters in a "
+                        "group with adaptive=False and no weight decay")
+    args = p.parse_args(argv)
+    if args.optimizer != "default" and args.model.lower() == "lstm":
+        p.error("--optimizer lars|lamb applies to the image models")
+    return args
+
+
+def image_optimizer(model, kind, lr):
+    """The optimizer of the image models: SGD, or LARS / LAMB with 0/1-dim parameters (biases, BN / LN
+    affine) excluded from weight decay and from the trust ratio."""
+    if kind == "default":
+        return torch.optim.SGD(model.parameters(), lr=lr, momentum=0.9, weight_decay=1e-4)
+    groups = [{"params": [p for p in model.parameters() if p.dim() > 1]},
+              {"params": [p for p in model.parameters() if p.dim() <= 1], "weight_decay": 0.0, "adaptive": False}]
+    groups = [g for g in groups if g["params"]]
+    if kind == "lars":
+        return hvd.LARS(groups, lr=lr, momentum=0.9, weight_decay=1e-4)
+    return hvd.LAMB(groups, lr=lr, weight_decay=0.01)
 
 
 if __name__ == "__main__":
@@ -172,7 +192,7 @@ if __name__ == "__main__":
         train_loader = _SynthLoader()
         test_loader = [batches.next()]
         lr = args.lr if args.lr != 1e-6 else 0.1
-        optimizer = torch.optim.SGD(model.parameters(), lr=lr, momentum=0.9, weight_decay=1e-4)
+        optimizer = image_optimizer(model, args.optimizer, lr)
         loss_fn = nn.CrossEntropyLoss()
 
     if args.cuda_graph and use_cuda:

@@ -44,7 +44,7 @@ struct CommCtx {
   int world;
 };
 
-enum { OPT_NONE = 0, OPT_SGD = 1, OPT_ADAM = 2 };
+enum { OPT_NONE = 0, OPT_SGD = 1, OPT_ADAM = 2, OPT_LARS = 3, OPT_LAMB = 4 };
 
 struct OptHyper {
   int kind;        // OPT_*
@@ -104,6 +104,29 @@ struct ClipArgs {
   float* coef;             // device scalar: min(max_norm / (norm + 1e-6), 1) (K8 writes, K9 reads)
   float max_norm;
   int nslots;              // K8: number of slots (buckets * B200DP_MAX_BLOCKS)
+};
+
+// Layer-wise adaptive optimizers (LARS / LAMB, h.kind OPT_LARS / OPT_LAMB) on the one-shot path.  Each tensor's
+// update is scaled by a trust ratio built from norms over the whole tensor, so the bucket kernel is split in
+// two, both launched from the bucket-ready hook: K10 reduces, forms the update direction into the fp32 arena
+// `r` and writes per-chunk partial sums of squares; K11 folds each tensor's partials into its trust ratio and
+// applies the update.  A chunk is a fixed-size slice of one tensor (the host builds the table once).
+struct LwChunk {
+  int first_vec;  // first 16-byte vector of the chunk in the bucket
+  int nvec;       // vectors in the chunk
+  int tfirst;     // first chunk of the tensor the chunk belongs to (index into this bucket's table)
+  int tcount;     // chunks of that tensor
+};
+
+struct LwArgs {
+  float* r;                // fp32 update direction of this bucket (LARS g + wd w, LAMB m^/(sqrt(v^)+eps) + wd w)
+  float* part;             // per chunk: {sum of w^2, sum of dir^2} (K10 writes, K11 reads)
+  float* ratio;            // per chunk: the tensor's trust ratio, written at the tensor's first chunk (K11)
+  const LwChunk* chunks;   // this bucket's chunk table
+  int nchunks;
+  int adaptive;            // 0: trust ratio 1 (biases, norm layers)
+  float trust_coef;        // LARS eta; 1 for LAMB
+  int pad_;
 };
 
 struct BcastArgs {
@@ -575,6 +598,232 @@ __global__ void __launch_bounds__(512) clip_apply_kernel(CommCtx c, ARArgs a, Cl
   finish_step(a);
 }
 
+// ------------------------------------------------------------------ K10 / K11: LARS / LAMB
+// fp32 master values of VN elements from element `idx`: the master arena, or the fp32 result bucket itself.
+template <typename T, int VN>
+__device__ __forceinline__ void load_master(const ARArgs& a, const T* out_local, size_t idx, float* p) {
+  if (a.master) {
+#pragma unroll
+    for (int i = 0; i < VN; i += 4) {
+      const float4 m = *reinterpret_cast<const float4*>(a.master + idx + i);
+      p[i] = m.x; p[i + 1] = m.y; p[i + 2] = m.z; p[i + 3] = m.w;
+    }
+  } else {
+    Vec<T>::unpack(*reinterpret_cast<const uint4*>(out_local + idx), p);
+  }
+}
+
+// block_sum_fixed for two values at once; the trailing barrier lets the caller run it again at once.
+__device__ __forceinline__ float2 block_sum2_fixed(float x, float y) {
+  __shared__ float2 s_part2[32];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    x += __shfl_xor_sync(0xffffffffu, x, o);
+    y += __shfl_xor_sync(0xffffffffu, y, o);
+  }
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (lane == 0) s_part2[warp] = make_float2(x, y);
+  __syncthreads();
+  float2 t = make_float2(0.0f, 0.0f);
+  if (warp == 0) {
+    if (lane < (int)(blockDim.x >> 5)) t = s_part2[lane];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      t.x += __shfl_xor_sync(0xffffffffu, t.x, o);
+      t.y += __shfl_xor_sync(0xffffffffu, t.y, o);
+    }
+  }
+  __syncthreads();
+  return t;  // valid in thread 0
+}
+
+// K10: K1's reduction (same fixed rank order, same `scale * sum`), then the update direction into `k.r`
+// (LAMB also updates exp_avg / exp_avg_sq in s0 / s1) and, per chunk, the fp32 sums of squares of the master
+// weights and of the direction.  CTAs walk whole chunks, so every partial covers one tensor only and is added
+// in a fixed order; every rank reduces the whole bucket and holds the same bits.  Step counters are read
+// (LAMB bias correction), not bumped.
+template <typename T>
+__global__ void __launch_bounds__(512) allreduce_oneshot_lw_kernel(CommCtx c, ARArgs a, LwArgs k) {
+  constexpr int VN = Vec<T>::N;
+  const T* out_local = reinterpret_cast<const T*>(a.out[c.rank]);
+  const bool lamb = a.h.kind == OPT_LAMB;
+  float bc1 = 1.0f, bc2_sqrt = 1.0f;
+  if (lamb) {
+    const float tf = (float)((a.step_ctr ? *a.step_ctr : 0) + 1);
+    bc1 = 1.0f - powf(a.h.beta1, tf);
+    bc2_sqrt = sqrtf(1.0f - powf(a.h.beta2, tf));
+  }
+
+  if (!rank_barrier(c, a.channel)) return;
+  for (int ch = blockIdx.x; ch < k.nchunks; ch += gridDim.x) {
+    const LwChunk q = k.chunks[ch];
+    float ww = 0.0f, dd = 0.0f;
+    for (int v = q.first_vec + (int)threadIdx.x; v < q.first_vec + q.nvec; v += blockDim.x) {
+      uint4 raw[B200DP_MAX_RANKS];
+#pragma unroll
+      for (int r = 0; r < B200DP_MAX_RANKS; ++r)
+        if (r < c.world) raw[r] = ld_peer_v4(reinterpret_cast<const uint4*>(a.in[r]) + v);
+      float g[VN], f[VN], p[VN];
+#pragma unroll
+      for (int i = 0; i < VN; ++i) g[i] = 0.0f;
+#pragma unroll
+      for (int r = 0; r < B200DP_MAX_RANKS; ++r) {
+        if (r < c.world) {
+          Vec<T>::unpack(raw[r], f);
+#pragma unroll
+          for (int i = 0; i < VN; ++i) g[i] += f[i];
+        }
+      }
+      const size_t idx = (size_t)v * VN;
+      load_master<T, VN>(a, out_local, idx, p);
+#pragma unroll
+      for (int i = 0; i < VN; ++i) g[i] *= a.scale;
+      if (lamb) {
+#pragma unroll
+        for (int i = 0; i < VN; i += 4) {
+          float4 m = *reinterpret_cast<const float4*>(a.s0 + idx + i);
+          float4 s = *reinterpret_cast<const float4*>(a.s1 + idx + i);
+          float* mp = &m.x;
+          float* sp = &s.x;
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const float x = g[i + j];
+            mp[j] = fmaf(a.h.beta1, mp[j], (1.0f - a.h.beta1) * x);
+            sp[j] = fmaf(a.h.beta2, sp[j], (1.0f - a.h.beta2) * x * x);
+            const float denom = sqrtf(sp[j]) / bc2_sqrt + a.h.eps;
+            g[i + j] = fmaf(a.h.weight_decay, p[i + j], (mp[j] / bc1) / denom);
+          }
+          *reinterpret_cast<float4*>(a.s0 + idx + i) = m;
+          *reinterpret_cast<float4*>(a.s1 + idx + i) = s;
+        }
+      } else {
+#pragma unroll
+        for (int i = 0; i < VN; ++i) g[i] = fmaf(a.h.weight_decay, p[i], g[i]);
+      }
+#pragma unroll
+      for (int i = 0; i < VN; ++i) {
+        ww = fmaf(p[i], p[i], ww);
+        dd = fmaf(g[i], g[i], dd);
+      }
+#pragma unroll
+      for (int i = 0; i < VN; i += 4)
+        *reinterpret_cast<float4*>(k.r + idx + i) = make_float4(g[i], g[i + 1], g[i + 2], g[i + 3]);
+    }
+    const float2 s = block_sum2_fixed(ww, dd);
+    if (threadIdx.x == 0) {
+      k.part[2 * ch] = s.x;
+      k.part[2 * ch + 1] = s.y;
+    }
+  }
+  // Zero exactly the vectors this thread read: after the barrier, the CTA of the same index on every peer has
+  // read them too, while other CTAs may still be reading theirs.  Vectors outside every chunk (bucket padding)
+  // are never written, so they stay zero.
+  rank_barrier(c, a.channel);
+  if (a.zero_input) {
+    uint4* mine = reinterpret_cast<uint4*>(const_cast<void*>(a.in[c.rank]));
+    for (int ch = blockIdx.x; ch < k.nchunks; ch += gridDim.x) {
+      const LwChunk q = k.chunks[ch];
+      for (int v = q.first_vec + (int)threadIdx.x; v < q.first_vec + q.nvec; v += blockDim.x)
+        mine[v] = make_uint4(0, 0, 0, 0);
+    }
+  }
+}
+
+// Trust ratio of the tensor whose partials are chunks [first, first + count): thread t adds partials t,
+// t + blockDim, ... in double, then a fixed shuffle / warp tree, so every CTA that needs the ratio computes the
+// same bits without waiting for another.  1 when the group is not adaptive or either norm is not > 0.
+__device__ float lw_trust(const LwArgs& k, int first, int count) {
+  __shared__ double s_w[32], s_d[32];
+  __shared__ float s_ratio;
+  double w = 0.0, d = 0.0;
+  for (int i = threadIdx.x; i < count; i += blockDim.x) {
+    w += (double)k.part[2 * (first + i)];
+    d += (double)k.part[2 * (first + i) + 1];
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    w += __shfl_xor_sync(0xffffffffu, w, o);
+    d += __shfl_xor_sync(0xffffffffu, d, o);
+  }
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (lane == 0) {
+    s_w[warp] = w;
+    s_d[warp] = d;
+  }
+  __syncthreads();
+  if (warp == 0) {
+    const bool live = lane < (int)(blockDim.x >> 5);
+    w = live ? s_w[lane] : 0.0;
+    d = live ? s_d[lane] : 0.0;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      w += __shfl_xor_sync(0xffffffffu, w, o);
+      d += __shfl_xor_sync(0xffffffffu, d, o);
+    }
+    if (lane == 0) {
+      const double wn = sqrt(w), dn = sqrt(d);
+      s_ratio = (k.adaptive && wn > 0.0 && dn > 0.0) ? (float)((double)k.trust_coef * wn / dn) : 1.0f;
+    }
+  }
+  __syncthreads();
+  return s_ratio;
+}
+
+// K11: purely local.  LARS: buf = momentum * buf + (lr * trust) * r, w -= buf.  LAMB: w -= (lr * trust) * r.
+// Writes master, output and LARS state, then bumps the step counter.  A CTA recomputes the ratio only when its
+// next chunk belongs to another tensor.
+template <typename T>
+__global__ void __launch_bounds__(512) lw_apply_kernel(CommCtx c, ARArgs a, LwArgs k) {
+  constexpr int VN = Vec<T>::N;
+  const float lr = a.h.lr * (a.lr_scale ? *a.lr_scale : 1.0f);
+  const bool lamb = a.h.kind == OPT_LAMB;
+  T* out = reinterpret_cast<T*>(a.out[c.rank]);
+  int tensor = -1;
+  float trust = 1.0f;
+  for (int ch = blockIdx.x; ch < k.nchunks; ch += gridDim.x) {
+    const LwChunk q = k.chunks[ch];
+    if (q.tfirst != tensor) {
+      tensor = q.tfirst;
+      trust = lw_trust(k, q.tfirst, q.tcount);
+      if (ch == q.tfirst && threadIdx.x == 0) k.ratio[ch] = trust;
+    }
+    const float step = lr * trust;
+    for (int v = q.first_vec + (int)threadIdx.x; v < q.first_vec + q.nvec; v += blockDim.x) {
+      const size_t idx = (size_t)v * VN;
+      float d[VN], p[VN];
+#pragma unroll
+      for (int i = 0; i < VN; i += 4) {
+        const float4 x = *reinterpret_cast<const float4*>(k.r + idx + i);
+        d[i] = x.x; d[i + 1] = x.y; d[i + 2] = x.z; d[i + 3] = x.w;
+      }
+      load_master<T, VN>(a, out, idx, p);
+      if (lamb) {
+#pragma unroll
+        for (int i = 0; i < VN; ++i) p[i] = fmaf(-step, d[i], p[i]);
+      } else {
+#pragma unroll
+        for (int i = 0; i < VN; i += 4) {
+          float4 b = *reinterpret_cast<const float4*>(a.s0 + idx + i);
+          float* bp = &b.x;
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            bp[j] = fmaf(a.h.momentum, bp[j], step * d[i + j]);
+            p[i + j] -= bp[j];
+          }
+          *reinterpret_cast<float4*>(a.s0 + idx + i) = b;
+        }
+      }
+      if (a.master) {
+#pragma unroll
+        for (int i = 0; i < VN; i += 4)
+          *reinterpret_cast<float4*>(a.master + idx + i) = make_float4(p[i], p[i + 1], p[i + 2], p[i + 3]);
+      }
+      reinterpret_cast<uint4*>(out)[v] = Vec<T>::pack(p);
+    }
+  }
+  finish_step(a);
+}
+
 // ------------------------------------------------------------------ K2: two-shot (P2P) and K3: NVLS
 template <typename T, bool kNVLS>
 __global__ void __launch_bounds__(512) allreduce_sliced_kernel(CommCtx c, ARArgs a) {
@@ -797,6 +1046,14 @@ cudaError_t launch_clip(const CommCtx& c, const ARArgs& a, const ClipArgs& k, bo
   return cudaGetLastError();
 }
 
+template <typename T>
+cudaError_t launch_lw(const CommCtx& c, const ARArgs& a, const LwArgs& k, bool apply, int blocks, int threads,
+                      cudaStream_t st) {
+  if (apply) lw_apply_kernel<T><<<blocks, threads, 0, st>>>(c, a, k);
+  else allreduce_oneshot_lw_kernel<T><<<blocks, threads, 0, st>>>(c, a, k);
+  return cudaGetLastError();
+}
+
 }  // namespace
 
 extern "C" {
@@ -846,6 +1103,33 @@ int b200dp_comm_clip_finalize(const ClipArgs* clip, unsigned long long stream) {
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
     snprintf(g_comm_err, sizeof(g_comm_err), "clip finalize launch: %s", cudaGetErrorString(e));
+    return -1;
+  }
+  return 0;
+}
+
+int b200dp_comm_lw_bytes() { return (int)sizeof(LwArgs); }
+
+// phase: 0 reduce + direction + chunk partials (K10), 1 trust ratios + update + step counter (K11).
+// args->h.kind selects LARS or LAMB.  dtype as in b200dp_comm_allreduce.
+int b200dp_comm_lw_bucket(const CommCtx* ctx, const ARArgs* args, const LwArgs* lw, int phase, int dtype,
+                          int blocks, int threads, unsigned long long stream) {
+  if (blocks < 1 || blocks > B200DP_MAX_BLOCKS || threads < 32 || threads > 512 || (threads & 31) ||
+      ctx->world > B200DP_MAX_RANKS || args->channel < 0 || args->channel >= B200DP_NUM_CHANNELS ||
+      phase < 0 || phase > 1 || (args->h.kind != OPT_LARS && args->h.kind != OPT_LAMB) || lw->nchunks < 0) {
+    snprintf(g_comm_err, sizeof(g_comm_err),
+             "bad layer-wise launch config blocks=%d threads=%d world=%d ch=%d phase=%d kind=%d chunks=%d",
+             blocks, threads, ctx->world, args->channel, phase, args->h.kind, lw->nchunks);
+    return -1;
+  }
+  cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
+  cudaError_t e;
+  if (dtype == 0) e = launch_lw<float>(*ctx, *args, *lw, phase == 1, blocks, threads, st);
+  else if (dtype == 1) e = launch_lw<__nv_bfloat16>(*ctx, *args, *lw, phase == 1, blocks, threads, st);
+  else if (dtype == 2) e = launch_lw<__half>(*ctx, *args, *lw, phase == 1, blocks, threads, st);
+  else e = cudaErrorInvalidValue;
+  if (e != cudaSuccess) {
+    snprintf(g_comm_err, sizeof(g_comm_err), "layer-wise launch: %s", cudaGetErrorString(e));
     return -1;
   }
   return 0;

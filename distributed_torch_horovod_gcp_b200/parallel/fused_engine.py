@@ -16,7 +16,7 @@ Memory plan (per dtype arena, same element layout in every arena):
   P  parameters     symmetric   p.data are views        (peers push updated slices)
   M  fp32 master    local       only when dtype != fp32
   S0 momentum | exp_avg,  S1 exp_avg_sq   local fp32    (sharded by slice for K2/K3)
-  R  fp32 reduced gradient                local         clip mode only (max_grad_norm=)
+  R  fp32 reduced gradient | direction    local         clip mode (max_grad_norm=) and LARS / LAMB only
 
 Clip mode (``max_grad_norm=``) splits each bucket's kernel in two phases, because a global norm needs
 every bucket reduced before any bucket is updated: the bucket-ready hook launches a one-shot reduction
@@ -24,6 +24,13 @@ into R that also leaves one sum-of-squares slot per CTA (K1c); ``wait_all`` then
 that folds all slots into the norm and the clip coefficient (K8) and one local update per bucket that
 scales R by it and runs the unchanged K7 epilogue (K9).  One-shot everywhere means every rank holds the
 same bits of R, so every rank computes the same norm without a further exchange.
+
+LARS / LAMB (``hvd.LARS`` / ``hvd.LAMB``) scale each tensor's update by a trust ratio from norms over that
+whole tensor, so their bucket kernel is split in two as well, but both phases run from the bucket's own hook
+and still overlap backward: a one-shot reduction that writes the update direction to R and one fp32 partial
+sum of squares of the master weights and of the direction per chunk (K10), then a local update that folds
+each tensor's partials into its ratio in fp64 and applies it (K11).  A chunk is a fixed-size slice of one
+tensor; the per-bucket chunk table is built once here and kept on the device, so graph replays reuse it.
 """
 from __future__ import annotations
 
@@ -38,6 +45,9 @@ from ..utils import nvtx
 from .buckets import Bucket, arena_sizes
 
 _ENGINES: "weakref.WeakSet[FusedEngine]" = weakref.WeakSet()
+LW_CHUNK_ELEMS = 16384          # elements per chunk of the LARS / LAMB partial norms
+_LAYERWISE_KINDS = ("lars", "lamb")
+_logged_layerwise_fallback = False
 
 
 def live_engines():
@@ -57,10 +67,15 @@ def arena_view(flat: torch.Tensor, lo: int, param: torch.Tensor) -> torch.Tensor
 
 
 def _classify(opt) -> Optional[str]:
-    """Return 'sgd' | 'adam' | 'adamw' if the wrapped optimizer's update rule is one the fused
-    epilogue implements exactly, else None."""
+    """Return 'sgd' | 'adam' | 'adamw' | 'lars' | 'lamb' if the wrapped optimizer's update rule is one the
+    fused kernels implement exactly, else None."""
+    from ..torch.optim import LARS, LAMB
     if isinstance(opt, torch.optim.SGD):
         return "sgd"
+    if isinstance(opt, LARS):
+        return "lars"
+    if isinstance(opt, LAMB):
+        return "lamb"
     if isinstance(opt, torch.optim.AdamW):
         kind = "adamw"
     elif isinstance(opt, torch.optim.Adam):
@@ -79,8 +94,16 @@ class FusedEngine:
     @staticmethod
     def try_create(opt, buckets: List[Bucket], wire_dtype,
                    max_grad_norm: Optional[float] = None) -> Optional["FusedEngine"]:
+        global _logged_layerwise_fallback
         rt = _state.runtime()
         kind = _classify(opt)
+        if kind in _LAYERWISE_KINDS and (wire_dtype is not None or max_grad_norm is not None):
+            if not _logged_layerwise_fallback:
+                _state.log.warning("%s with %s runs on the generic path (all-reduce, then the optimizer's own "
+                                   "step): the fused engine does not combine them", type(opt).__name__,
+                                   "max_grad_norm" if max_grad_norm is not None else "wire compression")
+                _logged_layerwise_fallback = True
+            kind = None
         ok_dtypes = all(b.dtype in (torch.float32, torch.bfloat16, torch.float16) for b in buckets)
         devs = {b.device for b in buckets}
         wire_ok = wire_dtype is None or (wire_dtype in (torch.bfloat16, torch.float16) and
@@ -125,6 +148,8 @@ class FusedEngine:
         self.predivide = float(getattr(opt, "_gradient_predivide_factor", 1.0) or 1.0)
         self.max_grad_norm = None if max_grad_norm is None else float(max_grad_norm)
         self.clip = self.max_grad_norm is not None
+        self.layerwise = kind in _LAYERWISE_KINDS
+        second_moment = kind in ("adam", "adamw", "lamb")
         self.arenas: Dict[torch.dtype, dict] = {}
         for (dtype, device), n in arena_sizes(buckets).items():
             if self.wire is not None:
@@ -140,7 +165,7 @@ class FusedEngine:
                     "p": torch.zeros(n, dtype=torch.float32, device=device),      # the model's fp32 parameters
                     "M": None,
                     "S0": torch.zeros(n, dtype=torch.float32, device=device),
-                    "S1": torch.zeros(n, dtype=torch.float32, device=device) if kind != "sgd" else None,
+                    "S1": torch.zeros(n, dtype=torch.float32, device=device) if second_moment else None,
                 }
                 continue
             es = torch.empty((), dtype=dtype).element_size()
@@ -154,10 +179,11 @@ class FusedEngine:
                 "M": torch.zeros(n, dtype=torch.float32, device=device)
                 if dtype != torch.float32 else None,
                 "S0": torch.zeros(n, dtype=torch.float32, device=device),
-                "S1": torch.zeros(n, dtype=torch.float32, device=device) if kind != "sgd" else None,
+                "S1": torch.zeros(n, dtype=torch.float32, device=device) if second_moment else None,
             }
         for (dtype, device), n in arena_sizes(buckets).items():
-            self.arenas[dtype]["R"] = torch.zeros(n, dtype=torch.float32, device=device) if self.clip else None
+            self.arenas[dtype]["R"] = torch.zeros(n, dtype=torch.float32, device=device) \
+                if self.clip or self.layerwise else None
         # re-home parameters and gradients into the arenas
         with torch.no_grad():
             for b in buckets:
@@ -188,6 +214,8 @@ class FusedEngine:
             fin.slots, fin.nslots = self.slots.data_ptr(), self.slots.numel()
             fin.norm, fin.coef, fin.max_norm = self.grad_norm.data_ptr(), self.coef.data_ptr(), self.max_grad_norm
             self._fin_args = fin
+        if self.layerwise:
+            self._build_chunks()
         self._done = torch.cuda.Event()
         self.steps = 0
         self.rehomed = 0
@@ -254,7 +282,7 @@ class FusedEngine:
             a.inp[r], a.out[r] = gp[r], pp[r]
         both_mc = ar["G"].mc_ptr != 0 and ar["P"].mc_ptr != 0
         algo = symm.pick_algo(nbytes, need_mc=both_mc)
-        if self.wire is not None or self.clip:
+        if self.wire is not None or self.clip or self.layerwise:
             algo = S.ALGO_ONESHOT            # every rank must hold the full fp32 update / gradient (see __init__)
         if algo == S.ALGO_NVLS and not both_mc:
             algo = S.ALGO_TWOSHOT
@@ -290,6 +318,48 @@ class FusedEngine:
         ap.scale = 1.0
         return k, ap
 
+    def _build_chunks(self):
+        """LARS / LAMB: the chunk table of every bucket (one device tensor, a slice per bucket), the per-chunk
+        partial sums and the per-chunk ratio slots.  Tensors start on a 16-byte boundary, so a vector never
+        straddles two tensors; a tensor's last vector may end in padding, which is zero in every arena and adds
+        nothing to either norm."""
+        S = self.S
+        rows, first = [], {}
+        span = {}
+        for b in self.buckets:
+            vn = 16 // torch.empty((), dtype=b.dtype).element_size()
+            per = LW_CHUNK_ELEMS // vn
+            base = len(rows)
+            for s in b.slots:
+                v0, nv = s.offset // vn, (s.numel + vn - 1) // vn
+                t0, cnt = len(rows) - base, (nv + per - 1) // per
+                if cnt:
+                    first[s.name] = len(rows)
+                rows += [(v0 + c * per, min(per, nv - c * per), t0, cnt) for c in range(cnt)]
+            span[b.index] = (base, len(rows) - base)
+        total = max(len(rows), 1)
+        self.lw_chunks = torch.tensor(rows or [(0, 0, 0, 0)], dtype=torch.int32).to(self.device)
+        self.lw_part = torch.zeros(2 * total, dtype=torch.float32, device=self.device)
+        self.lw_ratio = torch.ones(total, dtype=torch.float32, device=self.device)
+        self._lw_first = first
+        self._lw_args: Dict[int, object] = {}
+        for b in self.buckets:
+            base, n = span[b.index]
+            k = S.LwArgs()
+            k.r = self.arenas[b.dtype]["R"].data_ptr() + 4 * b.flat_offset
+            k.part = self.lw_part.data_ptr() + 8 * base
+            k.ratio = self.lw_ratio.data_ptr() + 4 * base
+            k.chunks = self.lw_chunks.data_ptr() + 16 * base
+            k.nchunks = n
+            self._lw_args[b.index] = k
+
+    def trust_ratios(self) -> Dict[str, torch.Tensor]:
+        """LARS / LAMB: each parameter's trust ratio of the latest update, by name (0-dim fp32 views of a
+        device buffer that every step, graph replays included, rewrites)."""
+        if not self.layerwise:
+            return {}
+        return {name: self.lw_ratio[i] for name, i in self._lw_first.items()}
+
     # ------------------------------------------------------------------ hot path
     def _fill_hyper(self, a, group: dict):
         S, h = self.S, a.h
@@ -302,6 +372,13 @@ class FusedEngine:
             h.momentum = float(group.get("momentum", 0.0))
             h.dampening = float(group.get("dampening", 0.0))
             h.nesterov = int(bool(group.get("nesterov", False)))
+        elif self.kind == "lars":
+            h.kind = S.OPT_LARS
+            h.momentum = float(group["momentum"])
+        elif self.kind == "lamb":
+            h.kind = S.OPT_LAMB
+            b1, b2 = group["betas"]
+            h.beta1, h.beta2, h.eps = float(b1), float(b2), float(group["eps"])
         else:
             h.kind = S.OPT_ADAM
             b1, b2 = group["betas"]
@@ -337,6 +414,14 @@ class FusedEngine:
         kbytes = b.numel * torch.empty((), dtype=kdtype).element_size()
         if self.clip:
             self.symm.launch_clip_bucket(a, self._clip_args[b.index], self.S.CLIP_REDUCE, kdtype, kbytes, self.side)
+        elif self.layerwise:
+            group = self.opt.param_groups[b.group_index]
+            k = self._lw_args[b.index]
+            k.adaptive = int(bool(group["adaptive"]))
+            k.trust_coef = float(group["trust_coefficient"]) if self.kind == "lars" else 1.0
+            self.symm.launch_lw_bucket(a, k, self.S.LW_REDUCE, kdtype, kbytes, self.side)
+            self.symm.launch_lw_bucket(a, k, self.S.LW_APPLY, kdtype, kbytes, self.side)
+            self.kernel_launches += 1
         else:
             self.symm.launch_allreduce(a, self._algo[b.index], kdtype, kbytes, self.side)
         nvtx.pop()
@@ -428,6 +513,8 @@ class FusedEngine:
                 if self.kind == "sgd":
                     if opt.param_groups[b.group_index].get("momentum", 0.0) != 0.0:
                         st["momentum_buffer"] = v0
+                elif self.kind == "lars":
+                    st["momentum_buffer"] = v0
                 else:
                     st["step"] = torch.tensor(float(steps_dev))
                     st["exp_avg"] = v0
@@ -443,7 +530,7 @@ class FusedEngine:
             for s in b.slots:
                 st = opt.state.get(s.param, {})
                 lo = b.flat_offset + s.offset
-                if self.kind == "sgd":
+                if self.kind in ("sgd", "lars"):
                     mb = st.get("momentum_buffer")
                     if mb is not None:
                         arena_view(ar["S0"], lo, s.param).copy_(mb)

@@ -86,6 +86,7 @@ class LocalRuntime:
     launch_allreduce = S.SymmRuntime.launch_allreduce
     launch_clip_bucket = S.SymmRuntime.launch_clip_bucket
     launch_clip_finalize = S.SymmRuntime.launch_clip_finalize
+    launch_lw_bucket = S.SymmRuntime.launch_lw_bucket
 
     def allreduce_(self, t, prescale=1.0, postscale=1.0, algo=None):
         if prescale * postscale != 1.0:

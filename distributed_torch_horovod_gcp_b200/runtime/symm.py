@@ -27,7 +27,7 @@ CH_ENGINE, CH_USER, CH_BCAST, CH_OPT = 0, 1, 2, 3
 ALGO_ONESHOT, ALGO_TWOSHOT, ALGO_NVLS = 0, 1, 2
 ALGO_NAMES = {0: "oneshot", 1: "twoshot", 2: "nvls"}
 _DTYPE_CODE = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}
-OPT_NONE, OPT_SGD, OPT_ADAM = 0, 1, 2
+OPT_NONE, OPT_SGD, OPT_ADAM, OPT_LARS, OPT_LAMB = 0, 1, 2, 3, 4
 
 
 class CommCtx(ctypes.Structure):
@@ -60,6 +60,20 @@ class ClipArgs(ctypes.Structure):
 
 
 CLIP_REDUCE, CLIP_APPLY = 0, 1
+
+
+class LwChunk(ctypes.Structure):
+    _fields_ = [("first_vec", ctypes.c_int), ("nvec", ctypes.c_int), ("tfirst", ctypes.c_int),
+                ("tcount", ctypes.c_int)]
+
+
+class LwArgs(ctypes.Structure):
+    _fields_ = [("r", ctypes.c_uint64), ("part", ctypes.c_uint64), ("ratio", ctypes.c_uint64),
+                ("chunks", ctypes.c_uint64), ("nchunks", ctypes.c_int), ("adaptive", ctypes.c_int),
+                ("trust_coef", ctypes.c_float), ("pad_", ctypes.c_int)]
+
+
+LW_REDUCE, LW_APPLY = 0, 1
 
 
 class BcastArgs(ctypes.Structure):
@@ -236,15 +250,16 @@ class SymmRuntime:
         L.b200dp_comm_broadcast.argtypes = [P(CommCtx), P(BcastArgs), i, i, u64]
         L.b200dp_comm_clip_bucket.argtypes = [P(CommCtx), P(ARArgs), P(ClipArgs), i, i, i, i, u64]
         L.b200dp_comm_clip_finalize.argtypes = [P(ClipArgs), u64]
+        L.b200dp_comm_lw_bucket.argtypes = [P(CommCtx), P(ARArgs), P(LwArgs), i, i, i, i, u64]
         if hasattr(L, "b200dp_comm_collective"):
             L.b200dp_comm_collective.argtypes = [P(CommCtx), P(CollArgs), i, i, i, i, u64]
             if L.b200dp_comm_coll_bytes() != ctypes.sizeof(CollArgs):
                 raise RuntimeError("ctypes/C struct layout mismatch: CollArgs")
         lim = [ctypes.c_int() for _ in range(6)]
         L.b200dp_comm_limits(*[ctypes.byref(x) for x in lim])
-        got = tuple(x.value for x in lim) + (L.b200dp_comm_clip_bytes(),)
+        got = tuple(x.value for x in lim) + (L.b200dp_comm_clip_bytes(), L.b200dp_comm_lw_bytes())
         want = (MAX_RANKS, MAX_BLOCKS, NUM_CHANNELS, ctypes.sizeof(CommCtx), ctypes.sizeof(ARArgs),
-                ctypes.sizeof(BcastArgs), ctypes.sizeof(ClipArgs))
+                ctypes.sizeof(BcastArgs), ctypes.sizeof(ClipArgs), ctypes.sizeof(LwArgs))
         if got != want:
             raise RuntimeError(f"ctypes/C struct layout mismatch: C={got} python={want}")
 
@@ -406,6 +421,17 @@ class SymmRuntime:
     def launch_clip_finalize(self, clip: ClipArgs, stream: torch.cuda.Stream):
         """Sum every bucket's norm slots (fixed order) into the global norm and the clip coefficient."""
         rc = self.lib.b200dp_comm_clip_finalize(ctypes.byref(clip), stream.cuda_stream)
+        if rc != 0:
+            raise RuntimeError((self.lib.b200dp_comm_last_error() or b"").decode())
+        self.launches += 1
+
+    def launch_lw_bucket(self, args: ARArgs, lw: LwArgs, phase: int, dtype: torch.dtype, nbytes: int,
+                         stream: torch.cuda.Stream):
+        """One bucket of a LARS / LAMB engine: ``LW_REDUCE`` (one-shot reduction, update direction into
+        ``lw.r``, per-chunk sums of squares) or ``LW_APPLY`` (per-tensor trust ratios, update, step counter)."""
+        blocks = self.pick_blocks(ALGO_ONESHOT, nbytes)
+        rc = self.lib.b200dp_comm_lw_bucket(ctypes.byref(self.ctx), ctypes.byref(args), ctypes.byref(lw),
+                                            phase, _DTYPE_CODE[dtype], blocks, 512, stream.cuda_stream)
         if rc != 0:
             raise RuntimeError((self.lib.b200dp_comm_last_error() or b"").decode())
         self.launches += 1

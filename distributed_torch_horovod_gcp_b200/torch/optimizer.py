@@ -475,7 +475,8 @@ def DistributedOptimizer(optimizer, named_parameters=None, compression=Compressi
 
     Arguments follow Horovod (SURVEY.md §2.3 A6); ``bucket_bytes``, ``fused`` and
     ``max_grad_norm`` are H100-runtime extensions (``fused=None`` → use the fused sm_90a kernel
-    when the optimizer is plain SGD(-momentum) / Adam / AdamW on CUDA with the symmetric runtime;
+    when the optimizer is plain SGD(-momentum) / Adam / AdamW / ``hvd.LARS`` / ``hvd.LAMB`` on CUDA with
+    the symmetric runtime;
     ``max_grad_norm=X`` → clip the reduced gradient by its global L2 norm before every update, as
     ``torch.nn.utils.clip_grad_norm_(params, X)`` would; the norm is ``optimizer.grad_norm``).
     """

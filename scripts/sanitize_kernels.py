@@ -4,7 +4,8 @@ Shapes are small (the tools slow kernels 10-100x) but cover: multi-tile persiste
 CTA are not reachable at these sizes on 132 SMs, so max_ctas is forced down where the API allows), the
 statistics / residual / masked-residual / split-K epilogues (per-CTA statistics slots, last-arriver split-K
 reduction, fp32 and bf16 add / store outputs), 3x3 / strided / 1x1 conv paths incl. split-K wgrad, BN, LN, pooling, attention and the LSTM
-recurrence, plus the fused engine's clip-by-global-norm kernels (reduce into R with norm slots, finalize, update)."""
+recurrence, plus the fused engine's clip-by-global-norm kernels (reduce into R with norm slots, finalize, update) and its
+LARS / LAMB kernels (reduce + direction + chunk partials, trust ratios + update)."""
 import os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from distributed_torch_horovod_gcp_b200.ops import kernels, gemm as G, conv as C, bn as B
@@ -78,5 +79,20 @@ for _ in range(2):
     opt.zero_grad()
 torch.cuda.synchronize()
 print("clip ok", float(opt.grad_norm))
+# LARS / LAMB: reduce + direction + chunk partials, then ratios + update; bf16 buckets of several tensors, and
+# an fp32 tensor of several chunks shared by several CTAs
+for kind, dt, width in (("lamb", bf, 100), ("lars", torch.float32, 400)):
+    net = nn.Sequential(nn.Linear(96, width), nn.ReLU(), nn.Linear(width, 7)).to(dev).to(dt)
+    groups = [{"params": [p for p in net.parameters() if p.dim() > 1]},
+              {"params": [p for p in net.parameters() if p.dim() == 1], "weight_decay": 0.0, "adaptive": False}]
+    base = hvd.LAMB(groups, lr=1e-3) if kind == "lamb" else hvd.LARS(groups, lr=0.1, weight_decay=1e-4)
+    opt = hvd.DistributedOptimizer(base, named_parameters=net.named_parameters(), bucket_bytes=4096)
+    assert opt.fused_engine is not None and opt.fused_engine.layerwise
+    for _ in range(2):
+        net(torch.randn(8, 96, device=dev, dtype=dt)).float().square().mean().backward()
+        opt.step()
+        opt.zero_grad()
+    torch.cuda.synchronize()
+    print(kind, "ok", float(opt.fused_engine.lw_ratio.sum()))
 hvd.shutdown()
 print("all ok")
