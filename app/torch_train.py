@@ -11,7 +11,8 @@ gradient averaging through ``hvd.DistributedOptimizer`` and an initial
 
 Optional flags / environment variables (all default to the reference behaviour) select the
 [DRIVER] benchmark variants from BASELINE.json (``--model resnet18|resnet50|resnet152|
-vit_b_16``, ``--dtype bf16``, ``--device cpu`` for the CPU/Gloo plumbing config, …).
+vit_b_16``, ``--dtype bf16``, ``--device cpu`` for the CPU/Gloo plumbing config, …), and the
+GPT-2 causal language model on synthetic tokens (``--model gpt2|gpt-tiny``, ``--seq-len``).
 """
 import argparse
 import datetime
@@ -31,7 +32,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import distributed_torch_horovod_gcp_b200.torch as hvd  # noqa: E402
 from distributed_torch_horovod_gcp_b200.data import (  # noqa: E402,F401
     x_cols, y_cols, read_file_from_aws, reshape_and_scale_data_for_training, TimeSeriesDataSet,
-    MinMaxScaler, StandardScaler, ensure_dataset, DeviceBatchLoader, SyntheticImageBatches)
+    MinMaxScaler, StandardScaler, ensure_dataset, DeviceBatchLoader, SyntheticImageBatches, SyntheticTokenBatches)
 from distributed_torch_horovod_gcp_b200.models import LSTM, build as build_model  # noqa: E402
 from distributed_torch_horovod_gcp_b200.utils import getGPUs  # noqa: E402
 
@@ -55,7 +56,9 @@ def parse_args(argv=None):
     p.add_argument("--image-size", type=int, default=int(env("B200DP_IMAGE_SIZE", "0")))
     p.add_argument("--num-classes", type=int, default=int(env("B200DP_NUM_CLASSES", "0")))
     p.add_argument("--steps-per-epoch", type=int, default=int(env("B200DP_STEPS_PER_EPOCH", "20")),
-                   help="synthetic image models only")
+                   help="synthetic image and GPT models only")
+    p.add_argument("--seq-len", type=int, default=int(env("B200DP_SEQ_LEN", "0")),
+                   help="GPT models: tokens per sequence (0 = the model's context)")
     p.add_argument("--no-validate", action="store_true")
     p.add_argument("--cuda-graph", action="store_true",
                    default=env("B200DP_CUDA_GRAPH", "0") == "1",
@@ -75,7 +78,8 @@ def parse_args(argv=None):
                    help="clip the averaged gradient by its global L2 norm to at most this value before "
                         "each update (DistributedOptimizer max_grad_norm=; 0 = off, the reference)")
     p.add_argument("--optimizer", default=env("B200DP_OPTIMIZER", "default"), choices=["default", "lars", "lamb"],
-                   help="image models: 'default' = SGD momentum 0.9, wd 1e-4 (the LSTM always uses Adam); "
+                   help="image models: 'default' = SGD momentum 0.9, wd 1e-4 (the LSTM always uses Adam; "
+                        "the GPT models AdamW, see gpt_optimizer); "
                         "'lars' / 'lamb' = hvd.LARS / hvd.LAMB with biases and norm-layer parameters in a "
                         "group with adaptive=False and no weight decay")
     args = p.parse_args(argv)
@@ -95,6 +99,18 @@ def image_optimizer(model, kind, lr):
     if kind == "lars":
         return hvd.LARS(groups, lr=lr, momentum=0.9, weight_decay=1e-4)
     return hvd.LAMB(groups, lr=lr, weight_decay=0.01)
+
+
+def is_gpt(name):
+    return name.lower().replace("-", "").replace("_", "") in ("gpt2", "gpttiny")
+
+
+def gpt_optimizer(model, lr):
+    """The GPT-2 recipe: AdamW, betas (0.9, 0.95), weight decay 0.1 on matrices and embeddings (2 or more
+    dimensions), none on biases and LayerNorm parameters."""
+    groups = [{"params": [p for p in model.parameters() if p.dim() >= 2], "weight_decay": 0.1},
+              {"params": [p for p in model.parameters() if p.dim() < 2], "weight_decay": 0.0}]
+    return torch.optim.AdamW(groups, lr=lr, betas=(0.9, 0.95))
 
 
 if __name__ == "__main__":
@@ -167,6 +183,23 @@ if __name__ == "__main__":
                      dropout=args.lstm_dropout)
         optimizer = torch.optim.Adam(model.parameters(), lr=args.lr)
         loss_fn = nn.MSELoss(reduction="mean")
+    elif is_gpt(args.model):
+        model = build_model(args.model).to(_DEVICE)
+        if compute_dtype != torch.float32:
+            model = model.to(compute_dtype)
+        seq_len = args.seq_len or model.context
+        tokens = SyntheticTokenBatches(args.batch_size, seq_len, model.vocab, _DEVICE, seed=hvd.rank())
+
+        class _TokenLoader:
+            def __iter__(self_inner):
+                for _ in range(args.steps_per_epoch):
+                    yield tokens.next()
+        train_loader = _TokenLoader()
+        test_loader = [tokens.next()]
+        lr = args.lr if args.lr != 1e-6 else 6e-4
+        optimizer = gpt_optimizer(model, lr) if args.optimizer == "default" else \
+            image_optimizer(model, args.optimizer, lr)
+        loss_fn = nn.CrossEntropyLoss()
     else:
         small = args.model.lower().replace("-", "").replace("_", "") == "resnet18" and not use_cuda
         image_size = args.image_size or (32 if small else 224)

@@ -1,6 +1,6 @@
-// Flash attention for sm_90a (bf16, head dim 64, non-causal): forward and backward on wgmma.
+// Flash attention for sm_90a (bf16, head dim 64, optionally causal): forward and backward on wgmma.
 //
-//   O = softmax(Q K^T / sqrt(d)) V           per (batch, head); S x S scores never leave the SM.
+//   O = softmax(Q K^T / sqrt(d) [+ causal mask]) V     per (batch, head); S x S scores never leave the SM.
 //
 // Forward, one CTA per (batch, head, 128-query tile), 288 threads:
 //   warp 8          TMA producer: Q tile once, then K_0, V_0, K_1, V_1, ... through a 3-tile ring
@@ -18,7 +18,13 @@
 // accumulators resident in registers across the query loop), and its 64 query rows of dQ_i = dS K_j go
 // out as fp32 RED.ADDs into a workspace (the only cross-CTA reduction).
 //
-// Replaces F.scaled_dot_product_attention (cuDNN / flash library kernels) on the ViT-B/16 path.
+// Causal (CAUSAL = true, query i sees keys 0..i): query and key tiles are both 128 wide, so only the
+// diagonal tile is partly masked.  Forward query tile qt visits KV tiles 0..qt; backward KV block kb visits
+// query tiles kb..q_tiles-1; on the diagonal tile a key column past the query row is dropped wherever the
+// sequence-tail mask drops columns (row max, P, dS), so masked products are exact zeros.  The causal grids
+// launch the longest tiles first.
+//
+// Replaces F.scaled_dot_product_attention (cuDNN / flash library kernels) on the ViT-B/16 and GPT paths.
 // The reference application has no attention.
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -83,6 +89,7 @@ constexpr int FW_SMEM = TILE_BYTES * (1 + FW_RING) + 2 * TILE_BYTES /*P*/ + 1024
 
 // Fragment of an m64 x N wgmma accumulator held by thread t of a warpgroup: element 4j + e is row
 // 16 (t / 32) + (t % 32) / 4 + 8 (e / 2), column 8 j + 2 (t % 4) + e % 2.
+template <bool CAUSAL>
 __global__ void __launch_bounds__(AT, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                 const __grid_constant__ CUtensorMap map_v, const AttnFwdParams p) {
@@ -98,10 +105,11 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
   uint64_t* kv_empty = bars + 4;                         // [3]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int qt = blockIdx.x % p.q_tiles;
-  const int bh = blockIdx.x / p.q_tiles;
+  const int BH = p.B * p.H;
+  const int qt = CAUSAL ? p.q_tiles - 1 - blockIdx.x / BH : blockIdx.x % p.q_tiles;
+  const int bh = CAUSAL ? blockIdx.x % BH : blockIdx.x / p.q_tiles;
   const int h = bh % p.H, b = bh / p.H;
-  const int nb = p.kv_blocks;
+  const int nb = CAUSAL ? qt + 1 : p.kv_blocks;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_q);
@@ -159,12 +167,14 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
       }
       if (leader) mbar_arrive(&kv_empty[st]);
       // ---- online softmax on the fragment
+      const bool diag = CAUSAL && j == qt;                // causal diagonal tile: key column <= query row
       float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
       for (int jj = 0; jj < TILE / 8; ++jj)
 #pragma unroll
         for (int e = 0; e < 4; ++e)
-          if (8 * jj + cq + (e & 1) < valid) mx[e >> 1] = fmaxf(mx[e >> 1], sc[4 * jj + e]);
+          if (8 * jj + cq + (e & 1) < valid && (!diag || 8 * jj + cq + (e & 1) <= r0 + 8 * (e >> 1)))
+            mx[e >> 1] = fmaxf(mx[e >> 1], sc[4 * jj + e]);
       float mn[2], alpha[2];
 #pragma unroll
       for (int h2 = 0; h2 < 2; ++h2) {
@@ -178,7 +188,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
         float pe[4];
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
-          pe[e] = (8 * jj + cq + (e & 1) < valid) ? ex2(fmaf(sc[4 * jj + e], p.scale_log2, -mn[e >> 1])) : 0.f;
+          pe[e] = (8 * jj + cq + (e & 1) < valid && (!diag || 8 * jj + cq + (e & 1) <= r0 + 8 * (e >> 1)))
+                      ? ex2(fmaf(sc[4 * jj + e], p.scale_log2, -mn[e >> 1])) : 0.f;
           l[e >> 1] += pe[e];
         }
         st_pair_sw(sP_u, r0, 8 * jj + cq, TILE_BYTES, pe[0], pe[1]);
@@ -267,6 +278,7 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const __nv_bfloat16* __
 constexpr int BW_RING = 2;
 constexpr int BW_SMEM = TILE_BYTES * (2 + 2 * BW_RING) + 4 * TILE_BYTES + 1024 + 256;
 
+template <bool CAUSAL>
 __global__ void __launch_bounds__(AT, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                 const __grid_constant__ CUtensorMap map_v, const __grid_constant__ CUtensorMap map_do,
@@ -285,10 +297,12 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
   uint64_t* r_empty = bars + 3;                          // [2]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int kb = blockIdx.x % p.kv_blocks;
-  const int bh = blockIdx.x / p.kv_blocks;
+  const int BH = p.B * p.H;
+  const int kb = CAUSAL ? blockIdx.x / BH : blockIdx.x % p.kv_blocks;
+  const int bh = CAUSAL ? blockIdx.x % BH : blockIdx.x / p.kv_blocks;
   const int h = bh % p.H, b = bh / p.H;
   const int nq = p.q_tiles;
+  const int i0 = CAUSAL ? kb : 0;                        // first query tile that sees this key block
   const int kvalid = min(TILE, p.S - kb * TILE);
 
   if (threadIdx.x == 0) {
@@ -310,9 +324,9 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
       mbar_expect_tx(kv_full, 2 * TILE_BYTES);
       tma_load_4d(&map_k, kv_full, sK, 0, kb * TILE, h, b);
       tma_load_4d(&map_v, kv_full, sV, 0, kb * TILE, h, b);
-      for (int i = 0; i < nq; ++i) {
-        const int st = i % BW_RING;
-        mbar_wait(&r_empty[st], ((i / BW_RING) & 1) ^ 1);
+      for (int i = i0; i < nq; ++i) {
+        const int st = (i - i0) % BW_RING;
+        mbar_wait(&r_empty[st], (((i - i0) / BW_RING) & 1) ^ 1);
         mbar_expect_tx(&r_full[st], 2 * TILE_BYTES);
         tma_load_4d(&map_q, &r_full[st], sR + (2 * st) * TILE_BYTES, 0, i * TILE, h, b);
         tma_load_4d(&map_do, &r_full[st], sR + (2 * st + 1) * TILE_BYTES, 0, i * TILE, h, b);
@@ -339,10 +353,10 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
 #pragma unroll
     for (int i = 0; i < HD / 2; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
     mbar_wait(kv_full, 0);
-    for (int i = 0; i < nq; ++i) {
-      const int st = i % BW_RING;
+    for (int i = i0; i < nq; ++i) {
+      const int st = (i - i0) % BW_RING;
       const uint32_t sQ_u = smem_u32(sR + (2 * st) * TILE_BYTES), sO_u = sQ_u + TILE_BYTES;
-      mbar_wait(&r_full[st], (i / BW_RING) & 1);
+      mbar_wait(&r_full[st], ((i - i0) / BW_RING) & 1);
       // ---- S = Q_i K_j^T, dP = dO_i V_j^T for this warpgroup's 64 query rows
       float sc[TILE / 2], dp[TILE / 2];
       {
@@ -361,6 +375,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
       // ---- P = exp2(S c - LSE), dS = P (dP - D) / sqrt(d) -> bf16 smem
       float lse2[2], dl[2];
       bool qok[2];
+      const bool diag = CAUSAL && i == kb;                // causal diagonal tile: key column <= query row
 #pragma unroll
       for (int h2 = 0; h2 < 2; ++h2) {
         const int qrow = i * TILE + r0 + 8 * h2;
@@ -374,7 +389,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
           const int h2 = e >> 1;
-          const bool ok = qok[h2] && (8 * jj + cq + (e & 1) < kvalid);
+          const bool ok = qok[h2] && (8 * jj + cq + (e & 1) < kvalid) && (!diag || 8 * jj + cq + (e & 1) <= r0 + 8 * h2);
           const float pe = ok ? ex2(fmaf(sc[4 * jj + e], p.scale_log2, -lse2[h2])) : 0.f;
           pv[e] = pe;
           ds[e] = pe * (dp[4 * jj + e] - dl[h2]) * p.scale;
@@ -454,12 +469,15 @@ extern "C" {
 
 const char* b200dp_attn_last_error() { return g_err; }
 
-// strides: element strides {batch, head, seq} of each tensor (head dim 64 contiguous)
-int b200dp_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int B, int H, int S, int D,
-                    const long long* qs, const long long* ks, const long long* vs, const long long* os, float scale,
-                    unsigned long long stream) {
+// strides: element strides {batch, head, seq} of each tensor (head dim 64 contiguous).  causal: 0 or 1 (query i
+// sees keys 0..i; q, k and v share one sequence length S, so the mask always applies).
+int b200dp_attn_fwd_ex(const void* q, const void* k, const void* v, void* o, float* lse, int B, int H, int S, int D,
+                       const long long* qs, const long long* ks, const long long* vs, const long long* os, float scale,
+                       int causal, unsigned long long stream) {
   if (ensure_init()) return -1;
   if (D != HD) return fail("head dim must be 64");
+  if (causal != 0 && causal != 1) return fail("causal must be 0 or 1");
+  if (B < 1 || H < 1 || S < 1) return fail("attention shapes must be positive");
   CUtensorMap mq, mk, mv;
   if (make_qkv_map(&mq, q, B, H, S, qs[0], qs[1], qs[2]) || make_qkv_map(&mk, k, B, H, S, ks[0], ks[1], ks[2]) ||
       make_qkv_map(&mv, v, B, H, S, vs[0], vs[1], vs[2]))
@@ -473,21 +491,37 @@ int b200dp_attn_fwd(const void* q, const void* k, const void* v, void* o, float*
   p.o = reinterpret_cast<__nv_bfloat16*>(o);
   p.o_sb = os[0]; p.o_sh = os[1]; p.o_ss = os[2];
   p.lse = lse;
-  if (smem_attr_once<attn_fwd_kernel>(FW_SMEM)) return -1;
-  attn_fwd_kernel<<<B * H * p.q_tiles, AT, FW_SMEM, (cudaStream_t)(uintptr_t)stream>>>(mq, mk, mv, p);
+  const dim3 grid(B * H * p.q_tiles);
+  cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
+  if (causal) {
+    if (smem_attr_once<attn_fwd_kernel<true>>(FW_SMEM)) return -1;
+    attn_fwd_kernel<true><<<grid, AT, FW_SMEM, st>>>(mq, mk, mv, p);
+  } else {
+    if (smem_attr_once<attn_fwd_kernel<false>>(FW_SMEM)) return -1;
+    attn_fwd_kernel<false><<<grid, AT, FW_SMEM, st>>>(mq, mk, mv, p);
+  }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(cudaGetErrorString(e), (int)e);
   return 0;
+}
+
+// The non-causal forward under its original signature, which Python callers bind with fixed ctypes argtypes.
+int b200dp_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int B, int H, int S, int D,
+                    const long long* qs, const long long* ks, const long long* vs, const long long* os, float scale,
+                    unsigned long long stream) {
+  return b200dp_attn_fwd_ex(q, k, v, o, lse, B, H, S, D, qs, ks, vs, os, scale, 0, stream);
 }
 
 // dq_acc: fp32 workspace (strides dqs, 64 contiguous) zeroed by the caller; delta: [B][H][S] fp32 workspace
 int b200dp_attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* dout, const float* lse,
                     float* delta, float* dq_acc, void* dk, void* dv, int B, int H, int S, int D, const long long* qs,
                     const long long* ks, const long long* vs, const long long* os, const long long* dos,
-                    const long long* dqs, const long long* dks, const long long* dvs, float scale,
+                    const long long* dqs, const long long* dks, const long long* dvs, float scale, int causal,
                     unsigned long long stream) {
   if (ensure_init()) return -1;
   if (D != HD) return fail("head dim must be 64");
+  if (causal != 0 && causal != 1) return fail("causal must be 0 or 1");
+  if (B < 1 || H < 1 || S < 1) return fail("attention shapes must be positive");
   cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
   CUtensorMap mq, mk, mv, mdo;
   if (make_qkv_map(&mq, q, B, H, S, qs[0], qs[1], qs[2]) || make_qkv_map(&mk, k, B, H, S, ks[0], ks[1], ks[2]) ||
@@ -509,8 +543,14 @@ int b200dp_attn_bwd(const void* q, const void* k, const void* v, const void* o, 
   p.dk = reinterpret_cast<__nv_bfloat16*>(dk); p.dv = reinterpret_cast<__nv_bfloat16*>(dv);
   p.dk_sb = dks[0]; p.dk_sh = dks[1]; p.dk_ss = dks[2];
   p.dv_sb = dvs[0]; p.dv_sh = dvs[1]; p.dv_ss = dvs[2];
-  if (smem_attr_once<attn_bwd_kernel>(BW_SMEM)) return -1;
-  attn_bwd_kernel<<<B * H * p.kv_blocks, AT, BW_SMEM, st>>>(mq, mk, mv, mdo, p);
+  const dim3 grid(B * H * p.kv_blocks);
+  if (causal) {
+    if (smem_attr_once<attn_bwd_kernel<true>>(BW_SMEM)) return -1;
+    attn_bwd_kernel<true><<<grid, AT, BW_SMEM, st>>>(mq, mk, mv, mdo, p);
+  } else {
+    if (smem_attr_once<attn_bwd_kernel<false>>(BW_SMEM)) return -1;
+    attn_bwd_kernel<false><<<grid, AT, BW_SMEM, st>>>(mq, mk, mv, mdo, p);
+  }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(cudaGetErrorString(e), (int)e);
   return 0;

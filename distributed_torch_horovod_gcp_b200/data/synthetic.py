@@ -5,6 +5,8 @@ data of the benchmark's shape").
 device on a copy stream (double-buffered), so an end-to-end step really contains the H2D
 copy of that step's inputs — the e2e number in bench.py counts these bytes.
 
+``SyntheticTokenBatches`` draws language-model token batches directly on the device.
+
 ``DeviceBatchLoader`` is the H100-first replacement for the reference's
 DataLoader+DistributedSampler on tiny tensors (app/torch_train.py:248-251): the whole
 (small) training set lives on the device, the sharded permutation is computed once per
@@ -64,6 +66,22 @@ class SyntheticImageBatches:
             y.record_stream(torch.cuda.current_stream())
         self._staged = self._stage()
         return x, y
+
+
+class SyntheticTokenBatches:
+    """Language-model batches of uniform random tokens drawn on ``device`` from a seeded generator:
+    ``next()`` returns (inputs [B, S], targets [B * S]), both int64, the targets being the inputs
+    shifted left by one position (drawn as one [B, S + 1] sequence)."""
+
+    def __init__(self, batch: int, seq_len: int, vocab: int, device=None, seed: int = 0):
+        self.batch, self.seq_len, self.vocab = batch, seq_len, vocab
+        self.device = torch.device(device) if device is not None else torch.device("cpu")
+        self.gen = torch.Generator(device=self.device).manual_seed(seed)
+
+    def next(self) -> Tuple[torch.Tensor, torch.Tensor]:
+        t = torch.randint(0, self.vocab, (self.batch, self.seq_len + 1), generator=self.gen,
+                          device=self.device, dtype=torch.int64)
+        return t[:, :-1], t[:, 1:].reshape(-1)
 
 
 class DeviceBatchLoader:

@@ -1,0 +1,66 @@
+"""Decoder-only transformer language model, GPT-2 small by default: 124 475 904 parameters in 148 tensors
+(vocabulary 50 257 padded to 50 304, a multiple of 128, so the LM-head GEMM tiles evenly).
+
+Token + learned position embedding, ``depth`` pre-LN blocks (``vit.EncoderBlock`` with ``causal=True``, so
+attention runs on the causal flash-attention kernel, and LayerNorm eps 1e-5), a final LayerNorm, and an LM
+head tied to the token embedding (``F2.linear(x, wte.weight)``, no bias).  Initialisation follows GPT-2:
+N(0, 0.02) everywhere, with the residual projections (``proj``, ``fc2``) at 0.02 / sqrt(2 * depth).
+
+The MLP is the fused node's exact (erf) GELU, not GPT-2's tanh approximation, so weights trained by the
+original GPT-2 code would see a slightly different activation here.
+"""
+from __future__ import annotations
+
+import math
+
+from torch import nn
+
+from ..ops import functional as F2
+from ..ops import grad_sink
+from .vit import EncoderBlock
+
+
+class GPT(nn.Module):
+    def __init__(self, vocab: int = 50304, context: int = 1024, depth: int = 12, heads: int = 12,
+                 dim: int = 768, mlp_dim: int = 3072):
+        super().__init__()
+        self.vocab, self.context, self.dim = vocab, context, dim
+        self.wte = nn.Embedding(vocab, dim)
+        self.wpe = nn.Embedding(context, dim)
+        self.layers = nn.ModuleList([EncoderBlock(dim, heads, mlp_dim, causal=True, eps=1e-5)
+                                     for _ in range(depth)])
+        self.ln_f = nn.LayerNorm(dim, eps=1e-5)
+        for m in self.modules():
+            if isinstance(m, (nn.Linear, nn.Embedding)):
+                nn.init.normal_(m.weight, mean=0.0, std=0.02)
+            if isinstance(m, nn.Linear):
+                nn.init.zeros_(m.bias)
+        for blk in self.layers:
+            for lin in (blk.proj, blk.fc2):
+                nn.init.normal_(lin.weight, mean=0.0, std=0.02 / math.sqrt(2 * depth))
+
+    def forward(self, idx):
+        """``idx``: [B, S] int64 token ids, S <= context.  Returns logits [B * S, vocab] (rows in (b, s)
+        order, ready for ``nn.CrossEntropyLoss`` against targets of shape [B * S])."""
+        B, S = idx.shape
+        if S > self.context:
+            raise ValueError(f"sequence length {S} exceeds the model's context of {self.context}")
+        # the token embedding is also the LM head: two uses, so its gradient is summed by autograd
+        # rather than written straight into the gradient bucket by the LM head's GEMM
+        grad_sink.note_forward(self.wte.weight)
+        x = self.wte(idx) + self.wpe.weight[:S]
+        for blk in self.layers:
+            x = blk(x)
+        x = F2.layer_norm(x, self.ln_f.weight, self.ln_f.bias, self.ln_f.eps)
+        return F2.linear(x.reshape(B * S, self.dim), self.wte.weight)
+
+
+def gpt2(**kw):
+    return GPT(**kw)
+
+
+def gpt_tiny(**kw):
+    """2 layers, 2 heads of 64 (the attention kernel's head dim), width 128, vocab 512, context 128."""
+    d = dict(vocab=512, context=128, depth=2, heads=2, dim=128, mlp_dim=512)
+    d.update(kw)
+    return GPT(**d)

@@ -16,20 +16,23 @@ from ..ops import functional as F2
 
 
 class EncoderBlock(nn.Module):
-    def __init__(self, dim: int, heads: int, mlp_dim: int):
+    """Pre-LN transformer block.  ``causal=True`` makes it a decoder block (``models.gpt``)."""
+
+    def __init__(self, dim: int, heads: int, mlp_dim: int, causal: bool = False, eps: float = 1e-6):
         super().__init__()
         self.heads = heads
-        self.ln_1 = nn.LayerNorm(dim, eps=1e-6)
+        self.causal = causal
+        self.ln_1 = nn.LayerNorm(dim, eps=eps)
         self.qkv = nn.Linear(dim, 3 * dim)
         self.proj = nn.Linear(dim, dim)
-        self.ln_2 = nn.LayerNorm(dim, eps=1e-6)
+        self.ln_2 = nn.LayerNorm(dim, eps=eps)
         self.fc1 = nn.Linear(dim, mlp_dim)
         self.fc2 = nn.Linear(mlp_dim, dim)
 
     def forward(self, x):
         B, S, D = x.shape
         h = F2.layer_norm(x, self.ln_1.weight, self.ln_1.bias, self.ln_1.eps)
-        a = F2.qkv_attention(h, self.qkv.weight, self.qkv.bias, self.heads)   # [B,S,D]
+        a = F2.qkv_attention(h, self.qkv.weight, self.qkv.bias, self.heads, self.causal)   # [B,S,D]
         x = F2.linear(a, self.proj.weight, self.proj.bias, residual=x)
         h = F2.layer_norm(x, self.ln_2.weight, self.ln_2.bias, self.ln_2.eps)
         return F2.mlp(h, self.fc1.weight, self.fc1.bias, self.fc2.weight, self.fc2.bias, residual=x)

@@ -1,5 +1,5 @@
 """Flash attention binding (csrc/attn_sm90.cu): wgmma forward + backward, bf16, head dim 64,
-non-causal (the ViT-B/16 configuration).  ``attention_fused(q, k, v)`` takes ``[B, H, S, 64]``
+non-causal (ViT-B/16) or causal (GPT).  ``attention_fused(q, k, v, causal=False)`` takes ``[B, H, S, 64]``
 tensors with ANY batch/head/sequence strides (64 contiguous) — in the model they are the three dense
 ``[B*S, D]`` projection outputs viewed as ``[B, S, H, 64]`` and transposed, so no un-pack / re-pack
 copy exists in either direction: the output and all three gradients are produced in ``[B, S, H, 64]``
@@ -25,7 +25,8 @@ def register(lib, have):
     vp, i, f, u64 = ctypes.c_void_p, ctypes.c_int, ctypes.c_float, ctypes.c_uint64
     lp = ctypes.POINTER(ctypes.c_longlong)
     lib.b200dp_attn_fwd.argtypes = [vp, vp, vp, vp, vp, i, i, i, i, lp, lp, lp, lp, f, u64]
-    lib.b200dp_attn_bwd.argtypes = [vp] * 10 + [i, i, i, i] + [lp] * 8 + [f, u64]
+    lib.b200dp_attn_fwd_ex.argtypes = [vp, vp, vp, vp, vp, i, i, i, i, lp, lp, lp, lp, f, i, u64]
+    lib.b200dp_attn_bwd.argtypes = [vp] * 10 + [i, i, i, i] + [lp] * 8 + [f, i, u64]
     lib.b200dp_attn_last_error.restype = ctypes.c_char_p
     if hasattr(lib, "b200dp_cast_acc_zero"):
         lib.b200dp_cast_acc_zero.argtypes = [vp, vp, ctypes.c_longlong, i, i, i, u64]
@@ -69,7 +70,7 @@ def _dq_workspace(B, S, H, dev):
 
 class _AttnFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, q, k, v):
+    def forward(ctx, q, k, v, causal):
         q, k, v = _fix(q), _fix(k), _fix(v)
         B, H, S, D = q.shape
         dev = q.device
@@ -77,13 +78,14 @@ class _AttnFn(torch.autograd.Function):
         need = any(ctx.needs_input_grad)
         lse = torch.empty((B, H, S), dtype=torch.float32, device=dev) if need else None
         scale = 1.0 / math.sqrt(D)
-        _ck(_lib.b200dp_attn_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(),
-                                 lse.data_ptr() if lse is not None else None, B, H, S, D,
-                                 _strides(q), _strides(k), _strides(v), _strides(o), scale,
-                                 torch.cuda.current_stream(dev).cuda_stream))
+        _ck(_lib.b200dp_attn_fwd_ex(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(),
+                                    lse.data_ptr() if lse is not None else None, B, H, S, D,
+                                    _strides(q), _strides(k), _strides(v), _strides(o), scale, int(causal),
+                                    torch.cuda.current_stream(dev).cuda_stream))
         counters.bump("attn_fwd")
         if need:
             ctx.save_for_backward(q, k, v, o, lse)
+            ctx.causal = causal
         return o
 
     @staticmethod
@@ -101,15 +103,20 @@ class _AttnFn(torch.autograd.Function):
         _ck(_lib.b200dp_attn_bwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), do.data_ptr(),
                                  lse.data_ptr(), delta.data_ptr(), acc.data_ptr(), dk.data_ptr(), dv.data_ptr(),
                                  B, H, S, D, _strides(q), _strides(k), _strides(v), _strides(o), _strides(do),
-                                 _strides(acc_v), _strides(dk), _strides(dv), 1.0 / math.sqrt(D), st))
+                                 _strides(acc_v), _strides(dk), _strides(dv), 1.0 / math.sqrt(D),
+                                 int(ctx.causal), st))
         rc = _lib.b200dp_cast_acc_zero(acc.data_ptr(), dq.data_ptr(), acc.numel(), 1, 0, 1, st)
         if rc != 0:
             raise RuntimeError("cast_acc_zero failed")
         counters.bump("attn_bwd", 3)
-        return dq, dk, dv
+        return dq, dk, dv, None
 
 
-def attention_fused(q, k, v):
+def attention_fused(q, k, v, causal=False):
     """softmax(q k^T / sqrt(64)) v for [B, H, S, 64] bf16 tensors; returns [B, H, S, 64] (memory order
-    [B, S, H, 64])."""
-    return _AttnFn.apply(q, k, v)
+    [B, S, H, 64]).  ``causal=True`` masks key j out of query i's softmax wherever j > i (a decoder's
+    self-attention); q, k and v must then have the same sequence length."""
+    if causal and not (q.shape[2] == k.shape[2] == v.shape[2]):
+        raise ValueError(f"causal attention needs one sequence length for q, k and v; got "
+                         f"{q.shape[2]}, {k.shape[2]}, {v.shape[2]}")
+    return _AttnFn.apply(q, k, v, bool(causal))

@@ -111,24 +111,27 @@ def layer_norm(x, weight, bias, eps: float = 1e-6):
 
 
 # ------------------------------------------------------------------ attention
-def attention_reference(qkv, heads: int):
+def attention_reference(qkv, heads: int, causal: bool = False):
+    """Self-attention of a packed ``[B, S, 3 D]`` q|k|v tensor; ``causal=True``: position i attends to
+    positions 0..i only."""
     B, S, D3 = qkv.shape
     D = D3 // 3
     hd = D // heads
     q, k, v = qkv.view(B, S, 3, heads, hd).permute(2, 0, 3, 1, 4)
-    o = F.scaled_dot_product_attention(q, k, v)
+    o = F.scaled_dot_product_attention(q, k, v, is_causal=causal)
     return o.transpose(1, 2).reshape(B, S, D)
 
 
-def attention(qkv, heads: int):
+def attention(qkv, heads: int, causal: bool = False):
     k = _kernels(qkv)
     if k is not None and k.has("attention"):
-        return k.attention(qkv, heads)
-    return attention_reference(qkv, heads)
+        return k.attention(qkv, heads, causal)
+    return attention_reference(qkv, heads, causal)
 
 
-def qkv_attention(x, weight, bias, heads: int):
-    """Multi-head self-attention input stage: packed QKV projection + scaled-dot-product attention.
+def qkv_attention(x, weight, bias, heads: int, causal: bool = False):
+    """Multi-head self-attention input stage: packed QKV projection + scaled-dot-product attention
+    (``causal=True``: position i attends to positions 0..i only, as in a decoder).
     Kernel path: q, k, v are produced as three dense matrices (no un-pack / re-pack copies)."""
     k = _kernels(x)
     if k is not None and k.has("linear") and k.linear_supported(x, weight) and weight.shape[0] % 24 == 0 \
@@ -140,11 +143,11 @@ def qkv_attention(x, weight, bias, heads: int):
         if k.has("attention_fused") and hd == 64 and os.environ.get("B200DP_ATTN_KERNEL", "1") == "1":
             from . import attention as _attn
             if _attn.supported(q, kk, v):
-                o = _attn.attention_fused(q, kk, v)       # [B,H,S,hd] view of [B,S,H,hd] memory
+                o = _attn.attention_fused(q, kk, v, causal)   # [B,H,S,hd] view of [B,S,H,hd] memory
                 return o.transpose(1, 2).reshape(B, S, D)  # a view: no copy
-        o = F.scaled_dot_product_attention(q, kk, v)
+        o = F.scaled_dot_product_attention(q, kk, v, is_causal=causal)
         return o.transpose(1, 2).reshape(B, S, D)
-    return attention(linear(x, weight, bias), heads)
+    return attention(linear(x, weight, bias), heads, causal)
 
 
 # ------------------------------------------------------------------ ViT patch embedding

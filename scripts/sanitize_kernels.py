@@ -3,7 +3,7 @@
 Shapes are small (the tools slow kernels 10-100x) but cover: multi-tile persistent loops (several tiles per
 CTA are not reachable at these sizes on 132 SMs, so max_ctas is forced down where the API allows), the
 statistics / residual / masked-residual / split-K epilogues (per-CTA statistics slots, last-arriver split-K
-reduction, fp32 and bf16 add / store outputs), 3x3 / strided / 1x1 conv paths incl. split-K wgrad, BN, LN, pooling, attention and the LSTM
+reduction, fp32 and bf16 add / store outputs), 3x3 / strided / 1x1 conv paths incl. split-K wgrad, BN, LN, pooling, attention (non-causal and causal) and the LSTM
 recurrence, plus the fused engine's clip-by-global-norm kernels (reduce into R with norm slots, finalize, update) and its
 LARS / LAMB kernels (reduce + direction + chunk partials, trust ratios + update)."""
 import os, sys, torch
@@ -53,6 +53,10 @@ t = rnd(64, 256).requires_grad_(True)
 F2.layer_norm(t, ln.weight, ln.bias).float().sum().backward()
 q, k_, v = (rnd(2, 4, 197, 64, scale=0.5).requires_grad_(True) for _ in range(3))
 kernels.attention_fused(q, k_, v).float().sum().backward()
+# causal: the diagonal tile's mask, the shortened KV / query-tile loops and the reversed tile order
+for S in (197, 300):
+    q, k_, v = (rnd(2, 3, S, 64, scale=0.5).requires_grad_(True) for _ in range(3))
+    kernels.attention_fused(q, k_, v, causal=True).float().sum().backward()
 from distributed_torch_horovod_gcp_b200.models import LSTM
 m = LSTM(23, 20, 1, 256, device=torch.device(dev)).to(dev)
 xs = torch.randn(8, 20, 23, device=dev)
