@@ -4,7 +4,8 @@
 
 Produces ``distributed_torch_horovod_gcp_b200/lib/*.so`` for sm_90a (H100):
   libb200dp_comm.so     csrc/runtime.cpp + csrc/comm_kernels.cu
-  libb200dp_kernels.so  csrc/gemm_sm90.cu, conv_sm90.cu, elementwise.cu, lstm_kernels.cu, lstm_rec_sm90.cu ...
+  libb200dp_kernels.so  csrc/gemm_sm90.cu, conv_sm90.cu, elementwise.cu, lstm_kernels.cu, lstm_rec_sm90.cu,
+                        attn_sm90.cu, xent_sm90.cu
 nvcc cross-compiles without a GPU, so this also runs on the CPU dev box.
 """
 from __future__ import annotations
@@ -29,7 +30,7 @@ NVCC_FLAGS = [
 TARGETS = {
     "libb200dp_comm.so": ["runtime.cpp", "comm_kernels.cu"],
     "libb200dp_kernels.so": ["gemm_sm90.cu", "conv_sm90.cu", "elementwise.cu", "lstm_kernels.cu",
-                             "lstm_rec_sm90.cu", "attn_sm90.cu"],
+                             "lstm_rec_sm90.cu", "attn_sm90.cu", "xent_sm90.cu"],
 }
 
 

@@ -39,9 +39,11 @@ class GPT(nn.Module):
             for lin in (blk.proj, blk.fc2):
                 nn.init.normal_(lin.weight, mean=0.0, std=0.02 / math.sqrt(2 * depth))
 
-    def forward(self, idx):
-        """``idx``: [B, S] int64 token ids, S <= context.  Returns logits [B * S, vocab] (rows in (b, s)
-        order, ready for ``nn.CrossEntropyLoss`` against targets of shape [B * S])."""
+    def forward(self, idx, targets=None):
+        """``idx``: [B, S] int64 token ids, S <= context.  Without ``targets``: the logits [B * S, vocab] (rows
+        in (b, s) order, ready for ``nn.CrossEntropyLoss`` against targets of shape [B * S]).  With ``targets``
+        ([B, S] or [B * S]): the mean cross-entropy loss, through ``linear_cross_entropy`` on the LM head, which
+        never materialises the logits on the kernel path."""
         B, S = idx.shape
         if S > self.context:
             raise ValueError(f"sequence length {S} exceeds the model's context of {self.context}")
@@ -52,6 +54,8 @@ class GPT(nn.Module):
         for blk in self.layers:
             x = blk(x)
         x = F2.layer_norm(x, self.ln_f.weight, self.ln_f.bias, self.ln_f.eps)
+        if targets is not None:
+            return F2.linear_cross_entropy(x.reshape(B * S, self.dim), self.wte.weight, targets.reshape(-1))
         return F2.linear(x.reshape(B * S, self.dim), self.wte.weight)
 
 

@@ -11,7 +11,9 @@ from . import ln as _ln
 from . import conv as _conv
 from . import lstm_rec as _lstm_rec
 from . import attention as _attn
+from . import xent as _xent
 from .attention import attention_fused  # noqa: F401
+from .xent import linear_cross_entropy  # noqa: F401
 from .lstm_rec import lstm_recurrent  # noqa: F401
 from .conv import conv3x3, conv2d as conv2d_implicit  # noqa: F401
 from .ln import layer_norm  # noqa: F401
@@ -27,6 +29,7 @@ def register(lib, have: Dict[str, bool]) -> None:
     _conv.register(lib, have)
     _lstm_rec.register(lib, have)
     _attn.register(lib, have)
+    _xent.register(lib, have)
 
 
 def linear_supported(x, weight) -> bool:
@@ -35,3 +38,7 @@ def linear_supported(x, weight) -> bool:
 
 def layer_norm_supported(x, weight, bias) -> bool:
     return _ln.supported(x, weight, bias)
+
+
+def linear_cross_entropy_supported(x, weight, targets) -> bool:
+    return _xent.supported(x, weight, targets)

@@ -4,7 +4,8 @@ Each function is ONE fusable unit.  ``*_reference`` are plain PyTorch compositio
 path and the fp32 numerics oracle for the kernels' tests; the CUDA fast paths are the
 hand-written sm_90a kernels bound in ``ops.kernels``: wgmma GEMM with fused epilogues
 (ops/gemm.py), implicit-GEMM convolution (ops/conv.py), fused BN/ReLU/residual and max-pool
-(ops/bn.py), LayerNorm (ops/ln.py), flash attention forward/backward (ops/attention.py).
+(ops/bn.py), LayerNorm (ops/ln.py), flash attention forward/backward (ops/attention.py), the LM head
+fused with its cross-entropy loss (ops/xent.py).
 """
 from __future__ import annotations
 
@@ -148,6 +149,35 @@ def qkv_attention(x, weight, bias, heads: int, causal: bool = False):
         o = F.scaled_dot_product_attention(q, kk, v, is_causal=causal)
         return o.transpose(1, 2).reshape(B, S, D)
     return attention(linear(x, weight, bias), heads, causal)
+
+
+# ------------------------------------------------------------------ LM head + cross-entropy
+def linear_cross_entropy_reference(x, weight, targets, ignore_index: int = -100, reduction: str = "mean"):
+    logits = F.linear(x, weight).float()
+    return F.cross_entropy(logits.reshape(-1, logits.shape[-1]), targets.reshape(-1), ignore_index=ignore_index,
+                           reduction=reduction)
+
+
+def linear_cross_entropy(x, weight, targets, ignore_index: int = -100, reduction: str = "mean"):
+    """``F.cross_entropy(F.linear(x, weight).float(), targets.reshape(-1), ignore_index, reduction)`` for
+    ``x`` [..., D], ``weight`` [V, D] and int64 ``targets`` with ``x.shape[:-1]`` elements; ``"none"`` returns
+    fp32 [N], ``"sum"`` / ``"mean"`` an fp32 scalar.
+
+    Kernel path (bf16 ``x`` and ``weight`` on an sm_90 device, D % 8 == 0, V % 8 == 0, 16-byte-aligned
+    rows): the [N, V] logits are never stored (ops/xent.py); the backward holds one bf16 chunk of at most
+    256 MiB of them.  There, a target outside [0, V) that is not ``ignore_index`` gives its row a NaN loss
+    and a NaN gradient row instead of torch's device assert.  Anything else takes the composition above."""
+    if reduction not in ("none", "sum", "mean"):
+        raise ValueError(f"reduction must be 'none', 'sum' or 'mean'; got {reduction!r}")
+    if weight.dim() != 2 or x.dim() < 1 or x.shape[-1] != weight.shape[1]:
+        raise ValueError(f"x [..., D] and weight [V, D] do not match: {tuple(x.shape)} and {tuple(weight.shape)}")
+    n_rows = x.numel() // x.shape[-1] if x.shape[-1] else 0
+    if targets.numel() != n_rows:
+        raise ValueError(f"targets has {targets.numel()} elements; x has {n_rows} rows")
+    k = _kernels(x)
+    if k is not None and k.has("linear_cross_entropy") and k.linear_cross_entropy_supported(x, weight, targets):
+        return k.linear_cross_entropy(x, weight, targets, ignore_index, reduction)
+    return linear_cross_entropy_reference(x, weight, targets, ignore_index, reduction)
 
 
 # ------------------------------------------------------------------ ViT patch embedding

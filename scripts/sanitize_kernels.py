@@ -3,7 +3,7 @@
 Shapes are small (the tools slow kernels 10-100x) but cover: multi-tile persistent loops (several tiles per
 CTA are not reachable at these sizes on 132 SMs, so max_ctas is forced down where the API allows), the
 statistics / residual / masked-residual / split-K epilogues (per-CTA statistics slots, last-arriver split-K
-reduction, fp32 and bf16 add / store outputs), 3x3 / strided / 1x1 conv paths incl. split-K wgrad, BN, LN, pooling, attention (non-causal and causal) and the LSTM
+reduction, fp32 and bf16 add / store outputs), 3x3 / strided / 1x1 conv paths incl. split-K wgrad, BN, LN, pooling, attention (non-causal and causal), the fused LM-head cross-entropy and the LSTM
 recurrence, plus the fused engine's clip-by-global-norm kernels (reduce into R with norm slots, finalize, update) and its
 LARS / LAMB kernels (reduce + direction + chunk partials, trust ratios + update)."""
 import os, sys, torch
@@ -57,6 +57,16 @@ kernels.attention_fused(q, k_, v).float().sum().backward()
 for S in (197, 300):
     q, k_, v = (rnd(2, 3, S, 64, scale=0.5).requires_grad_(True) for _ in range(3))
     kernels.attention_fused(q, k_, v, causal=True).float().sum().backward()
+# fused LM-head cross-entropy: N and V not multiples of 128, an ignored row, 3 CTAs over several vocab ranges each,
+# and 128-row backward chunks (the last one partial) with fp32 dW accumulation
+from distributed_torch_horovod_gcp_b200.ops import xent as XE
+XE._CHUNK_BYTES = 2 * 128 * 1000
+xx, ww = rnd(300, 64).requires_grad_(True), rnd(1000, 64, scale=0.2).requires_grad_(True)
+tt = torch.randint(0, 1000, (300,), device=dev)
+tt[5] = -100
+XE.linear_cross_entropy(xx, ww, tt, max_ctas=3).backward()
+XE.linear_cross_entropy(xx, ww, tt, reduction="none", max_ctas=3).sum().backward()
+print("xent ok", float(xx.grad.float().abs().sum()))
 from distributed_torch_horovod_gcp_b200.models import LSTM
 m = LSTM(23, 20, 1, 256, device=torch.device(dev)).to(dev)
 xs = torch.randn(8, 20, 23, device=dev)
