@@ -324,15 +324,22 @@ struct StepInfo {
   float lr;
 };
 
+// Adam / LAMB bias corrections 1 - beta1^t and sqrt(1 - beta2^t) for step t (1-based), each rounded to fp32 once.
+// They are formed in double: in fp32, 1 - beta^t cancels for beta near 1 and small t and magnifies the rounding of
+// beta^t by beta^t / (1 - beta^t) (about 10^5 for beta2 = 0.99999), far beyond the rest of the update's error.
+__device__ __forceinline__ void bias_corrections(float beta1, float beta2, int t, float* bc1, float* bc2_sqrt) {
+  const double tf = (double)t;
+  *bc1 = (float)(1.0 - pow((double)beta1, tf));
+  *bc2_sqrt = (float)sqrt(1.0 - pow((double)beta2, tf));
+}
+
 __device__ __forceinline__ StepInfo make_step(const ARArgs& a) {
   StepInfo s;
   const int t = a.step_ctr ? *a.step_ctr : 0;
   s.first = (t == 0);
   s.lr = a.h.lr * (a.lr_scale ? *a.lr_scale : 1.0f);
   if (a.h.kind == OPT_ADAM) {
-    const float tf = (float)(t + 1);
-    s.bc1 = 1.0f - powf(a.h.beta1, tf);
-    s.bc2_sqrt = sqrtf(1.0f - powf(a.h.beta2, tf));
+    bias_corrections(a.h.beta1, a.h.beta2, t + 1, &s.bc1, &s.bc2_sqrt);
   } else {
     s.bc1 = 1.0f;
     s.bc2_sqrt = 1.0f;
@@ -648,11 +655,7 @@ __global__ void __launch_bounds__(512) allreduce_oneshot_lw_kernel(CommCtx c, AR
   const T* out_local = reinterpret_cast<const T*>(a.out[c.rank]);
   const bool lamb = a.h.kind == OPT_LAMB;
   float bc1 = 1.0f, bc2_sqrt = 1.0f;
-  if (lamb) {
-    const float tf = (float)((a.step_ctr ? *a.step_ctr : 0) + 1);
-    bc1 = 1.0f - powf(a.h.beta1, tf);
-    bc2_sqrt = sqrtf(1.0f - powf(a.h.beta2, tf));
-  }
+  if (lamb) bias_corrections(a.h.beta1, a.h.beta2, (a.step_ctr ? *a.step_ctr : 0) + 1, &bc1, &bc2_sqrt);
 
   if (!rank_barrier(c, a.channel)) return;
   for (int ch = blockIdx.x; ch < k.nchunks; ch += gridDim.x) {
