@@ -313,6 +313,50 @@ struct Vec<__half> {
   __device__ static uint4 mc_reduce(const void* p) { return mc_ld_reduce_f16(p); }
 };
 
+// ------------------------------------------------------------------ shared kernel pieces
+// Zero-on-consume tail of the grid-stride one-shot kernels, run after the closing barrier: every peer has read
+// this thread's vectors of the local gradient bucket, so zero them, or, for an in-place one-shot, overwrite them
+// with the result kept in `restore`.
+__device__ __forceinline__ void release_input(const void* in, const uint4* restore, size_t start, size_t nvec,
+                                              size_t stride) {
+  uint4* mine = reinterpret_cast<uint4*>(const_cast<void*>(in));
+  for (size_t v = start; v < nvec; v += stride) mine[v] = restore ? restore[v] : make_uint4(0, 0, 0, 0);
+}
+
+// ------------------------------------------------------------------ fp32 arenas (master, S0, S1, R)
+template <int VN>
+__device__ __forceinline__ void load_f32(const float* src, float* x) {
+#pragma unroll
+  for (int i = 0; i < VN; i += 4) {
+    const float4 m = *reinterpret_cast<const float4*>(src + i);
+    x[i] = m.x; x[i + 1] = m.y; x[i + 2] = m.z; x[i + 3] = m.w;
+  }
+}
+
+template <int VN>
+__device__ __forceinline__ void store_f32(float* dst, const float* x) {
+#pragma unroll
+  for (int i = 0; i < VN; i += 4)
+    *reinterpret_cast<float4*>(dst + i) = make_float4(x[i], x[i + 1], x[i + 2], x[i + 3]);
+}
+
+// fp32 master values of VN elements from element `idx`: the master arena, or the fp32 result bucket itself.
+// The master load is spelled out rather than taken from load_f32: through load_f32, nvcc 12.9 splits each
+// 128-bit master load of the sliced kernels (K2/K3) into four 32-bit loads.
+template <typename T, int VN>
+__device__ __forceinline__ void load_master(const ARArgs& a, const T* out_local, size_t idx, float* p) {
+  if (a.master) {
+#pragma unroll
+    for (int i = 0; i < VN; i += 4) {
+      const float4 m = *reinterpret_cast<const float4*>(a.master + idx + i);
+      p[i] = m.x; p[i + 1] = m.y; p[i + 2] = m.z; p[i + 3] = m.w;
+    }
+  } else {
+    const uint4 v = *reinterpret_cast<const uint4*>(out_local + idx);
+    Vec<T>::unpack(v, p);
+  }
+}
+
 // ------------------------------------------------------------------ K7: fused optimizer epilogue
 // `g[]` holds the reduced gradient of VN consecutive elements starting at element `idx`.
 // Returns the values to store in the result bucket (updated parameters, or the scaled
@@ -347,6 +391,14 @@ __device__ __forceinline__ StepInfo make_step(const ARArgs& a) {
   return s;
 }
 
+// Adam / LAMB update of the moments m and v of one element with gradient g (torch.optim semantics, non-amsgrad);
+// returns the denominator sqrt(v^) + eps.  The callers form the update from it differently.
+__device__ __forceinline__ float adam_moments(const OptHyper& h, float bc2_sqrt, float g, float& m, float& v) {
+  m = fmaf(h.beta1, m, (1.0f - h.beta1) * g);      // lerp(m, g, 1-b1)
+  v = fmaf(h.beta2, v, (1.0f - h.beta2) * g * g);
+  return sqrtf(v) / bc2_sqrt + h.eps;
+}
+
 template <typename T, int VN>
 __device__ __forceinline__ void epilogue(const ARArgs& a, const StepInfo& s, size_t idx, float* g,
                                          const T* out_local, float* o) {
@@ -358,16 +410,7 @@ __device__ __forceinline__ void epilogue(const ARArgs& a, const StepInfo& s, siz
     return;
   }
   float p[VN];
-  if (a.master) {
-#pragma unroll
-    for (int i = 0; i < VN; i += 4) {
-      const float4 m = *reinterpret_cast<const float4*>(a.master + idx + i);
-      p[i] = m.x; p[i + 1] = m.y; p[i + 2] = m.z; p[i + 3] = m.w;
-    }
-  } else {  // the result bucket is fp32 and is the master copy
-    const uint4 v = *reinterpret_cast<const uint4*>(out_local + idx);
-    Vec<T>::unpack(v, p);
-  }
+  load_master<T, VN>(a, out_local, idx, p);
   if (a.h.maximize) {
 #pragma unroll
     for (int i = 0; i < VN; ++i) g[i] = -g[i];
@@ -383,32 +426,21 @@ __device__ __forceinline__ void epilogue(const ARArgs& a, const StepInfo& s, siz
 #pragma unroll
         for (int i = 0; i < VN; ++i) b[i] = g[i];
       } else {
-#pragma unroll
-        for (int i = 0; i < VN; i += 4) {
-          const float4 m = *reinterpret_cast<const float4*>(a.s0 + idx + i);
-          b[i] = m.x; b[i + 1] = m.y; b[i + 2] = m.z; b[i + 3] = m.w;
-        }
+        load_f32<VN>(a.s0 + idx, b);
 #pragma unroll
         for (int i = 0; i < VN; ++i)
           b[i] = fmaf(a.h.momentum, b[i], (1.0f - a.h.dampening) * g[i]);
       }
-#pragma unroll
-      for (int i = 0; i < VN; i += 4)
-        *reinterpret_cast<float4*>(a.s0 + idx + i) = make_float4(b[i], b[i + 1], b[i + 2], b[i + 3]);
+      store_f32<VN>(a.s0 + idx, b);
 #pragma unroll
       for (int i = 0; i < VN; ++i) g[i] = a.h.nesterov ? fmaf(a.h.momentum, b[i], g[i]) : b[i];
     }
 #pragma unroll
     for (int i = 0; i < VN; ++i) p[i] = fmaf(-s.lr, g[i], p[i]);
-  } else {  // Adam / AdamW (torch.optim semantics, non-amsgrad)
+  } else {  // Adam / AdamW
     float m[VN], v[VN];
-#pragma unroll
-    for (int i = 0; i < VN; i += 4) {
-      const float4 a0 = *reinterpret_cast<const float4*>(a.s0 + idx + i);
-      const float4 a1 = *reinterpret_cast<const float4*>(a.s1 + idx + i);
-      m[i] = a0.x; m[i + 1] = a0.y; m[i + 2] = a0.z; m[i + 3] = a0.w;
-      v[i] = a1.x; v[i + 1] = a1.y; v[i + 2] = a1.z; v[i + 3] = a1.w;
-    }
+    load_f32<VN>(a.s0 + idx, m);
+    load_f32<VN>(a.s1 + idx, v);
 #pragma unroll
     for (int i = 0; i < VN; ++i) {
       if (a.h.adamw) {
@@ -416,22 +448,13 @@ __device__ __forceinline__ void epilogue(const ARArgs& a, const StepInfo& s, siz
       } else if (a.h.weight_decay != 0.0f) {
         g[i] = fmaf(a.h.weight_decay, p[i], g[i]);
       }
-      m[i] = fmaf(a.h.beta1, m[i], (1.0f - a.h.beta1) * g[i]);      // lerp(m, g, 1-b1)
-      v[i] = fmaf(a.h.beta2, v[i], (1.0f - a.h.beta2) * g[i] * g[i]);
-      const float denom = sqrtf(v[i]) / s.bc2_sqrt + a.h.eps;
+      const float denom = adam_moments(a.h, s.bc2_sqrt, g[i], m[i], v[i]);
       p[i] = fmaf(-(s.lr / s.bc1), m[i] / denom, p[i]);
     }
-#pragma unroll
-    for (int i = 0; i < VN; i += 4) {
-      *reinterpret_cast<float4*>(a.s0 + idx + i) = make_float4(m[i], m[i + 1], m[i + 2], m[i + 3]);
-      *reinterpret_cast<float4*>(a.s1 + idx + i) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
-    }
+    store_f32<VN>(a.s0 + idx, m);
+    store_f32<VN>(a.s1 + idx, v);
   }
-  if (a.master) {
-#pragma unroll
-    for (int i = 0; i < VN; i += 4)
-      *reinterpret_cast<float4*>(a.master + idx + i) = make_float4(p[i], p[i + 1], p[i + 2], p[i + 3]);
-  }
+  if (a.master) store_f32<VN>(a.master + idx, p);
 #pragma unroll
   for (int i = 0; i < VN; ++i) o[i] = p[i];
 }
@@ -483,31 +506,40 @@ __global__ void __launch_bounds__(512) allreduce_oneshot_kernel(CommCtx c, ARArg
     reinterpret_cast<uint4*>(out_local)[v] = Vec<T>::pack(o);
   }
   rank_barrier(c, a.channel);  // every peer has finished reading my gradients
-  if (a.copy_back | a.zero_input) {
-    uint4* mine = reinterpret_cast<uint4*>(const_cast<void*>(a.in[c.rank]));
-    for (size_t v = start; v < nvec; v += stride)
-      mine[v] = a.copy_back ? reinterpret_cast<const uint4*>(a.scratch)[v] : make_uint4(0, 0, 0, 0);
-  }
+  if (a.copy_back | a.zero_input)
+    release_input(a.in[c.rank], a.copy_back ? reinterpret_cast<const uint4*>(a.scratch) : nullptr, start, nvec,
+                  stride);
   finish_step(a);
 }
 
 // ------------------------------------------------------------------ K1c / K8 / K9: clip by global norm
-// Fixed-shape block sum of one fp32 value per thread (warp butterfly, then warp 0 over the warp partials):
-// the same inputs give the same bits on every rank and every run.
-__device__ __forceinline__ float block_sum_fixed(float v) {
-  __shared__ float s_part[32];
+// Fixed-shape block sum (warp butterfly, then warp 0 over the warp partials) of one value per thread: an fp32
+// value, or a pair of fp32 or fp64 values.  The same inputs give the same bits on every rank and every run.
+struct DoublePair {
+  double x, y;
+};
+__device__ __forceinline__ float shfl_xor_add(float v, int o) { return v + __shfl_xor_sync(0xffffffffu, v, o); }
+__device__ __forceinline__ float2 shfl_xor_add(float2 v, int o) {
+  return make_float2(shfl_xor_add(v.x, o), shfl_xor_add(v.y, o));
+}
+__device__ __forceinline__ DoublePair shfl_xor_add(DoublePair v, int o) {
+  return {v.x + __shfl_xor_sync(0xffffffffu, v.x, o), v.y + __shfl_xor_sync(0xffffffffu, v.y, o)};
+}
+
+template <typename V>
+__device__ __forceinline__ V block_sum_fixed(V v) {
+  __shared__ V s_part[32];
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  for (int o = 16; o > 0; o >>= 1) v = shfl_xor_add(v, o);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (lane == 0) s_part[warp] = v;
   __syncthreads();
-  float t = 0.0f;
   if (warp == 0) {
-    t = lane < (int)(blockDim.x >> 5) ? s_part[lane] : 0.0f;
+    v = lane < (int)(blockDim.x >> 5) ? s_part[lane] : V{};
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+    for (int o = 16; o > 0; o >>= 1) v = shfl_xor_add(v, o);
   }
-  return t;  // valid in thread 0
+  return v;  // valid in thread 0; s_part is free again after the next __syncthreads()
 }
 
 // K1c: K1's reduction (same fixed rank order, same `scale * sum`), but the result goes to the fp32 arena
@@ -544,17 +576,12 @@ __global__ void __launch_bounds__(512) allreduce_oneshot_clip_kernel(CommCtx c, 
       acc[i] *= a.scale;
       sq = fmaf(acc[i], acc[i], sq);
     }
-#pragma unroll
-    for (int i = 0; i < VN; i += 4)
-      *reinterpret_cast<float4*>(k.r + v * VN + i) = make_float4(acc[i], acc[i + 1], acc[i + 2], acc[i + 3]);
+    store_f32<VN>(k.r + v * VN, acc);
   }
   const float total = block_sum_fixed(sq);
   if (threadIdx.x == 0) k.slots[blockIdx.x] = total;  // a CTA without elements writes 0
   rank_barrier(c, a.channel);  // every peer has finished reading my gradients
-  if (a.zero_input) {
-    uint4* mine = reinterpret_cast<uint4*>(const_cast<void*>(a.in[c.rank]));
-    for (size_t v = start; v < nvec; v += stride) mine[v] = make_uint4(0, 0, 0, 0);
-  }
+  if (a.zero_input) release_input(a.in[c.rank], nullptr, start, nvec, stride);
 }
 
 // K8: one CTA.  Thread t adds slots t, t + blockDim, ... in double, then a fixed tree in shared memory
@@ -591,11 +618,7 @@ __global__ void __launch_bounds__(512) clip_apply_kernel(CommCtx c, ARArgs a, Cl
   T* out = reinterpret_cast<T*>(a.out[c.rank]);
   for (size_t v = start; v < nvec; v += stride) {
     float g[VN];
-#pragma unroll
-    for (int i = 0; i < VN; i += 4) {
-      const float4 x = *reinterpret_cast<const float4*>(k.r + v * VN + i);
-      g[i] = x.x; g[i + 1] = x.y; g[i + 2] = x.z; g[i + 3] = x.w;
-    }
+    load_f32<VN>(k.r + v * VN, g);
 #pragma unroll
     for (int i = 0; i < VN; ++i) g[i] *= coef;
     float o[VN];
@@ -606,44 +629,6 @@ __global__ void __launch_bounds__(512) clip_apply_kernel(CommCtx c, ARArgs a, Cl
 }
 
 // ------------------------------------------------------------------ K10 / K11: LARS / LAMB
-// fp32 master values of VN elements from element `idx`: the master arena, or the fp32 result bucket itself.
-template <typename T, int VN>
-__device__ __forceinline__ void load_master(const ARArgs& a, const T* out_local, size_t idx, float* p) {
-  if (a.master) {
-#pragma unroll
-    for (int i = 0; i < VN; i += 4) {
-      const float4 m = *reinterpret_cast<const float4*>(a.master + idx + i);
-      p[i] = m.x; p[i + 1] = m.y; p[i + 2] = m.z; p[i + 3] = m.w;
-    }
-  } else {
-    Vec<T>::unpack(*reinterpret_cast<const uint4*>(out_local + idx), p);
-  }
-}
-
-// block_sum_fixed for two values at once; the trailing barrier lets the caller run it again at once.
-__device__ __forceinline__ float2 block_sum2_fixed(float x, float y) {
-  __shared__ float2 s_part2[32];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    x += __shfl_xor_sync(0xffffffffu, x, o);
-    y += __shfl_xor_sync(0xffffffffu, y, o);
-  }
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (lane == 0) s_part2[warp] = make_float2(x, y);
-  __syncthreads();
-  float2 t = make_float2(0.0f, 0.0f);
-  if (warp == 0) {
-    if (lane < (int)(blockDim.x >> 5)) t = s_part2[lane];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      t.x += __shfl_xor_sync(0xffffffffu, t.x, o);
-      t.y += __shfl_xor_sync(0xffffffffu, t.y, o);
-    }
-  }
-  __syncthreads();
-  return t;  // valid in thread 0
-}
-
 // K10: K1's reduction (same fixed rank order, same `scale * sum`), then the update direction into `k.r`
 // (LAMB also updates exp_avg / exp_avg_sq in s0 / s1) and, per chunk, the fp32 sums of squares of the master
 // weights and of the direction.  CTAs walk whole chunks, so every partial covers one tensor only and is added
@@ -684,20 +669,16 @@ __global__ void __launch_bounds__(512) allreduce_oneshot_lw_kernel(CommCtx c, AR
       if (lamb) {
 #pragma unroll
         for (int i = 0; i < VN; i += 4) {
-          float4 m = *reinterpret_cast<const float4*>(a.s0 + idx + i);
-          float4 s = *reinterpret_cast<const float4*>(a.s1 + idx + i);
-          float* mp = &m.x;
-          float* sp = &s.x;
+          float m[4], s[4];
+          load_f32<4>(a.s0 + idx + i, m);
+          load_f32<4>(a.s1 + idx + i, s);
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
-            const float x = g[i + j];
-            mp[j] = fmaf(a.h.beta1, mp[j], (1.0f - a.h.beta1) * x);
-            sp[j] = fmaf(a.h.beta2, sp[j], (1.0f - a.h.beta2) * x * x);
-            const float denom = sqrtf(sp[j]) / bc2_sqrt + a.h.eps;
-            g[i + j] = fmaf(a.h.weight_decay, p[i + j], (mp[j] / bc1) / denom);
+            const float denom = adam_moments(a.h, bc2_sqrt, g[i + j], m[j], s[j]);
+            g[i + j] = fmaf(a.h.weight_decay, p[i + j], (m[j] / bc1) / denom);
           }
-          *reinterpret_cast<float4*>(a.s0 + idx + i) = m;
-          *reinterpret_cast<float4*>(a.s1 + idx + i) = s;
+          store_f32<4>(a.s0 + idx + i, m);
+          store_f32<4>(a.s1 + idx + i, s);
         }
       } else {
 #pragma unroll
@@ -708,11 +689,10 @@ __global__ void __launch_bounds__(512) allreduce_oneshot_lw_kernel(CommCtx c, AR
         ww = fmaf(p[i], p[i], ww);
         dd = fmaf(g[i], g[i], dd);
       }
-#pragma unroll
-      for (int i = 0; i < VN; i += 4)
-        *reinterpret_cast<float4*>(k.r + idx + i) = make_float4(g[i], g[i + 1], g[i + 2], g[i + 3]);
+      store_f32<VN>(k.r + idx, g);
     }
-    const float2 s = block_sum2_fixed(ww, dd);
+    const float2 s = block_sum_fixed(make_float2(ww, dd));
+    __syncthreads();  // the next chunk's sum reuses the block sum's shared memory
     if (threadIdx.x == 0) {
       k.part[2 * ch] = s.x;
       k.part[2 * ch + 1] = s.y;
@@ -736,37 +716,16 @@ __global__ void __launch_bounds__(512) allreduce_oneshot_lw_kernel(CommCtx c, AR
 // t + blockDim, ... in double, then a fixed shuffle / warp tree, so every CTA that needs the ratio computes the
 // same bits without waiting for another.  1 when the group is not adaptive or either norm is not > 0.
 __device__ float lw_trust(const LwArgs& k, int first, int count) {
-  __shared__ double s_w[32], s_d[32];
   __shared__ float s_ratio;
-  double w = 0.0, d = 0.0;
+  DoublePair wd = {0.0, 0.0};
   for (int i = threadIdx.x; i < count; i += blockDim.x) {
-    w += (double)k.part[2 * (first + i)];
-    d += (double)k.part[2 * (first + i) + 1];
+    wd.x += (double)k.part[2 * (first + i)];
+    wd.y += (double)k.part[2 * (first + i) + 1];
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    w += __shfl_xor_sync(0xffffffffu, w, o);
-    d += __shfl_xor_sync(0xffffffffu, d, o);
-  }
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (lane == 0) {
-    s_w[warp] = w;
-    s_d[warp] = d;
-  }
-  __syncthreads();
-  if (warp == 0) {
-    const bool live = lane < (int)(blockDim.x >> 5);
-    w = live ? s_w[lane] : 0.0;
-    d = live ? s_d[lane] : 0.0;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      w += __shfl_xor_sync(0xffffffffu, w, o);
-      d += __shfl_xor_sync(0xffffffffu, d, o);
-    }
-    if (lane == 0) {
-      const double wn = sqrt(w), dn = sqrt(d);
-      s_ratio = (k.adaptive && wn > 0.0 && dn > 0.0) ? (float)((double)k.trust_coef * wn / dn) : 1.0f;
-    }
+  wd = block_sum_fixed(wd);
+  if (threadIdx.x == 0) {
+    const double wn = sqrt(wd.x), dn = sqrt(wd.y);
+    s_ratio = (k.adaptive && wn > 0.0 && dn > 0.0) ? (float)((double)k.trust_coef * wn / dn) : 1.0f;
   }
   __syncthreads();
   return s_ratio;
@@ -794,33 +753,22 @@ __global__ void __launch_bounds__(512) lw_apply_kernel(CommCtx c, ARArgs a, LwAr
     for (int v = q.first_vec + (int)threadIdx.x; v < q.first_vec + q.nvec; v += blockDim.x) {
       const size_t idx = (size_t)v * VN;
       float d[VN], p[VN];
-#pragma unroll
-      for (int i = 0; i < VN; i += 4) {
-        const float4 x = *reinterpret_cast<const float4*>(k.r + idx + i);
-        d[i] = x.x; d[i + 1] = x.y; d[i + 2] = x.z; d[i + 3] = x.w;
-      }
+      load_f32<VN>(k.r + idx, d);
       load_master<T, VN>(a, out, idx, p);
       if (lamb) {
 #pragma unroll
         for (int i = 0; i < VN; ++i) p[i] = fmaf(-step, d[i], p[i]);
       } else {
+        float b[VN];
+        load_f32<VN>(a.s0 + idx, b);
 #pragma unroll
-        for (int i = 0; i < VN; i += 4) {
-          float4 b = *reinterpret_cast<const float4*>(a.s0 + idx + i);
-          float* bp = &b.x;
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            bp[j] = fmaf(a.h.momentum, bp[j], step * d[i + j]);
-            p[i + j] -= bp[j];
-          }
-          *reinterpret_cast<float4*>(a.s0 + idx + i) = b;
+        for (int i = 0; i < VN; ++i) {
+          b[i] = fmaf(a.h.momentum, b[i], step * d[i]);
+          p[i] -= b[i];
         }
+        store_f32<VN>(a.s0 + idx, b);
       }
-      if (a.master) {
-#pragma unroll
-        for (int i = 0; i < VN; i += 4)
-          *reinterpret_cast<float4*>(a.master + idx + i) = make_float4(p[i], p[i + 1], p[i + 2], p[i + 3]);
-      }
+      if (a.master) store_f32<VN>(a.master + idx, p);
       reinterpret_cast<uint4*>(out)[v] = Vec<T>::pack(p);
     }
   }
@@ -1027,34 +975,21 @@ __global__ void __launch_bounds__(512) broadcast_kernel(CommCtx c, BcastArgs a) 
   rank_barrier(c, a.channel);  // root's stores are visible to every rank
 }
 
-// ------------------------------------------------------------------ local helpers
+// ------------------------------------------------------------------ host launch helpers
 template <typename T>
-cudaError_t launch_ar(const CommCtx& c, const ARArgs& a, int algo, int blocks, int threads,
-                      cudaStream_t st) {
-  if (algo == 0) {
-    allreduce_oneshot_kernel<T><<<blocks, threads, 0, st>>>(c, a);
-  } else if (algo == 1) {
-    allreduce_sliced_kernel<T, false><<<blocks, threads, 0, st>>>(c, a);
-  } else {
-    allreduce_sliced_kernel<T, true><<<blocks, threads, 0, st>>>(c, a);
+struct TypeTag {
+  using type = T;
+};
+
+// Calls f(TypeTag<T>{}) with the element type of a dtype code (0 fp32, 1 bf16, 2 fp16).
+template <typename F>
+cudaError_t with_dtype(int dtype, F&& f) {
+  switch (dtype) {
+    case 0: return f(TypeTag<float>{});
+    case 1: return f(TypeTag<__nv_bfloat16>{});
+    case 2: return f(TypeTag<__half>{});
   }
-  return cudaGetLastError();
-}
-
-template <typename T>
-cudaError_t launch_clip(const CommCtx& c, const ARArgs& a, const ClipArgs& k, bool apply, int blocks,
-                        int threads, cudaStream_t st) {
-  if (apply) clip_apply_kernel<T><<<blocks, threads, 0, st>>>(c, a, k);
-  else allreduce_oneshot_clip_kernel<T><<<blocks, threads, 0, st>>>(c, a, k);
-  return cudaGetLastError();
-}
-
-template <typename T>
-cudaError_t launch_lw(const CommCtx& c, const ARArgs& a, const LwArgs& k, bool apply, int blocks, int threads,
-                      cudaStream_t st) {
-  if (apply) lw_apply_kernel<T><<<blocks, threads, 0, st>>>(c, a, k);
-  else allreduce_oneshot_lw_kernel<T><<<blocks, threads, 0, st>>>(c, a, k);
-  return cudaGetLastError();
+  return cudaErrorInvalidValue;
 }
 
 }  // namespace
@@ -1075,40 +1010,47 @@ int b200dp_comm_limits(int* max_ranks, int* max_blocks, int* channels, int* ctx_
   return 0;
 }
 
+// The launch checks of every entry point.  The grid must fit the per-block barrier counters and slots
+// (1..B200DP_MAX_BLOCKS CTAs) and be whole warps of at most 512 threads (the block sums and __launch_bounds__);
+// the world and the channel must fit the signal pad; `sel` (algorithm, phase or collective mode) must be below
+// `nsel` and the dtype code known.  Sets the error message and returns false otherwise.
+static bool launch_ok(const char* what, const CommCtx* ctx, int channel, const char* sel_name, int sel, int nsel,
+                      int dtype, int blocks, int threads) {
+  if (blocks >= 1 && blocks <= B200DP_MAX_BLOCKS && threads >= 32 && threads <= 512 && (threads & 31) == 0 &&
+      ctx->world <= B200DP_MAX_RANKS && channel >= 0 && channel < B200DP_NUM_CHANNELS && sel >= 0 && sel < nsel &&
+      dtype >= 0 && dtype <= 2)
+    return true;
+  snprintf(g_comm_err, sizeof(g_comm_err), "bad %s launch: blocks=%d threads=%d world=%d channel=%d %s=%d dtype=%d",
+           what, blocks, threads, ctx->world, channel, sel_name, sel, dtype);
+  return false;
+}
+
+// 0, or -1 with the launch error in b200dp_comm_last_error().
+static int launched(const char* what, cudaError_t e) {
+  if (e == cudaSuccess) return 0;
+  snprintf(g_comm_err, sizeof(g_comm_err), "%s launch: %s", what, cudaGetErrorString(e));
+  return -1;
+}
+
 int b200dp_comm_clip_bytes() { return (int)sizeof(ClipArgs); }
 
 // phase: 0 reduce into k.r + norm slots (K1c), 1 clip + optimizer update from k.r (K9).  dtype as in
 // b200dp_comm_allreduce: the dtype of the gradient bucket on the wire and of the parameter output.
 int b200dp_comm_clip_bucket(const CommCtx* ctx, const ARArgs* args, const ClipArgs* clip, int phase, int dtype,
                             int blocks, int threads, unsigned long long stream) {
-  if (blocks < 1 || blocks > B200DP_MAX_BLOCKS || threads < 32 || threads > 512 || (threads & 31) ||
-      ctx->world > B200DP_MAX_RANKS || args->channel < 0 || args->channel >= B200DP_NUM_CHANNELS ||
-      phase < 0 || phase > 1) {
-    snprintf(g_comm_err, sizeof(g_comm_err), "bad clip launch config blocks=%d threads=%d world=%d ch=%d phase=%d",
-             blocks, threads, ctx->world, args->channel, phase);
-    return -1;
-  }
+  if (!launch_ok("clip", ctx, args->channel, "phase", phase, 2, dtype, blocks, threads)) return -1;
   cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
-  cudaError_t e;
-  if (dtype == 0) e = launch_clip<float>(*ctx, *args, *clip, phase == 1, blocks, threads, st);
-  else if (dtype == 1) e = launch_clip<__nv_bfloat16>(*ctx, *args, *clip, phase == 1, blocks, threads, st);
-  else if (dtype == 2) e = launch_clip<__half>(*ctx, *args, *clip, phase == 1, blocks, threads, st);
-  else e = cudaErrorInvalidValue;
-  if (e != cudaSuccess) {
-    snprintf(g_comm_err, sizeof(g_comm_err), "clip launch: %s", cudaGetErrorString(e));
-    return -1;
-  }
-  return 0;
+  return launched("clip", with_dtype(dtype, [&](auto tag) {
+    using T = typename decltype(tag)::type;
+    if (phase == 1) clip_apply_kernel<T><<<blocks, threads, 0, st>>>(*ctx, *args, *clip);
+    else allreduce_oneshot_clip_kernel<T><<<blocks, threads, 0, st>>>(*ctx, *args, *clip);
+    return cudaGetLastError();
+  }));
 }
 
 int b200dp_comm_clip_finalize(const ClipArgs* clip, unsigned long long stream) {
   clip_finalize_kernel<<<1, 256, 0, (cudaStream_t)(uintptr_t)stream>>>(*clip);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    snprintf(g_comm_err, sizeof(g_comm_err), "clip finalize launch: %s", cudaGetErrorString(e));
-    return -1;
-  }
-  return 0;
+  return launched("clip finalize", cudaGetLastError());
 }
 
 int b200dp_comm_lw_bytes() { return (int)sizeof(LwArgs); }
@@ -1117,104 +1059,61 @@ int b200dp_comm_lw_bytes() { return (int)sizeof(LwArgs); }
 // args->h.kind selects LARS or LAMB.  dtype as in b200dp_comm_allreduce.
 int b200dp_comm_lw_bucket(const CommCtx* ctx, const ARArgs* args, const LwArgs* lw, int phase, int dtype,
                           int blocks, int threads, unsigned long long stream) {
-  if (blocks < 1 || blocks > B200DP_MAX_BLOCKS || threads < 32 || threads > 512 || (threads & 31) ||
-      ctx->world > B200DP_MAX_RANKS || args->channel < 0 || args->channel >= B200DP_NUM_CHANNELS ||
-      phase < 0 || phase > 1 || (args->h.kind != OPT_LARS && args->h.kind != OPT_LAMB) || lw->nchunks < 0) {
-    snprintf(g_comm_err, sizeof(g_comm_err),
-             "bad layer-wise launch config blocks=%d threads=%d world=%d ch=%d phase=%d kind=%d chunks=%d",
-             blocks, threads, ctx->world, args->channel, phase, args->h.kind, lw->nchunks);
+  if (!launch_ok("layer-wise", ctx, args->channel, "phase", phase, 2, dtype, blocks, threads)) return -1;
+  if ((args->h.kind != OPT_LARS && args->h.kind != OPT_LAMB) || lw->nchunks < 0) {
+    snprintf(g_comm_err, sizeof(g_comm_err), "bad layer-wise launch: kind=%d chunks=%d", args->h.kind, lw->nchunks);
     return -1;
   }
   cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
-  cudaError_t e;
-  if (dtype == 0) e = launch_lw<float>(*ctx, *args, *lw, phase == 1, blocks, threads, st);
-  else if (dtype == 1) e = launch_lw<__nv_bfloat16>(*ctx, *args, *lw, phase == 1, blocks, threads, st);
-  else if (dtype == 2) e = launch_lw<__half>(*ctx, *args, *lw, phase == 1, blocks, threads, st);
-  else e = cudaErrorInvalidValue;
-  if (e != cudaSuccess) {
-    snprintf(g_comm_err, sizeof(g_comm_err), "layer-wise launch: %s", cudaGetErrorString(e));
-    return -1;
-  }
-  return 0;
+  return launched("layer-wise", with_dtype(dtype, [&](auto tag) {
+    using T = typename decltype(tag)::type;
+    if (phase == 1) lw_apply_kernel<T><<<blocks, threads, 0, st>>>(*ctx, *args, *lw);
+    else allreduce_oneshot_lw_kernel<T><<<blocks, threads, 0, st>>>(*ctx, *args, *lw);
+    return cudaGetLastError();
+  }));
 }
 
 // algo: 0 one-shot, 1 two-shot, 2 NVLS.  dtype: 0 fp32, 1 bf16, 2 fp16.
 int b200dp_comm_allreduce(const CommCtx* ctx, const ARArgs* args, int algo, int dtype, int blocks,
                           int threads, unsigned long long stream) {
-  if (blocks < 1 || blocks > B200DP_MAX_BLOCKS || threads < 32 || threads > 512 ||
-      ctx->world > B200DP_MAX_RANKS || args->channel < 0 || args->channel >= B200DP_NUM_CHANNELS) {
-    snprintf(g_comm_err, sizeof(g_comm_err), "bad launch config blocks=%d threads=%d world=%d ch=%d",
-             blocks, threads, ctx->world, args->channel);
-    return -1;
-  }
+  if (!launch_ok("allreduce", ctx, args->channel, "algo", algo, 3, dtype, blocks, threads)) return -1;
   cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
-  cudaError_t e;
-  if (dtype == 0) e = launch_ar<float>(*ctx, *args, algo, blocks, threads, st);
-  else if (dtype == 1) e = launch_ar<__nv_bfloat16>(*ctx, *args, algo, blocks, threads, st);
-  else if (dtype == 2) e = launch_ar<__half>(*ctx, *args, algo, blocks, threads, st);
-  else e = cudaErrorInvalidValue;
-  if (e != cudaSuccess) {
-    snprintf(g_comm_err, sizeof(g_comm_err), "allreduce launch: %s", cudaGetErrorString(e));
-    return -1;
-  }
-  return 0;
+  return launched("allreduce", with_dtype(dtype, [&](auto tag) {
+    using T = typename decltype(tag)::type;
+    if (algo == 0) allreduce_oneshot_kernel<T><<<blocks, threads, 0, st>>>(*ctx, *args);
+    else if (algo == 1) allreduce_sliced_kernel<T, false><<<blocks, threads, 0, st>>>(*ctx, *args);
+    else allreduce_sliced_kernel<T, true><<<blocks, threads, 0, st>>>(*ctx, *args);
+    return cudaGetLastError();
+  }));
 }
 
 // mode: 0 reduce-scatter, 1 all-gather, 2 all-to-all.  dtype as in b200dp_comm_allreduce (reduce-scatter only).
 int b200dp_comm_collective(const CommCtx* ctx, const CollArgs* args, int mode, int dtype, int blocks, int threads,
                            unsigned long long stream) {
-  if (blocks < 1 || blocks > B200DP_MAX_BLOCKS || threads < 32 || threads > 512 ||
-      args->channel < 0 || args->channel >= B200DP_NUM_CHANNELS) {
-    snprintf(g_comm_err, sizeof(g_comm_err), "bad launch config");
-    return -1;
-  }
+  if (!launch_ok("collective", ctx, args->channel, "mode", mode, 3, dtype, blocks, threads)) return -1;
   cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
-  if (mode == 0) {
-    const bool mc = args->use_mc != 0;
-    if (dtype == 0) {
-      if (mc) reducescatter_kernel<float, true><<<blocks, threads, 0, st>>>(*ctx, *args);
-      else reducescatter_kernel<float, false><<<blocks, threads, 0, st>>>(*ctx, *args);
-    } else if (dtype == 1) {
-      if (mc) reducescatter_kernel<__nv_bfloat16, true><<<blocks, threads, 0, st>>>(*ctx, *args);
-      else reducescatter_kernel<__nv_bfloat16, false><<<blocks, threads, 0, st>>>(*ctx, *args);
-    } else if (dtype == 2) {
-      if (mc) reducescatter_kernel<__half, true><<<blocks, threads, 0, st>>>(*ctx, *args);
-      else reducescatter_kernel<__half, false><<<blocks, threads, 0, st>>>(*ctx, *args);
-    } else {
-      snprintf(g_comm_err, sizeof(g_comm_err), "reduce-scatter: unsupported dtype %d", dtype);
-      return -1;
-    }
-  } else if (mode == 1) {
+  if (mode == 1) {
     allgather_kernel<<<blocks, threads, 0, st>>>(*ctx, *args);
   } else if (mode == 2) {
     alltoall_kernel<<<blocks, threads, 0, st>>>(*ctx, *args);
   } else {
-    snprintf(g_comm_err, sizeof(g_comm_err), "unknown collective mode %d", mode);
-    return -1;
+    return launched("reduce-scatter", with_dtype(dtype, [&](auto tag) {
+      using T = typename decltype(tag)::type;
+      if (args->use_mc) reducescatter_kernel<T, true><<<blocks, threads, 0, st>>>(*ctx, *args);
+      else reducescatter_kernel<T, false><<<blocks, threads, 0, st>>>(*ctx, *args);
+      return cudaGetLastError();
+    }));
   }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    snprintf(g_comm_err, sizeof(g_comm_err), "collective launch: %s", cudaGetErrorString(e));
-    return -1;
-  }
-  return 0;
+  return launched("collective", cudaGetLastError());
 }
 
 int b200dp_comm_coll_bytes() { return (int)sizeof(CollArgs); }
 
 int b200dp_comm_broadcast(const CommCtx* ctx, const BcastArgs* args, int blocks, int threads,
                           unsigned long long stream) {
-  if (blocks < 1 || blocks > B200DP_MAX_BLOCKS || threads < 32 || threads > 512) {
-    snprintf(g_comm_err, sizeof(g_comm_err), "bad launch config");
-    return -1;
-  }
+  if (!launch_ok("broadcast", ctx, args->channel, "-", 0, 1, 0, blocks, threads)) return -1;
   broadcast_kernel<<<blocks, threads, 0, (cudaStream_t)(uintptr_t)stream>>>(*ctx, *args);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    snprintf(g_comm_err, sizeof(g_comm_err), "broadcast launch: %s", cudaGetErrorString(e));
-    return -1;
-  }
-  return 0;
+  return launched("broadcast", cudaGetLastError());
 }
 
 }  // extern "C"

@@ -34,6 +34,7 @@ tensor; the per-bucket chunk table is built once here and kept on the device, so
 """
 from __future__ import annotations
 
+import contextlib
 import weakref
 from typing import Dict, List, Optional
 
@@ -48,6 +49,10 @@ _ENGINES: "weakref.WeakSet[FusedEngine]" = weakref.WeakSet()
 LW_CHUNK_ELEMS = 16384          # elements per chunk of the LARS / LAMB partial norms
 _LAYERWISE_KINDS = ("lars", "lamb")
 _logged_layerwise_fallback = False
+
+
+def _elem_size(dtype: torch.dtype) -> int:
+    return torch.empty((), dtype=dtype).element_size()
 
 
 def live_engines():
@@ -152,38 +157,19 @@ class FusedEngine:
         second_moment = kind in ("adam", "adamw", "lamb")
         self.arenas: Dict[torch.dtype, dict] = {}
         for (dtype, device), n in arena_sizes(buckets).items():
-            if self.wire is not None:
-                wes = torch.empty((), dtype=self.wire).element_size()
-                G = symm.alloc(n * wes)
-                P = symm.alloc(n * wes)                     # 16-bit shadow of the updated parameters (kernel output)
-                gw = G.tensor(self.wire, n)
-                gw.zero_()
-                P.tensor(self.wire, n).zero_()
-                self.arenas[dtype] = {
-                    "G": G, "P": P, "gw": gw,
-                    "g": torch.zeros(n, dtype=torch.float32, device=device),      # local fp32 gradients (autograd)
-                    "p": torch.zeros(n, dtype=torch.float32, device=device),      # the model's fp32 parameters
-                    "M": None,
-                    "S0": torch.zeros(n, dtype=torch.float32, device=device),
-                    "S1": torch.zeros(n, dtype=torch.float32, device=device) if second_moment else None,
-                }
-                continue
-            es = torch.empty((), dtype=dtype).element_size()
-            G = symm.alloc(n * es)
-            P = symm.alloc(n * es)
-            g, p = G.tensor(dtype, n), P.tensor(dtype, n)
+            def f32(on: bool = True):
+                return torch.zeros(n, dtype=torch.float32, device=device) if on else None
+            kdtype = self.wire if self.wire is not None else dtype      # dtype the kernel moves over NVLink
+            G = symm.alloc(n * _elem_size(kdtype))
+            P = symm.alloc(n * _elem_size(kdtype))                       # with wire: 16-bit shadow of the parameters
+            g, p = G.tensor(kdtype, n), P.tensor(kdtype, n)
             g.zero_()
             p.zero_()
-            self.arenas[dtype] = {
-                "G": G, "P": P, "g": g, "p": p,
-                "M": torch.zeros(n, dtype=torch.float32, device=device)
-                if dtype != torch.float32 else None,
-                "S0": torch.zeros(n, dtype=torch.float32, device=device),
-                "S1": torch.zeros(n, dtype=torch.float32, device=device) if second_moment else None,
-            }
-        for (dtype, device), n in arena_sizes(buckets).items():
-            self.arenas[dtype]["R"] = torch.zeros(n, dtype=torch.float32, device=device) \
-                if self.clip or self.layerwise else None
+            ar = {"G": G, "P": P, "g": g, "p": p, "M": f32(dtype != torch.float32), "S0": f32(),
+                  "S1": f32(second_moment), "R": f32(self.clip or self.layerwise)}
+            if self.wire is not None:       # local fp32 gradients (autograd) and the model's fp32 parameters
+                ar["gw"], ar["g"], ar["p"] = g, f32(), f32()
+            self.arenas[dtype] = ar
         # re-home parameters and gradients into the arenas
         with torch.no_grad():
             for b in buckets:
@@ -198,7 +184,11 @@ class FusedEngine:
         self.side = torch.cuda.Stream(device=self.device, priority=-1)
         self._args: Dict[int, object] = {}
         self._algo: Dict[int, int] = {}
+        self._kdtype: Dict[int, torch.dtype] = {}       # per bucket: dtype and byte count the kernel moves
+        self._kbytes: Dict[int, int] = {}
         for b in buckets:
+            self._kdtype[b.index] = self.wire if self.wire is not None else b.dtype
+            self._kbytes[b.index] = b.numel * _elem_size(self._kdtype[b.index])
             self._args[b.index], self._algo[b.index] = self._make_args(b)
         self.grad_norm: Optional[torch.Tensor] = None
         if self.clip:
@@ -272,10 +262,8 @@ class FusedEngine:
     def _make_args(self, b: Bucket):
         S, symm = self.S, self.symm
         ar = self.arenas[b.dtype]
-        kdtype = self.wire if self.wire is not None else b.dtype      # dtype the kernel moves over NVLink
-        es = torch.empty((), dtype=kdtype).element_size()
-        off = b.flat_offset * es
-        nbytes = b.numel * es
+        nbytes = self._kbytes[b.index]
+        off = b.flat_offset * _elem_size(self._kdtype[b.index])
         a = S.ARArgs()
         gp, pp = ar["G"].ptrs_at(off), ar["P"].ptrs_at(off)
         for r in range(self.world):
@@ -362,7 +350,9 @@ class FusedEngine:
 
     # ------------------------------------------------------------------ hot path
     def _fill_hyper(self, a, group: dict):
+        """This step's hyper-parameters of ``group`` and the ``lr_scale`` pointer, into argument block ``a``."""
         S, h = self.S, a.h
+        a.lr_scale = self.lr_scale.data_ptr() if self.lr_scale is not None else 0
         lr = group["lr"]
         h.lr = float(lr)
         h.weight_decay = float(group.get("weight_decay", 0.0))
@@ -390,7 +380,6 @@ class FusedEngine:
         self._check_homes(b)
         a = self._args[b.index]
         self._fill_hyper(a, self.opt.param_groups[b.group_index])
-        a.lr_scale = self.lr_scale.data_ptr() if self.lr_scale is not None else 0
         if self.wire is not None:            # compress: fp32 gradients -> wire dtype in symmetric memory
             ar = self.arenas[b.dtype]
             lo, hi = b.flat_offset, b.flat_offset + b.numel
@@ -403,35 +392,38 @@ class FusedEngine:
         ev = torch.cuda.Event()
         ev.record(cur)
         self.side.wait_event(ev)
+        op = "FUSED_ALLREDUCE_" + self.S.ALGO_NAMES[self._algo[b.index]].upper()
+        kdtype, kbytes = self._kdtype[b.index], self._kbytes[b.index]
+        with self._span(f"bucket.{b.index}", op, b.nbytes, f"bucket.{b.index} {op} {b.nbytes / 2**20:.1f}MB"):
+            if self.clip:
+                self.symm.launch_clip_bucket(a, self._clip_args[b.index], self.S.CLIP_REDUCE, kdtype, kbytes, self.side)
+            elif self.layerwise:
+                group = self.opt.param_groups[b.group_index]
+                k = self._lw_args[b.index]
+                k.adaptive = int(bool(group["adaptive"]))
+                k.trust_coef = float(group["trust_coefficient"]) if self.kind == "lars" else 1.0
+                self.symm.launch_lw_bucket(a, k, self.S.LW_REDUCE, kdtype, kbytes, self.side)
+                self.symm.launch_lw_bucket(a, k, self.S.LW_APPLY, kdtype, kbytes, self.side)
+                self.kernel_launches += 1
+            else:
+                self.symm.launch_allreduce(a, self._algo[b.index], kdtype, kbytes, self.side)
+            self.kernel_launches += 1
+        return True
+
+    @contextlib.contextmanager
+    def _span(self, name: str, op: str, nbytes: int, label: str):
+        """NVTX range ``label`` and timeline span (``name``, ``op``) around the launches made inside it on the
+        side stream."""
         tl = _state.runtime().timeline
         if tl is not None:
             s_ev, e_ev = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             s_ev.record(self.side)
-        if nvtx.enabled():
-            nvtx.push(f"bucket.{b.index} FUSED_ALLREDUCE_{self.S.ALGO_NAMES[self._algo[b.index]].upper()} "
-                      f"{b.nbytes / 2**20:.1f}MB")
-        kdtype = self.wire if self.wire is not None else b.dtype
-        kbytes = b.numel * torch.empty((), dtype=kdtype).element_size()
-        if self.clip:
-            self.symm.launch_clip_bucket(a, self._clip_args[b.index], self.S.CLIP_REDUCE, kdtype, kbytes, self.side)
-        elif self.layerwise:
-            group = self.opt.param_groups[b.group_index]
-            k = self._lw_args[b.index]
-            k.adaptive = int(bool(group["adaptive"]))
-            k.trust_coef = float(group["trust_coefficient"]) if self.kind == "lars" else 1.0
-            self.symm.launch_lw_bucket(a, k, self.S.LW_REDUCE, kdtype, kbytes, self.side)
-            self.symm.launch_lw_bucket(a, k, self.S.LW_APPLY, kdtype, kbytes, self.side)
-            self.kernel_launches += 1
-        else:
-            self.symm.launch_allreduce(a, self._algo[b.index], kdtype, kbytes, self.side)
+        nvtx.push(label)
+        yield
         nvtx.pop()
-        self.kernel_launches += 1
         if tl is not None:
             e_ev.record(self.side)
-            tl.cuda_span(f"bucket.{b.index}", "FUSED_ALLREDUCE_" +
-                         self.S.ALGO_NAMES[self._algo[b.index]].upper(), s_ev, e_ev,
-                         bytes=b.nbytes)
-        return True
+            tl.cuda_span(name, op, s_ev, e_ev, bytes=nbytes)
 
     def wait_all(self, launched):
         if self.clip:
@@ -443,27 +435,16 @@ class FusedEngine:
     def _clip_and_update(self):
         """Clip mode, after every bucket's reduce phase: the global norm and the clip coefficient (one
         launch), then the optimizer update of every bucket from R (one launch each), all on the side stream."""
-        tl = _state.runtime().timeline
-        if tl is not None:
-            s_ev, e_ev = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            s_ev.record(self.side)
-        nvtx.push("CLIP_FINALIZE_APPLY")
-        self.symm.launch_clip_finalize(self._fin_args, self.side)
-        self.kernel_launches += 1
-        lr_scale = self.lr_scale.data_ptr() if self.lr_scale is not None else 0
-        for b in self.buckets:
-            ap = self._apply_args[b.index]
-            self._fill_hyper(ap, self.opt.param_groups[b.group_index])
-            ap.lr_scale = lr_scale
-            kdtype = self.wire if self.wire is not None else b.dtype
-            kbytes = b.numel * torch.empty((), dtype=kdtype).element_size()
-            self.symm.launch_clip_bucket(ap, self._clip_args[b.index], self.S.CLIP_APPLY, kdtype, kbytes, self.side)
+        nbytes = sum(b.numel for b in self.buckets) * 4
+        with self._span("optimizer", "CLIP_FINALIZE_APPLY", nbytes, "CLIP_FINALIZE_APPLY"):
+            self.symm.launch_clip_finalize(self._fin_args, self.side)
             self.kernel_launches += 1
-        nvtx.pop()
-        if tl is not None:
-            e_ev.record(self.side)
-            tl.cuda_span("optimizer", "CLIP_FINALIZE_APPLY", s_ev, e_ev,
-                         bytes=sum(b.numel for b in self.buckets) * 4)
+            for b in self.buckets:
+                ap = self._apply_args[b.index]
+                self._fill_hyper(ap, self.opt.param_groups[b.group_index])
+                self.symm.launch_clip_bucket(ap, self._clip_args[b.index], self.S.CLIP_APPLY, self._kdtype[b.index],
+                                             self._kbytes[b.index], self.side)
+                self.kernel_launches += 1
 
     def after_step(self):
         self.steps += 1

@@ -35,7 +35,7 @@ class _LocalBuffer:
         return [self.local_ptr + off]
 
 
-class LocalRuntime:
+class LocalRuntime(S.KernelLauncher):
     _inst: Optional["LocalRuntime"] = None
 
     @classmethod
@@ -82,11 +82,6 @@ class LocalRuntime:
     def pick_blocks(self, algo: int, nbytes: int) -> int:
         per_block = 512 * 16 * 4
         return int(max(1, min((nbytes + per_block - 1) // per_block, self.max_blocks or 128)))
-
-    launch_allreduce = S.SymmRuntime.launch_allreduce
-    launch_clip_bucket = S.SymmRuntime.launch_clip_bucket
-    launch_clip_finalize = S.SymmRuntime.launch_clip_finalize
-    launch_lw_bucket = S.SymmRuntime.launch_lw_bucket
 
     def allreduce_(self, t, prescale=1.0, postscale=1.0, algo=None):
         if prescale * postscale != 1.0:

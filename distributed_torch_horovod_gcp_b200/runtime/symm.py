@@ -142,7 +142,45 @@ def watchdog_seconds() -> float:
     return 300.0
 
 
-class SymmRuntime:
+class KernelLauncher:
+    """The fused-kernel launches, shared by ``SymmRuntime`` and the world-size-1 ``LocalRuntime``: both provide
+    ``lib``, ``ctx``, ``launches`` and ``pick_blocks``."""
+
+    def _launched(self, rc: int):
+        """Raise the library's message if a C entry point failed; count the launch otherwise."""
+        if rc != 0:
+            raise RuntimeError((self.lib.b200dp_comm_last_error() or b"").decode())
+        self.launches += 1
+
+    def launch_allreduce(self, args: ARArgs, algo: int, dtype: torch.dtype, nbytes: int,
+                         stream: torch.cuda.Stream, blocks: Optional[int] = None):
+        blocks = blocks or self.pick_blocks(algo, nbytes)
+        self._launched(self.lib.b200dp_comm_allreduce(ctypes.byref(self.ctx), ctypes.byref(args), algo,
+                                                      _DTYPE_CODE[dtype], blocks, 512, stream.cuda_stream))
+
+    def launch_clip_bucket(self, args: ARArgs, clip: ClipArgs, phase: int, dtype: torch.dtype, nbytes: int,
+                           stream: torch.cuda.Stream):
+        """One bucket of the clip-mode engine: ``CLIP_REDUCE`` (one-shot reduction into ``clip.r`` plus the
+        per-CTA norm slots) or ``CLIP_APPLY`` (scale ``clip.r`` by the clip coefficient, optimizer update).
+        Both phases of a bucket use the same grid, so the reduce phase fills the same slots every step."""
+        blocks = self.pick_blocks(ALGO_ONESHOT, nbytes)
+        self._launched(self.lib.b200dp_comm_clip_bucket(ctypes.byref(self.ctx), ctypes.byref(args), ctypes.byref(clip),
+                                                        phase, _DTYPE_CODE[dtype], blocks, 512, stream.cuda_stream))
+
+    def launch_clip_finalize(self, clip: ClipArgs, stream: torch.cuda.Stream):
+        """Sum every bucket's norm slots (fixed order) into the global norm and the clip coefficient."""
+        self._launched(self.lib.b200dp_comm_clip_finalize(ctypes.byref(clip), stream.cuda_stream))
+
+    def launch_lw_bucket(self, args: ARArgs, lw: LwArgs, phase: int, dtype: torch.dtype, nbytes: int,
+                         stream: torch.cuda.Stream):
+        """One bucket of a LARS / LAMB engine: ``LW_REDUCE`` (one-shot reduction, update direction into
+        ``lw.r``, per-chunk sums of squares) or ``LW_APPLY`` (per-tensor trust ratios, update, step counter)."""
+        blocks = self.pick_blocks(ALGO_ONESHOT, nbytes)
+        self._launched(self.lib.b200dp_comm_lw_bucket(ctypes.byref(self.ctx), ctypes.byref(args), ctypes.byref(lw),
+                                                      phase, _DTYPE_CODE[dtype], blocks, 512, stream.cuda_stream))
+
+
+class SymmRuntime(KernelLauncher):
     def __init__(self):
         raise RuntimeError("use SymmRuntime.create")
 
@@ -397,45 +435,6 @@ class SymmRuntime:
         return int(min(b, cap))
 
     # ------------------------------------------------------------------ launches
-    def launch_allreduce(self, args: ARArgs, algo: int, dtype: torch.dtype, nbytes: int,
-                         stream: torch.cuda.Stream, blocks: Optional[int] = None):
-        blocks = blocks or self.pick_blocks(algo, nbytes)
-        rc = self.lib.b200dp_comm_allreduce(ctypes.byref(self.ctx), ctypes.byref(args), algo,
-                                            _DTYPE_CODE[dtype], blocks, 512, stream.cuda_stream)
-        if rc != 0:
-            raise RuntimeError((self.lib.b200dp_comm_last_error() or b"").decode())
-        self.launches += 1
-
-    def launch_clip_bucket(self, args: ARArgs, clip: ClipArgs, phase: int, dtype: torch.dtype, nbytes: int,
-                           stream: torch.cuda.Stream):
-        """One bucket of the clip-mode engine: ``CLIP_REDUCE`` (one-shot reduction into ``clip.r`` plus the
-        per-CTA norm slots) or ``CLIP_APPLY`` (scale ``clip.r`` by the clip coefficient, optimizer update).
-        Both phases of a bucket use the same grid, so the reduce phase fills the same slots every step."""
-        blocks = self.pick_blocks(ALGO_ONESHOT, nbytes)
-        rc = self.lib.b200dp_comm_clip_bucket(ctypes.byref(self.ctx), ctypes.byref(args), ctypes.byref(clip),
-                                              phase, _DTYPE_CODE[dtype], blocks, 512, stream.cuda_stream)
-        if rc != 0:
-            raise RuntimeError((self.lib.b200dp_comm_last_error() or b"").decode())
-        self.launches += 1
-
-    def launch_clip_finalize(self, clip: ClipArgs, stream: torch.cuda.Stream):
-        """Sum every bucket's norm slots (fixed order) into the global norm and the clip coefficient."""
-        rc = self.lib.b200dp_comm_clip_finalize(ctypes.byref(clip), stream.cuda_stream)
-        if rc != 0:
-            raise RuntimeError((self.lib.b200dp_comm_last_error() or b"").decode())
-        self.launches += 1
-
-    def launch_lw_bucket(self, args: ARArgs, lw: LwArgs, phase: int, dtype: torch.dtype, nbytes: int,
-                         stream: torch.cuda.Stream):
-        """One bucket of a LARS / LAMB engine: ``LW_REDUCE`` (one-shot reduction, update direction into
-        ``lw.r``, per-chunk sums of squares) or ``LW_APPLY`` (per-tensor trust ratios, update, step counter)."""
-        blocks = self.pick_blocks(ALGO_ONESHOT, nbytes)
-        rc = self.lib.b200dp_comm_lw_bucket(ctypes.byref(self.ctx), ctypes.byref(args), ctypes.byref(lw),
-                                            phase, _DTYPE_CODE[dtype], blocks, 512, stream.cuda_stream)
-        if rc != 0:
-            raise RuntimeError((self.lib.b200dp_comm_last_error() or b"").decode())
-        self.launches += 1
-
     def _lane(self, lane: int):
         """(staging buffer, signal channel) of a lane.  Lane 0 serves user collectives on the caller's
         stream; lane 1 is private to DistributedOptimizer's un-fused bucket path, which runs on its own
@@ -489,18 +488,7 @@ class SymmRuntime:
             t.is_contiguous(), "prepare_allreduce needs a 16B-aligned contiguous symmetric tensor"
         buf, off = loc
         nbytes = t.numel() * es
-        a = ARArgs()
-        ptrs = buf.ptrs_at(off)
-        for r in range(self.world):
-            a.inp[r] = ptrs[r]
-            a.out[r] = ptrs[r]
-        a.n, a.scale, a.channel = t.numel(), float(scale), CH_USER
-        a.h.kind = OPT_NONE
-        algo = self.pick_algo(nbytes, need_mc=buf.mc_ptr != 0) if algo is None else algo
-        if algo == ALGO_NVLS and buf.mc_ptr == 0:
-            algo = ALGO_TWOSHOT
-        if algo == ALGO_NVLS:
-            a.in_mc = a.out_mc = buf.mc_ptr + off
+        a, algo = self._user_args(buf, off, t.numel(), nbytes, scale, algo, CH_USER)
         if algo == ALGO_ONESHOT:
             scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
             a.scratch, a.copy_back = scratch.data_ptr(), 1
@@ -512,30 +500,34 @@ class SymmRuntime:
         dev = self.device
 
         def launch(_keep=(a, scratch, t)):
-            rc = fn(ctx_ref, a_ref, algo, code, blocks, 512, torch.cuda.current_stream(dev).cuda_stream)
-            if rc != 0:
-                raise RuntimeError((self.lib.b200dp_comm_last_error() or b"").decode())
+            self._launched(fn(ctx_ref, a_ref, algo, code, blocks, 512, torch.cuda.current_stream(dev).cuda_stream))
         launch.algo = ALGO_NAMES[algo]
         launch.blocks = blocks
         return launch
 
-    def _ar_symm(self, buf: SymmBuffer, off: int, numel: int, dtype, scale, stream, algo,
-                 user: bool = False, channel: int = CH_USER):
-        es = torch.empty((), dtype=dtype).element_size()
-        nbytes = numel * es
+    def _user_args(self, buf: SymmBuffer, off: int, numel: int, nbytes: int, scale: float, algo: Optional[int],
+                   channel: int) -> Tuple[ARArgs, int]:
+        """Argument block of an in-place sum-allreduce (no optimizer) of ``numel`` elements at byte ``off`` of
+        ``buf``, and its algorithm: ``algo``, or the tuned choice; two-shot instead of NVLS where ``buf`` has no
+        multicast address.  The caller supplies the one-shot scratch."""
         a = ARArgs()
         ptrs = buf.ptrs_at(off)
         for r in range(self.world):
             a.inp[r] = ptrs[r]
             a.out[r] = ptrs[r]
-        a.n, a.scale, a.channel = numel, scale, channel
+        a.n, a.scale, a.channel = numel, float(scale), channel
         a.h.kind = OPT_NONE
         algo = self.pick_algo(nbytes, need_mc=buf.mc_ptr != 0) if algo is None else algo
         if algo == ALGO_NVLS and buf.mc_ptr == 0:
             algo = ALGO_TWOSHOT
         if algo == ALGO_NVLS:
-            a.in_mc = buf.mc_ptr + off
-            a.out_mc = buf.mc_ptr + off
+            a.in_mc = a.out_mc = buf.mc_ptr + off
+        return a, algo
+
+    def _ar_symm(self, buf: SymmBuffer, off: int, numel: int, dtype, scale, stream, algo,
+                 user: bool = False, channel: int = CH_USER):
+        nbytes = numel * torch.empty((), dtype=dtype).element_size()
+        a, algo = self._user_args(buf, off, numel, nbytes, scale, algo, channel)
         if algo == ALGO_ONESHOT:
             key = "scratch" if channel == CH_USER else "scratch_opt"
             sc = getattr(self, key, None)
@@ -549,11 +541,8 @@ class SymmRuntime:
     # ------------------------------------------------------------------ reduce-scatter / all-gather / all-to-all
     def _coll(self, mode: int, a: CollArgs, dtype, work_bytes: int, stream):
         blocks = max(1, min((work_bytes + 512 * 16 * 2 - 1) // (512 * 16 * 2), self.max_blocks or 48))
-        rc = self.lib.b200dp_comm_collective(ctypes.byref(self.ctx), ctypes.byref(a), mode,
-                                             _DTYPE_CODE.get(dtype, 0), blocks, 512, stream.cuda_stream)
-        if rc != 0:
-            raise RuntimeError((self.lib.b200dp_comm_last_error() or b"").decode())
-        self.launches += 1
+        self._launched(self.lib.b200dp_comm_collective(ctypes.byref(self.ctx), ctypes.byref(a), mode,
+                                                       _DTYPE_CODE.get(dtype, 0), blocks, 512, stream.cuda_stream))
 
     def reducescatter(self, src: torch.Tensor, out: torch.Tensor, scale: float = 1.0) -> torch.cuda.Event:
         """``out`` (numel = src.numel() / world) = scale * sum over ranks of chunk ``rank`` of ``src``.
@@ -655,11 +644,8 @@ class SymmRuntime:
         a.nbytes, a.root, a.channel = nbytes, root, CH_BCAST
         a.use_mc = 1 if (buf.mc_ptr and os.environ.get("B200DP_BCAST_P2P", "0") != "1") else 0
         blocks = max(1, min((nbytes + 512 * 16 * 4 - 1) // (512 * 16 * 4), 32))
-        rc = self.lib.b200dp_comm_broadcast(ctypes.byref(self.ctx), ctypes.byref(a), blocks, 512,
-                                            stream.cuda_stream)
-        if rc != 0:
-            raise RuntimeError((self.lib.b200dp_comm_last_error() or b"").decode())
-        self.launches += 1
+        self._launched(self.lib.b200dp_comm_broadcast(ctypes.byref(self.ctx), ctypes.byref(a), blocks, 512,
+                                                      stream.cuda_stream))
 
     # ------------------------------------------------------------------ watchdog / teardown
     def check_errors(self):
