@@ -74,6 +74,9 @@ def parse_args(argv=None):
                    help="dropout probability between stacked LSTM layers (nn.LSTM dropout=; 0 = off, the "
                         "reference).  Like the reference, validation does not switch the model to eval mode, "
                         "so with P > 0 the printed test_loss is computed with dropout on")
+    p.add_argument("--dropout", type=float, default=float(env("B200DP_DROPOUT", "0")),
+                   help="dropout probability of the GPT and ViT models (GPT: embedding, attention and residual "
+                        "dropout, as GPT-2's 0.1; ViT: token, attention and residual dropout; 0 = off)")
     p.add_argument("--clip-grad-norm", type=float, default=float(env("B200DP_CLIP_GRAD_NORM", "0")),
                    help="clip the averaged gradient by its global L2 norm to at most this value before "
                         "each update (DistributedOptimizer max_grad_norm=; 0 = off, the reference)")
@@ -85,6 +88,10 @@ def parse_args(argv=None):
     args = p.parse_args(argv)
     if args.optimizer != "default" and args.model.lower() == "lstm":
         p.error("--optimizer lars|lamb applies to the image models")
+    if not 0.0 <= args.dropout <= 1.0:
+        p.error(f"--dropout must be in [0, 1], got {args.dropout}")
+    if args.dropout and not (is_gpt(args.model) or is_vit(args.model)):
+        p.error("--dropout applies to the GPT and ViT models (the LSTM has --lstm-dropout)")
     return args
 
 
@@ -103,6 +110,19 @@ def image_optimizer(model, kind, lr):
 
 def is_gpt(name):
     return name.lower().replace("-", "").replace("_", "") in ("gpt2", "gpttiny")
+
+
+def is_vit(name):
+    return name.lower().replace("-", "").replace("_", "").startswith("vit")
+
+
+def dropout_kw(args):
+    """Model keyword arguments of ``--dropout`` (none at 0, so the models are built as without it)."""
+    if not args.dropout:
+        return {}
+    if is_gpt(args.model):
+        return {"dropout": args.dropout}
+    return {"dropout": args.dropout, "attention_dropout": args.dropout}
 
 
 def gpt_optimizer(model, lr):
@@ -184,7 +204,7 @@ if __name__ == "__main__":
         optimizer = torch.optim.Adam(model.parameters(), lr=args.lr)
         loss_fn = nn.MSELoss(reduction="mean")
     elif is_gpt(args.model):
-        model = build_model(args.model).to(_DEVICE)
+        model = build_model(args.model, **dropout_kw(args)).to(_DEVICE)
         if compute_dtype != torch.float32:
             model = model.to(compute_dtype)
         seq_len = args.seq_len or model.context
@@ -209,7 +229,7 @@ if __name__ == "__main__":
             kw["small_input"] = image_size <= 64
         else:
             kw["image_size"] = image_size
-        model = build_model(args.model, **kw).to(_DEVICE)
+        model = build_model(args.model, **kw, **dropout_kw(args)).to(_DEVICE)
         if compute_dtype != torch.float32:
             model = model.to(compute_dtype)
         if use_cuda:

@@ -16,9 +16,14 @@ optimizer).  ``mfu_whole_program`` is the model FLOPs (6 N tokens, N = parameter
 embedding, plus causal attention 6 L B S^2 D) per step time over the 989 TFLOP/s BF16 data-sheet figure: a
 whole-program rate, not any kernel's share of peak.
 
+Dropout arm (``--dropout P``, off by default): attention adds ``causal_drop_ms`` / ``noncausal_drop_ms`` (the
+kernel with ``dropout_p = P``) and ``sdpa_causal_drop_ms`` (SDPA flash with ``dropout_p = P``) on the same
+tensors, and the whole step adds a third alternated arm, ``kernels_dropout``: GPT-2 small built with
+``dropout = P`` (embedding, attention and residual dropout) on the kernels.
+
 Prints one JSON line per config with the card name and power limit read in the same run.
 
-    python benchmarks/gpt_bench.py [--iters 50] [--warmup 10] [--rounds 3]
+    python benchmarks/gpt_bench.py [--iters 50] [--warmup 10] [--rounds 3] [--dropout 0.1]
 """
 import argparse
 import json
@@ -65,31 +70,40 @@ def attention_configs(args, name, power):
                        for _ in range(4)]
         q, k, v = [t.requires_grad_(True) for t in (q, k, v)]
 
-        def kernel(causal):
+        def kernel(causal, p=0.0):
             def run():
-                attention.attention_fused(q, k, v, causal=causal).backward(do)
+                attention.attention_fused(q, k, v, causal=causal, dropout_p=p).backward(do)
             return run
 
-        def sdpa():
-            F.scaled_dot_product_attention(q, k, v, is_causal=True).backward(do)
+        def sdpa(p=0.0):
+            def run():
+                F.scaled_dot_product_attention(q, k, v, dropout_p=p, is_causal=True).backward(do)
+            return run
 
         res = {"config": "attention", "batch_heads": B * H, "seq": S, "head_dim": 64}
         res["causal_ms"] = round(time_ms(kernel(True), args.iters, args.warmup), 4)
         res["noncausal_ms"] = round(time_ms(kernel(False), args.iters, args.warmup), 4)
-        res["sdpa_causal_ms"] = round(time_ms(sdpa, args.iters, args.warmup), 4)
+        res["sdpa_causal_ms"] = round(time_ms(sdpa(), args.iters, args.warmup), 4)
         res["causal_vs_noncausal"] = round(res["noncausal_ms"] / res["causal_ms"], 3)
         res["causal_vs_sdpa"] = round(res["sdpa_causal_ms"] / res["causal_ms"], 3)
         flops = 3.5 * 4 * B * H * S * S * 64 / 2
         res["causal_tflops"] = round(flops / (res["causal_ms"] * 1e-3) / 1e12, 1)
+        if args.dropout:
+            res["dropout_p"] = args.dropout
+            res["causal_drop_ms"] = round(time_ms(kernel(True, args.dropout), args.iters, args.warmup), 4)
+            res["noncausal_drop_ms"] = round(time_ms(kernel(False, args.dropout), args.iters, args.warmup), 4)
+            res["sdpa_causal_drop_ms"] = round(time_ms(sdpa(args.dropout), args.iters, args.warmup), 4)
+            res["causal_drop_cost"] = round(res["causal_drop_ms"] / res["causal_ms"], 3)
+            res["noncausal_drop_cost"] = round(res["noncausal_drop_ms"] / res["noncausal_ms"], 3)
         res.update({"gpu": name, "power_limit": power})
         print(json.dumps(res), flush=True)
 
 
-def step_arm(hvd, kernels_on, x, y, warmup):
+def step_arm(hvd, kernels_on, x, y, warmup, dropout=0.0):
     from distributed_torch_horovod_gcp_b200.models import gpt2
     from distributed_torch_horovod_gcp_b200.utils.graph import GraphedStep
     torch.manual_seed(0)
-    model = gpt2().cuda().to(torch.bfloat16)
+    model = gpt2(dropout=dropout).cuda().to(torch.bfloat16)
     groups = [{"params": [p for p in model.parameters() if p.dim() >= 2], "weight_decay": 0.1},
               {"params": [p for p in model.parameters() if p.dim() < 2], "weight_decay": 0.0}]
     opt = hvd.DistributedOptimizer(torch.optim.AdamW(groups, lr=6e-4, betas=(0.9, 0.95)),
@@ -120,7 +134,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=50)
     ap.add_argument("--warmup", type=int, default=10)
-    ap.add_argument("--rounds", type=int, default=3, help="alternations of the two whole-step arms")
+    ap.add_argument("--rounds", type=int, default=3, help="alternations of the whole-step arms")
+    ap.add_argument("--dropout", type=float, default=0.0, help="add the dropout arms with this probability")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("gpt_bench needs a GPU")
@@ -141,10 +156,15 @@ def main():
     assert c1.get("attn_fwd", 0) > c0.get("attn_fwd", 0), "the kernel arm did not run the attention kernel"
     run_s, _ = step_arm(hvd, False, x, y, 3)
     assert counters.snapshot().get("attn_fwd", 0) == c1.get("attn_fwd", 0), "the stand-in arm ran a kernel"
-    times = {"kernels": [], "stand_in": []}
+    arms = {"kernels": run_k, "stand_in": run_s}
+    if args.dropout:
+        c2 = counters.snapshot()
+        arms["kernels_dropout"], _ = step_arm(hvd, True, x, y, 3, args.dropout)
+        assert counters.snapshot().get("attn_fwd_dropout", 0) > c2.get("attn_fwd_dropout", 0)
+    times = {arm: [] for arm in arms}
     for _ in range(args.rounds):
-        times["kernels"].append(time_ms(run_k, args.iters, args.warmup))
-        times["stand_in"].append(time_ms(run_s, args.iters, args.warmup))
+        for arm, run in arms.items():
+            times[arm].append(time_ms(run, args.iters, args.warmup))
     tokens = B * S
     flops = 6 * n_params * tokens + 6 * 12 * B * S * S * 768
     res = {"config": "gpt2_step", "batch": B, "seq": S, "dtype": "bf16", "params_counted": n_params,
@@ -156,6 +176,9 @@ def main():
         res[f"{arm}_tokens_per_s"] = round(tokens / (best * 1e-3))
         res[f"{arm}_mfu_whole_program"] = round(flops / (best * 1e-3) / PEAK_BF16, 4)
     res["speedup"] = round(res["stand_in_step_ms"] / res["kernels_step_ms"], 3)
+    if args.dropout:
+        res["dropout_p"] = args.dropout
+        res["dropout_cost"] = round(res["kernels_dropout_step_ms"] / res["kernels_step_ms"], 3)
     res.update({"gpu": name, "power_limit": power, "peak_bf16_tflops_datasheet": PEAK_BF16 / 1e12})
     print(json.dumps(res), flush=True)
     hvd.shutdown()

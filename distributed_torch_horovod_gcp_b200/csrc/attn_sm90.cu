@@ -24,6 +24,27 @@
 // sequence-tail mask drops columns (row max, P, dS), so masked products are exact zeros.  The causal grids
 // launch the longest tiles first.
 //
+// Dropout (DROPOUT = true, probability p > 0; p = 0 launches the DROPOUT = false kernels):
+//   O = (Z o P) V with P the softmax and Z = keep / q, keep in {0, 1}, q = t / 2^16 the keep probability,
+//   t = round((1 - p) 2^16) (philox.cuh: p has a resolution of 2^-16; t = 0, i.e. p = 1, gives scale 0 and
+//   exact zeros).  Forward: the row sum l and the saved LSE are the un-dropped ones, the P tile that feeds the
+//   PV wgmma is keep ? P : 0, and 1/q = 2^16 / t is folded into the final 1 / l multiply.  Backward, with the
+//   same bits recomputed: dV += (keep o P)^T dO, scaled by 1/q once at the end; dS = P o (Z o dP - D) / sqrt(d),
+//   where D = rowsum(dO o O) of the dropped O (= rowsum(P o Z o dP)), so attn_delta_kernel is unchanged.
+//
+//   The mask.  Each (b, h, query row r, key column c) has one keep bit, a pure function of the 128-bit seed
+//   (seed[0], seed[1] in device memory, drawn by torch's CUDA generator) and of (b, h, r, c) alone, so it
+//   does not depend on tiles, grid, strides or CAUSAL:
+//     u    = Philox4x32-10(key = (seed[0] mod 2^32, seed[0] / 2^32),
+//                          counter = (4 (c / 16) + (c mod 8) / 2,  8 (r / 16) + r mod 8,  b H + h,  seed[1] mod 2^32))
+//     word = u[2 ((r / 8) mod 2) + (c / 8) mod 2]           (u[0..3] = the four 32-bit outputs)
+//     bits = (c mod 2) ? word >> 16 : word mod 2^16
+//     keep = bits < t
+//   One Philox call covers rows {r, r + 8} x columns {c, c + 1, c + 8, c + 9} (r mod 16 < 8, c mod 16 < 8,
+//   c even): exactly the 8 elements one thread holds for fragment column pairs jj = 2m, 2m + 1 (see the
+//   fragment layout above attn_fwd_kernel; S = Q K^T has the same layout in the backward), so each thread
+//   draws each Philox output once: 8 calls per 128 x 128 tile.
+//
 // Replaces F.scaled_dot_product_attention (cuDNN / flash library kernels) on the ViT-B/16 and GPT paths.
 // The reference application has no attention.
 #include <cuda.h>
@@ -49,6 +70,9 @@ struct AttnFwdParams {
   __nv_bfloat16* o;
   long long o_sb, o_sh, o_ss;        // element strides of O (d contiguous)
   float* lse;                        // [B][H][S] natural-log sum-exp of the scaled scores (nullptr: not saved)
+  const unsigned long long* seed;    // DROPOUT: Philox key, offset (2 words in device memory)
+  uint32_t drop_thr;                 // DROPOUT: keep when the element's 16 bits are below this (t)
+  float drop_scale;                  // DROPOUT: 2^16 / t (0 when t = 0)
 };
 
 __device__ __forceinline__ float ex2(float x) {
@@ -81,6 +105,23 @@ __device__ __forceinline__ float quad_sum(float v) {
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
+// Dropout bits (see the header): the Philox output for query rows {row, row + 8} (row = the global row of the
+// thread's r0) and key columns col + cq + {0, 1, 8, 9} (col = the global column of fragment pair jj, jj even).
+__device__ __forceinline__ uint4 drop_draw(const unsigned long long* seed, int bh, int row, int col, int cq) {
+  const unsigned long long k = seed[0];
+  const uint32_t off = (uint32_t)seed[1];
+  return philox4x32_10(make_uint4((uint32_t)((col >> 4) * 4 + (cq >> 1)), (uint32_t)((row >> 4) * 8 + (row & 7)),
+                                  (uint32_t)bh, off),
+                       make_uint2((uint32_t)k, (uint32_t)(k >> 32)));
+}
+// Keep bit of fragment element 4 jj + e from the draw of pair 2 (jj / 2): row r0 + 8 (e / 2), column
+// 8 jj + cq + e % 2 -> word 2 (e / 2) + jj % 2, low / high 16 bits for e % 2 = 0 / 1.
+__device__ __forceinline__ bool drop_keep(const uint4& u, int jj, int e, uint32_t thr) {
+  const int w = 2 * (e >> 1) + (jj & 1);
+  const uint32_t word = w == 0 ? u.x : w == 1 ? u.y : w == 2 ? u.z : u.w;
+  return ((e & 1) ? word >> 16 : word & 0xffffu) < thr;
+}
+
 // ---------------------------------------------------------------------------------------------------
 // forward
 // ---------------------------------------------------------------------------------------------------
@@ -89,7 +130,7 @@ constexpr int FW_SMEM = TILE_BYTES * (1 + FW_RING) + 2 * TILE_BYTES /*P*/ + 1024
 
 // Fragment of an m64 x N wgmma accumulator held by thread t of a warpgroup: element 4j + e is row
 // 16 (t / 32) + (t % 32) / 4 + 8 (e / 2), column 8 j + 2 (t % 4) + e % 2.
-template <bool CAUSAL>
+template <bool CAUSAL, bool DROPOUT>
 __global__ void __launch_bounds__(AT, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                 const __grid_constant__ CUtensorMap map_v, const AttnFwdParams p) {
@@ -183,14 +224,21 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
         m[h2] = mn[h2];
         l[h2] *= alpha[h2];
       }
+      uint4 rnd;
 #pragma unroll
       for (int jj = 0; jj < TILE / 8; ++jj) {
+        if constexpr (DROPOUT) {
+          if ((jj & 1) == 0) rnd = drop_draw(p.seed, bh, qt * TILE + r0, j * TILE + 8 * jj, cq);
+        }
         float pe[4];
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
           pe[e] = (8 * jj + cq + (e & 1) < valid && (!diag || 8 * jj + cq + (e & 1) <= r0 + 8 * (e >> 1)))
                       ? ex2(fmaf(sc[4 * jj + e], p.scale_log2, -mn[e >> 1])) : 0.f;
           l[e >> 1] += pe[e];
+          if constexpr (DROPOUT) {
+            if (!drop_keep(rnd, jj, e, p.drop_thr)) pe[e] = 0.f;   // l keeps the un-dropped sum
+          }
         }
         st_pair_sw(sP_u, r0, 8 * jj + cq, TILE_BYTES, pe[0], pe[1]);
         st_pair_sw(sP_u, r0 + 8, 8 * jj + cq, TILE_BYTES, pe[2], pe[3]);
@@ -221,7 +269,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
       const float lt = quad_sum(l[h2]);
       const int qrow = qt * TILE + r0 + 8 * h2;
       if (qrow < p.S) {
-        const float inv = __fdividef(1.0f, lt);
+        const float inv = __fdividef(1.0f, lt) * (DROPOUT ? p.drop_scale : 1.0f);   // dropout: 1/q folded in
         uint32_t* dst = reinterpret_cast<uint32_t*>(p.o + (size_t)b * p.o_sb + (size_t)h * p.o_sh + (size_t)qrow * p.o_ss);
 #pragma unroll
         for (int jj = 0; jj < HD / 8; ++jj)
@@ -245,6 +293,9 @@ struct AttnBwdParams {
   long long dq_sb, dq_sh, dq_ss;
   __nv_bfloat16* dk; __nv_bfloat16* dv;
   long long dk_sb, dk_sh, dk_ss, dv_sb, dv_sh, dv_ss;
+  const unsigned long long* seed;    // DROPOUT: as in AttnFwdParams
+  uint32_t drop_thr;
+  float drop_scale;
 };
 
 // delta[b][h][s] = sum_d dO * O   (8 lanes per row: one 16-byte load of each tensor per lane)
@@ -278,7 +329,7 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const __nv_bfloat16* __
 constexpr int BW_RING = 2;
 constexpr int BW_SMEM = TILE_BYTES * (2 + 2 * BW_RING) + 4 * TILE_BYTES + 1024 + 256;
 
-template <bool CAUSAL>
+template <bool CAUSAL, bool DROPOUT>
 __global__ void __launch_bounds__(AT, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                 const __grid_constant__ CUtensorMap map_v, const __grid_constant__ CUtensorMap map_do,
@@ -383,16 +434,27 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
         lse2[h2] = qok[h2] ? p.lse[bh_off + qrow] * 1.4426950408889634f : 0.f;
         dl[h2] = qok[h2] ? p.delta[bh_off + qrow] : 0.f;
       }
+      uint4 rnd;
 #pragma unroll
       for (int jj = 0; jj < TILE / 8; ++jj) {
+        if constexpr (DROPOUT) {
+          if ((jj & 1) == 0) rnd = drop_draw(p.seed, bh, i * TILE + r0, kb * TILE + 8 * jj, cq);
+        }
         float pv[4], ds[4];
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
           const int h2 = e >> 1;
           const bool ok = qok[h2] && (8 * jj + cq + (e & 1) < kvalid) && (!diag || 8 * jj + cq + (e & 1) <= r0 + 8 * h2);
           const float pe = ok ? ex2(fmaf(sc[4 * jj + e], p.scale_log2, -lse2[h2])) : 0.f;
-          pv[e] = pe;
-          ds[e] = pe * (dp[4 * jj + e] - dl[h2]) * p.scale;
+          if constexpr (DROPOUT) {
+            // dV takes keep o P (1/q applied at the end); dS = P (Z dP - D) / sqrt(d)
+            const bool kp = drop_keep(rnd, jj, e, p.drop_thr);
+            pv[e] = kp ? pe : 0.f;
+            ds[e] = pe * ((kp ? dp[4 * jj + e] * p.drop_scale : 0.f) - dl[h2]) * p.scale;
+          } else {
+            pv[e] = pe;
+            ds[e] = pe * (dp[4 * jj + e] - dl[h2]) * p.scale;
+          }
         }
         st_pair_sw(sP_u, r0, 8 * jj + cq, TILE_BYTES, pv[0], pv[1]);
         st_pair_sw(sP_u, r0 + 8, 8 * jj + cq, TILE_BYTES, pv[2], pv[3]);
@@ -446,7 +508,10 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
 #pragma unroll
         for (int jj = 0; jj < HD / 8; ++jj) {
           pk[(8 * jj + cq) >> 1] = pack2(dk[4 * jj + 2 * h2], dk[4 * jj + 2 * h2 + 1]);
-          pv[(8 * jj + cq) >> 1] = pack2(dv[4 * jj + 2 * h2], dv[4 * jj + 2 * h2 + 1]);
+          if constexpr (DROPOUT)
+            pv[(8 * jj + cq) >> 1] = pack2(dv[4 * jj + 2 * h2] * p.drop_scale, dv[4 * jj + 2 * h2 + 1] * p.drop_scale);
+          else
+            pv[(8 * jj + cq) >> 1] = pack2(dv[4 * jj + 2 * h2], dv[4 * jj + 2 * h2 + 1]);
         }
       }
     }
@@ -463,6 +528,37 @@ int make_qkv_map(CUtensorMap* m, const void* ptr, int B, int H, int S, long long
   return encode_map(m, ptr, 4, dims, strides, box);
 }
 
+// causal / dropout arguments shared by the forward and the backward; fills the dropout fields of the params
+template <typename Params>
+int check_mode(int causal, const unsigned long long* seed, float drop_p, Params& p) {
+  if (causal != 0 && causal != 1) return fail("causal must be 0 or 1");
+  if (!(drop_p >= 0.f && drop_p <= 1.f)) return fail("attention dropout p must be in [0, 1]");
+  if (drop_p > 0.f && seed == nullptr) return fail("attention dropout needs a seed");
+  p.seed = seed;
+  p.drop_thr = dropout_thr16(drop_p);
+  p.drop_scale = dropout_scale16(p.drop_thr);
+  return 0;
+}
+
+template <bool CAUSAL, bool DROPOUT, typename... Args>
+int launch_fwd(dim3 grid, cudaStream_t st, Args... args) {
+  if (smem_attr_once<attn_fwd_kernel<CAUSAL, DROPOUT>>(FW_SMEM)) return -1;
+  attn_fwd_kernel<CAUSAL, DROPOUT><<<grid, AT, FW_SMEM, st>>>(args...);
+  return 0;
+}
+template <bool CAUSAL, bool DROPOUT, typename... Args>
+int launch_bwd(dim3 grid, cudaStream_t st, Args... args) {
+  if (smem_attr_once<attn_bwd_kernel<CAUSAL, DROPOUT>>(BW_SMEM)) return -1;
+  attn_bwd_kernel<CAUSAL, DROPOUT><<<grid, AT, BW_SMEM, st>>>(args...);
+  return 0;
+}
+
+int launched() {
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(cudaGetErrorString(e), (int)e);
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -470,20 +566,23 @@ extern "C" {
 const char* b200dp_attn_last_error() { return g_err; }
 
 // strides: element strides {batch, head, seq} of each tensor (head dim 64 contiguous).  causal: 0 or 1 (query i
-// sees keys 0..i; q, k and v share one sequence length S, so the mask always applies).
-int b200dp_attn_fwd_ex(const void* q, const void* k, const void* v, void* o, float* lse, int B, int H, int S, int D,
-                       const long long* qs, const long long* ks, const long long* vs, const long long* os, float scale,
-                       int causal, unsigned long long stream) {
+// sees keys 0..i; q, k and v share one sequence length S, so the mask always applies).  drop_p: attention
+// dropout probability in [0, 1]; 0 runs the kernels without dropout, otherwise `seed` is 2 words in device
+// memory (Philox key, offset: see the header for the mask).
+int b200dp_attn_fwd_dropout(const void* q, const void* k, const void* v, void* o, float* lse, int B, int H, int S,
+                            int D, const long long* qs, const long long* ks, const long long* vs, const long long* os,
+                            float scale, int causal, const unsigned long long* seed, float drop_p,
+                            unsigned long long stream) {
   if (ensure_init()) return -1;
   if (D != HD) return fail("head dim must be 64");
-  if (causal != 0 && causal != 1) return fail("causal must be 0 or 1");
+  AttnFwdParams p;
+  if (check_mode(causal, seed, drop_p, p)) return -1;
   if (B < 1 || H < 1 || S < 1) return fail("attention shapes must be positive");
   CUtensorMap mq, mk, mv;
   if (make_qkv_map(&mq, q, B, H, S, qs[0], qs[1], qs[2]) || make_qkv_map(&mk, k, B, H, S, ks[0], ks[1], ks[2]) ||
       make_qkv_map(&mv, v, B, H, S, vs[0], vs[1], vs[2]))
     return -1;
   if ((os[0] % 8) || (os[1] % 8) || (os[2] % 8) || ((uintptr_t)o & 15)) return fail("output must be 16-byte aligned");
-  AttnFwdParams p;
   p.B = B; p.H = H; p.S = S;
   p.q_tiles = (S + TILE - 1) / TILE;
   p.kv_blocks = (S + TILE - 1) / TILE;
@@ -493,34 +592,36 @@ int b200dp_attn_fwd_ex(const void* q, const void* k, const void* v, void* o, flo
   p.lse = lse;
   const dim3 grid(B * H * p.q_tiles);
   cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
-  if (causal) {
-    if (smem_attr_once<attn_fwd_kernel<true>>(FW_SMEM)) return -1;
-    attn_fwd_kernel<true><<<grid, AT, FW_SMEM, st>>>(mq, mk, mv, p);
-  } else {
-    if (smem_attr_once<attn_fwd_kernel<false>>(FW_SMEM)) return -1;
-    attn_fwd_kernel<false><<<grid, AT, FW_SMEM, st>>>(mq, mk, mv, p);
-  }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(cudaGetErrorString(e), (int)e);
-  return 0;
+  const bool drop = drop_p > 0.f;
+  const int rc = causal ? (drop ? launch_fwd<true, true>(grid, st, mq, mk, mv, p) : launch_fwd<true, false>(grid, st, mq, mk, mv, p))
+                        : (drop ? launch_fwd<false, true>(grid, st, mq, mk, mv, p) : launch_fwd<false, false>(grid, st, mq, mk, mv, p));
+  return rc ? rc : launched();
 }
 
-// The non-causal forward under its original signature, which Python callers bind with fixed ctypes argtypes.
+// The forward without dropout under its earlier signatures, which Python callers bind with fixed ctypes argtypes.
+int b200dp_attn_fwd_ex(const void* q, const void* k, const void* v, void* o, float* lse, int B, int H, int S, int D,
+                       const long long* qs, const long long* ks, const long long* vs, const long long* os, float scale,
+                       int causal, unsigned long long stream) {
+  return b200dp_attn_fwd_dropout(q, k, v, o, lse, B, H, S, D, qs, ks, vs, os, scale, causal, nullptr, 0.f, stream);
+}
 int b200dp_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int B, int H, int S, int D,
                     const long long* qs, const long long* ks, const long long* vs, const long long* os, float scale,
                     unsigned long long stream) {
-  return b200dp_attn_fwd_ex(q, k, v, o, lse, B, H, S, D, qs, ks, vs, os, scale, 0, stream);
+  return b200dp_attn_fwd_dropout(q, k, v, o, lse, B, H, S, D, qs, ks, vs, os, scale, 0, nullptr, 0.f, stream);
 }
 
-// dq_acc: fp32 workspace (strides dqs, 64 contiguous) zeroed by the caller; delta: [B][H][S] fp32 workspace
-int b200dp_attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* dout, const float* lse,
-                    float* delta, float* dq_acc, void* dk, void* dv, int B, int H, int S, int D, const long long* qs,
-                    const long long* ks, const long long* vs, const long long* os, const long long* dos,
-                    const long long* dqs, const long long* dks, const long long* dvs, float scale, int causal,
-                    unsigned long long stream) {
+// dq_acc: fp32 workspace (strides dqs, 64 contiguous) zeroed by the caller; delta: [B][H][S] fp32 workspace.
+// o is the (dropped) forward output; causal, seed and drop_p as given to the forward.
+int b200dp_attn_bwd_dropout(const void* q, const void* k, const void* v, const void* o, const void* dout,
+                            const float* lse, float* delta, float* dq_acc, void* dk, void* dv, int B, int H, int S,
+                            int D, const long long* qs, const long long* ks, const long long* vs, const long long* os,
+                            const long long* dos, const long long* dqs, const long long* dks, const long long* dvs,
+                            float scale, int causal, const unsigned long long* seed, float drop_p,
+                            unsigned long long stream) {
   if (ensure_init()) return -1;
   if (D != HD) return fail("head dim must be 64");
-  if (causal != 0 && causal != 1) return fail("causal must be 0 or 1");
+  AttnBwdParams p;
+  if (check_mode(causal, seed, drop_p, p)) return -1;
   if (B < 1 || H < 1 || S < 1) return fail("attention shapes must be positive");
   cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
   CUtensorMap mq, mk, mv, mdo;
@@ -531,7 +632,6 @@ int b200dp_attn_bwd(const void* q, const void* k, const void* v, const void* o, 
   attn_delta_kernel<<<(unsigned)((rows + 31) / 32), 256, 0, st>>>(
       reinterpret_cast<const __nv_bfloat16*>(o), reinterpret_cast<const __nv_bfloat16*>(dout), delta, B, H, S, os[0],
       os[1], os[2], dos[0], dos[1], dos[2]);
-  AttnBwdParams p;
   p.B = B; p.H = H; p.S = S;
   p.q_tiles = (S + TILE - 1) / TILE;
   p.kv_blocks = (S + TILE - 1) / TILE;
@@ -544,16 +644,22 @@ int b200dp_attn_bwd(const void* q, const void* k, const void* v, const void* o, 
   p.dk_sb = dks[0]; p.dk_sh = dks[1]; p.dk_ss = dks[2];
   p.dv_sb = dvs[0]; p.dv_sh = dvs[1]; p.dv_ss = dvs[2];
   const dim3 grid(B * H * p.kv_blocks);
-  if (causal) {
-    if (smem_attr_once<attn_bwd_kernel<true>>(BW_SMEM)) return -1;
-    attn_bwd_kernel<true><<<grid, AT, BW_SMEM, st>>>(mq, mk, mv, mdo, p);
-  } else {
-    if (smem_attr_once<attn_bwd_kernel<false>>(BW_SMEM)) return -1;
-    attn_bwd_kernel<false><<<grid, AT, BW_SMEM, st>>>(mq, mk, mv, mdo, p);
-  }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(cudaGetErrorString(e), (int)e);
-  return 0;
+  const bool drop = drop_p > 0.f;
+  const int rc = causal ? (drop ? launch_bwd<true, true>(grid, st, mq, mk, mv, mdo, p)
+                                : launch_bwd<true, false>(grid, st, mq, mk, mv, mdo, p))
+                        : (drop ? launch_bwd<false, true>(grid, st, mq, mk, mv, mdo, p)
+                                : launch_bwd<false, false>(grid, st, mq, mk, mv, mdo, p));
+  return rc ? rc : launched();
+}
+
+// The backward without dropout under its earlier signature.
+int b200dp_attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* dout, const float* lse,
+                    float* delta, float* dq_acc, void* dk, void* dv, int B, int H, int S, int D, const long long* qs,
+                    const long long* ks, const long long* vs, const long long* os, const long long* dos,
+                    const long long* dqs, const long long* dks, const long long* dvs, float scale, int causal,
+                    unsigned long long stream) {
+  return b200dp_attn_bwd_dropout(q, k, v, o, dout, lse, delta, dq_acc, dk, dv, B, H, S, D, qs, ks, vs, os, dos, dqs,
+                                 dks, dvs, scale, causal, nullptr, 0.f, stream);
 }
 
 }  // extern "C"

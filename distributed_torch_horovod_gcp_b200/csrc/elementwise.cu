@@ -14,6 +14,8 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include "philox.cuh"
+
 namespace {
 
 constexpr int THREADS = 256;
@@ -748,6 +750,39 @@ __global__ void cast_acc_zero_kernel(float* __restrict__ src, void* __restrict__
   }
 }
 
+// Dropout + residual add (bf16, memory-bound, one 16-byte vector of 8 elements per thread and step):
+//   out = residual + keep * y * (2^16 / t)      (residual == nullptr: plain dropout)
+// each product is rounded to fp32 and then added in fp32 (no fma), then rounded to bf16 once.  The keep bit of
+// element e is a pure function of the seed and e (philox.cuh for t and its resolution):
+//   u    = Philox4x32-10(key = (seed[0] mod 2^32, seed[0] / 2^32),
+//                        counter = ((e / 8) mod 2^32, (e / 8) / 2^32, seed[1] mod 2^32, seed[1] / 2^32))
+//   bits = (e mod 2) ? u[(e mod 8) / 2] >> 16 : u[(e mod 8) / 2] mod 2^16,   keep = bits < t
+// so one Philox call serves exactly one vector.  The backward is the same kernel on dout without a residual
+// (dy = keep * dout * 2^16 / t): the bits are drawn again from the seed rather than saved.
+__global__ void __launch_bounds__(THREADS) dropout_add_kernel(const uint4* __restrict__ y,
+                                                              const uint4* __restrict__ res, uint4* __restrict__ out,
+                                                              long long nvec, const unsigned long long* __restrict__ seed,
+                                                              uint32_t thr, float scale) {
+  const unsigned long long k = seed[0], off = seed[1];
+  const uint2 key = make_uint2((uint32_t)k, (uint32_t)(k >> 32));
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nvec; i += stride) {
+    const uint4 u = philox4x32_10(make_uint4((uint32_t)i, (uint32_t)((unsigned long long)i >> 32), (uint32_t)off,
+                                             (uint32_t)(off >> 32)), key);
+    const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+    float f[8], r[8];
+    unpack8(ldg_stream(y + i), f);
+    if (res != nullptr) unpack8(ldg_stream(res + i), r);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const uint32_t bits = (j & 1) ? w[j >> 1] >> 16 : w[j >> 1] & 0xffffu;
+      const float d = bits < thr ? __fmul_rn(f[j], scale) : 0.f;
+      f[j] = res != nullptr ? __fadd_rn(r[j], d) : d;
+    }
+    out[i] = pack8(f);
+  }
+}
+
 bool shape_ok(int C) {
   const int V = C / 8;
   return C % 8 == 0 && V >= 1 && V <= THREADS && (THREADS % V) == 0;   // V | 256 | 1024
@@ -775,6 +810,30 @@ int b200dp_cast_acc_zero(void* src, void* dst, long long n, int out_bf16, int ac
   else cast_acc_zero_kernel<false><<<grid, 256, 0, st>>>((float*)src, dst, n4, accumulate, zero_src);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail("cast_acc_zero launch", e);
+  return 0;
+}
+
+// out[n] = res[n] + dropout(y[n], p) for bf16 tensors (res == nullptr: out = dropout(y, p)); n % 8 == 0, all
+// three 16-byte aligned; 0 < p <= 1; seed: 2 words in device memory (Philox key, offset).  out may alias res.
+int b200dp_dropout_add(const void* y, const void* res, void* out, long long n, const unsigned long long* seed,
+                       float p, unsigned long long stream) {
+  if (n < 0 || n % 8 || ((uintptr_t)y & 15) || ((uintptr_t)res & 15) || ((uintptr_t)out & 15)) {
+    snprintf(g_err, sizeof(g_err), "dropout_add: n must be a multiple of 8 and every tensor 16-byte aligned");
+    return -1;
+  }
+  if (!(p > 0.f && p <= 1.f) || seed == nullptr) {
+    snprintf(g_err, sizeof(g_err), "dropout_add: needs 0 < p <= 1 and a seed");
+    return -1;
+  }
+  if (n == 0) return 0;
+  const uint32_t thr = dropout_thr16(p);
+  cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
+  long long grid = (n / 8 + THREADS - 1) / THREADS;
+  if (grid > reduce_grid() * 8) grid = reduce_grid() * 8;
+  dropout_add_kernel<<<(unsigned)grid, THREADS, 0, st>>>((const uint4*)y, (const uint4*)res, (uint4*)out, n / 8,
+                                                             seed, thr, dropout_scale16(thr));
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail("dropout_add launch", e);
   return 0;
 }
 

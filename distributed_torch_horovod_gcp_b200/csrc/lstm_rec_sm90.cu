@@ -724,20 +724,8 @@ struct InMmaArgs {
 // inter-layer dropout mask: keep[w] bit i = (element 32 w + i of the layer's output is kept), drawn with
 // Philox4x32-10 (Salmon et al., SC'11): key = seed[0], counter = (e / 4, seed[1]), output word e % 4,
 // kept when it is below `thr` = (1 - p) 2^32.  The seed lives in device memory (drawn by torch's CUDA
-// generator), so a replayed CUDA graph draws a fresh mask.
+// generator), so a replayed CUDA graph draws a fresh mask.  philox4x32_10 is in philox.cuh.
 // ---------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint4 philox4x32_10(uint4 ctr, uint2 key) {
-#pragma unroll
-  for (int r = 0; r < 10; ++r) {
-    const uint32_t lo0 = 0xD2511F53u * ctr.x, hi0 = __umulhi(0xD2511F53u, ctr.x);
-    const uint32_t lo1 = 0xCD9E8D57u * ctr.z, hi1 = __umulhi(0xCD9E8D57u, ctr.z);
-    ctr = make_uint4(hi1 ^ ctr.y ^ key.x, lo1, hi0 ^ ctr.w ^ key.y, lo0);
-    key.x += 0x9E3779B9u;
-    key.y += 0xBB67AE85u;
-  }
-  return ctr;
-}
-
 __global__ void __launch_bounds__(256) lstm_dropout_mask_kernel(uint32_t* __restrict__ keep,
                                                                 const unsigned long long* __restrict__ seed,
                                                                 size_t words, uint32_t thr) {

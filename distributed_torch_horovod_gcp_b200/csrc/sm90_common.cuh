@@ -16,6 +16,8 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include "philox.cuh"
+
 namespace {
 
 constexpr int BLOCK_M = 128;

@@ -6,6 +6,10 @@ attention runs on the causal flash-attention kernel, and LayerNorm eps 1e-5), a 
 head tied to the token embedding (``F2.linear(x, wte.weight)``, no bias).  Initialisation follows GPT-2:
 N(0, 0.02) everywhere, with the residual projections (``proj``, ``fc2``) at 0.02 / sqrt(2 * depth).
 
+``dropout`` (GPT-2 uses 0.1; default 0) is GPT-2's ``embd_pdrop``, ``attn_pdrop`` and ``resid_pdrop`` in one
+value, as nanoGPT's ``dropout``: in training mode it drops the embedding sum, the attention probabilities and
+the output of each residual branch.  Nothing is dropped inside the fused MLP node.
+
 The MLP is the fused node's exact (erf) GELU, not GPT-2's tanh approximation, so weights trained by the
 original GPT-2 code would see a slightly different activation here.
 """
@@ -22,12 +26,16 @@ from .vit import EncoderBlock
 
 class GPT(nn.Module):
     def __init__(self, vocab: int = 50304, context: int = 1024, depth: int = 12, heads: int = 12,
-                 dim: int = 768, mlp_dim: int = 3072):
+                 dim: int = 768, mlp_dim: int = 3072, dropout: float = 0.0):
         super().__init__()
+        if not 0.0 <= dropout <= 1.0:
+            raise ValueError(f"dropout must be in [0, 1], got {dropout}")
         self.vocab, self.context, self.dim = vocab, context, dim
+        self.dropout = float(dropout)
         self.wte = nn.Embedding(vocab, dim)
         self.wpe = nn.Embedding(context, dim)
-        self.layers = nn.ModuleList([EncoderBlock(dim, heads, mlp_dim, causal=True, eps=1e-5)
+        self.layers = nn.ModuleList([EncoderBlock(dim, heads, mlp_dim, causal=True, eps=1e-5, dropout=dropout,
+                                                  attention_dropout=dropout)
                                      for _ in range(depth)])
         self.ln_f = nn.LayerNorm(dim, eps=1e-5)
         for m in self.modules():
@@ -51,6 +59,8 @@ class GPT(nn.Module):
         # rather than written straight into the gradient bucket by the LM head's GEMM
         grad_sink.note_forward(self.wte.weight)
         x = self.wte(idx) + self.wpe.weight[:S]
+        if self.training and self.dropout > 0.0:
+            x = F2.dropout_add(x, None, self.dropout)
         for blk in self.layers:
             x = blk(x)
         x = F2.layer_norm(x, self.ln_f.weight, self.ln_f.bias, self.ln_f.eps)

@@ -12,7 +12,9 @@ from . import conv as _conv
 from . import lstm_rec as _lstm_rec
 from . import attention as _attn
 from . import xent as _xent
+from . import dropout as _dropout
 from .attention import attention_fused  # noqa: F401
+from .dropout import dropout_add  # noqa: F401
 from .xent import linear_cross_entropy  # noqa: F401
 from .lstm_rec import lstm_recurrent  # noqa: F401
 from .conv import conv3x3, conv2d as conv2d_implicit  # noqa: F401
@@ -30,6 +32,7 @@ def register(lib, have: Dict[str, bool]) -> None:
     _lstm_rec.register(lib, have)
     _attn.register(lib, have)
     _xent.register(lib, have)
+    _dropout.register(lib, have)
 
 
 def linear_supported(x, weight) -> bool:
@@ -42,3 +45,7 @@ def layer_norm_supported(x, weight, bias) -> bool:
 
 def linear_cross_entropy_supported(x, weight, targets) -> bool:
     return _xent.supported(x, weight, targets)
+
+
+def dropout_add_supported(y, residual) -> bool:
+    return _dropout.supported(y, residual)

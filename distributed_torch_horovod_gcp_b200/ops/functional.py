@@ -4,8 +4,9 @@ Each function is ONE fusable unit.  ``*_reference`` are plain PyTorch compositio
 path and the fp32 numerics oracle for the kernels' tests; the CUDA fast paths are the
 hand-written sm_90a kernels bound in ``ops.kernels``: wgmma GEMM with fused epilogues
 (ops/gemm.py), implicit-GEMM convolution (ops/conv.py), fused BN/ReLU/residual and max-pool
-(ops/bn.py), LayerNorm (ops/ln.py), flash attention forward/backward (ops/attention.py), the LM head
-fused with its cross-entropy loss (ops/xent.py).
+(ops/bn.py), LayerNorm (ops/ln.py), flash attention forward/backward with optional dropout
+(ops/attention.py), the LM head fused with its cross-entropy loss (ops/xent.py), dropout fused with the
+residual add (ops/dropout.py).
 """
 from __future__ import annotations
 
@@ -103,6 +104,33 @@ def mlp(x, w1, b1, w2, b2, residual=None):
     return linear_reference(linear_reference(x, w1, b1, act="gelu"), w2, b2, residual=residual)
 
 
+# ------------------------------------------------------------------ dropout (+ residual)
+def _check_p(p) -> float:
+    p = float(p)
+    if not 0.0 <= p <= 1.0:
+        raise ValueError(f"dropout probability must be in [0, 1], got {p}")
+    return p
+
+
+def dropout_add_reference(y, residual, p: float):
+    y = F.dropout(y, p)
+    return y if residual is None else residual + y
+
+
+def dropout_add(y, residual, p: float):
+    """``residual + F.dropout(y, p)`` (training-mode dropout; ``residual=None``: ``F.dropout(y, p)``).  Kernel
+    path (contiguous bf16 ``y`` and ``residual`` of one shape, numel % 8 == 0): one pass that draws the keep
+    mask, scales and adds (ops/dropout.py); its backward draws the same mask again from the saved seed.
+    ``p == 0`` adds ``y`` as it is.  Anything else takes the composition above."""
+    p = _check_p(p)
+    if p == 0.0:
+        return y if residual is None else residual + y
+    k = _kernels(y)
+    if k is not None and k.has("dropout_add") and k.dropout_add_supported(y, residual):
+        return k.dropout_add(y, residual, p)
+    return dropout_add_reference(y, residual, p)
+
+
 # ------------------------------------------------------------------ layer norm
 def layer_norm(x, weight, bias, eps: float = 1e-6):
     k = _kernels(x)
@@ -112,28 +140,32 @@ def layer_norm(x, weight, bias, eps: float = 1e-6):
 
 
 # ------------------------------------------------------------------ attention
-def attention_reference(qkv, heads: int, causal: bool = False):
+def attention_reference(qkv, heads: int, causal: bool = False, dropout_p: float = 0.0):
     """Self-attention of a packed ``[B, S, 3 D]`` q|k|v tensor; ``causal=True``: position i attends to
-    positions 0..i only."""
+    positions 0..i only; ``dropout_p``: dropout on the attention probabilities."""
+    dropout_p = _check_p(dropout_p)
     B, S, D3 = qkv.shape
     D = D3 // 3
     hd = D // heads
     q, k, v = qkv.view(B, S, 3, heads, hd).permute(2, 0, 3, 1, 4)
-    o = F.scaled_dot_product_attention(q, k, v, is_causal=causal)
+    o = F.scaled_dot_product_attention(q, k, v, dropout_p=dropout_p, is_causal=causal)
     return o.transpose(1, 2).reshape(B, S, D)
 
 
-def attention(qkv, heads: int, causal: bool = False):
+def attention(qkv, heads: int, causal: bool = False, dropout_p: float = 0.0):
+    dropout_p = _check_p(dropout_p)
     k = _kernels(qkv)
     if k is not None and k.has("attention"):
-        return k.attention(qkv, heads, causal)
-    return attention_reference(qkv, heads, causal)
+        return k.attention(qkv, heads, causal, dropout_p)
+    return attention_reference(qkv, heads, causal, dropout_p)
 
 
-def qkv_attention(x, weight, bias, heads: int, causal: bool = False):
+def qkv_attention(x, weight, bias, heads: int, causal: bool = False, dropout_p: float = 0.0):
     """Multi-head self-attention input stage: packed QKV projection + scaled-dot-product attention
-    (``causal=True``: position i attends to positions 0..i only, as in a decoder).
+    (``causal=True``: position i attends to positions 0..i only, as in a decoder; ``dropout_p``: dropout on
+    the attention probabilities, drawn inside the flash-attention kernels on the kernel path).
     Kernel path: q, k, v are produced as three dense matrices (no un-pack / re-pack copies)."""
+    dropout_p = _check_p(dropout_p)
     k = _kernels(x)
     if k is not None and k.has("linear") and k.linear_supported(x, weight) and weight.shape[0] % 24 == 0 \
             and os.environ.get("B200DP_SPLIT_QKV", "1") == "1":
@@ -144,11 +176,11 @@ def qkv_attention(x, weight, bias, heads: int, causal: bool = False):
         if k.has("attention_fused") and hd == 64 and os.environ.get("B200DP_ATTN_KERNEL", "1") == "1":
             from . import attention as _attn
             if _attn.supported(q, kk, v):
-                o = _attn.attention_fused(q, kk, v, causal)   # [B,H,S,hd] view of [B,S,H,hd] memory
+                o = _attn.attention_fused(q, kk, v, causal, dropout_p)   # [B,H,S,hd] view of [B,S,H,hd] memory
                 return o.transpose(1, 2).reshape(B, S, D)  # a view: no copy
-        o = F.scaled_dot_product_attention(q, kk, v, is_causal=causal)
+        o = F.scaled_dot_product_attention(q, kk, v, dropout_p=dropout_p, is_causal=causal)
         return o.transpose(1, 2).reshape(B, S, D)
-    return attention(linear(x, weight, bias), heads, causal)
+    return attention(linear(x, weight, bias), heads, causal, dropout_p)
 
 
 # ------------------------------------------------------------------ LM head + cross-entropy
