@@ -152,7 +152,7 @@ class _LinearFn(torch.autograd.Function):
             x2 = x2.contiguous()
         M = x2.shape[0]
         y = torch.empty((M, N), dtype=torch.bfloat16, device=x.device)
-        need_z = act != 0 and (x.requires_grad or weight.requires_grad)
+        need_z = act != 0 and any(ctx.needs_input_grad[0:3])      # dz feeds dx, dW and db; not dres
         z = torch.empty_like(y) if need_z else None
         r2 = None
         if residual is not None:
@@ -175,7 +175,7 @@ class _LinearFn(torch.autograd.Function):
         if not dy2.is_contiguous():
             dy2 = dy2.contiguous()
         dres = dy2.view(*ctx.x_shape[:-1], N) if ctx.has_res else None
-        if ctx.act != 0:
+        if ctx.act != 0 and any(ctx.needs_input_grad[0:3]):
             dz = act_backward(dy2, z, ctx.act)
         else:
             dz = dy2
