@@ -1012,18 +1012,32 @@ int b200dp_comm_limits(int* max_ranks, int* max_blocks, int* channels, int* ctx_
 
 // The launch checks of every entry point.  The grid must fit the per-block barrier counters and slots
 // (1..B200DP_MAX_BLOCKS CTAs) and be whole warps of at most 512 threads (the block sums and __launch_bounds__);
-// the world and the channel must fit the signal pad; `sel` (algorithm, phase or collective mode) must be below
-// `nsel` and the dtype code known.  Sets the error message and returns false otherwise.
+// the world and the channel must fit the signal pad, and the rank must lie in the world (it indexes `sig[]`);
+// `sel` (algorithm, phase or collective mode) must be below `nsel` and the dtype code known.  Sets the error
+// message and returns false otherwise.
 static bool launch_ok(const char* what, const CommCtx* ctx, int channel, const char* sel_name, int sel, int nsel,
                       int dtype, int blocks, int threads) {
   if (blocks >= 1 && blocks <= B200DP_MAX_BLOCKS && threads >= 32 && threads <= 512 && (threads & 31) == 0 &&
-      ctx->world <= B200DP_MAX_RANKS && channel >= 0 && channel < B200DP_NUM_CHANNELS && sel >= 0 && sel < nsel &&
-      dtype >= 0 && dtype <= 2)
+      ctx->world >= 1 && ctx->world <= B200DP_MAX_RANKS && ctx->rank >= 0 && ctx->rank < ctx->world &&
+      channel >= 0 && channel < B200DP_NUM_CHANNELS && sel >= 0 && sel < nsel && dtype >= 0 && dtype <= 2)
     return true;
-  snprintf(g_comm_err, sizeof(g_comm_err), "bad %s launch: blocks=%d threads=%d world=%d channel=%d %s=%d dtype=%d",
-           what, blocks, threads, ctx->world, channel, sel_name, sel, dtype);
+  snprintf(g_comm_err, sizeof(g_comm_err),
+           "bad %s launch: blocks=%d threads=%d rank=%d world=%d channel=%d %s=%d dtype=%d", what, blocks, threads,
+           ctx->rank, ctx->world, channel, sel_name, sel, dtype);
   return false;
 }
+
+// The kernels walk whole 16-byte vectors (`size / unit`) and would silently drop a tail: a size that is not a
+// multiple of `unit` is refused.  Sets the error message and returns false then.
+static bool size_ok(const char* what, const char* size_name, unsigned long long size, unsigned long long unit) {
+  if (size % unit == 0) return true;
+  snprintf(g_comm_err, sizeof(g_comm_err), "bad %s launch: %s=%llu is not a multiple of %llu", what, size_name,
+           size, unit);
+  return false;
+}
+
+// Elements of a dtype code per 16-byte vector.
+static unsigned long long vec_elems(int dtype) { return dtype == 0 ? 4 : 8; }
 
 // 0, or -1 with the launch error in b200dp_comm_last_error().
 static int launched(const char* what, cudaError_t e) {
@@ -1038,7 +1052,9 @@ int b200dp_comm_clip_bytes() { return (int)sizeof(ClipArgs); }
 // b200dp_comm_allreduce: the dtype of the gradient bucket on the wire and of the parameter output.
 int b200dp_comm_clip_bucket(const CommCtx* ctx, const ARArgs* args, const ClipArgs* clip, int phase, int dtype,
                             int blocks, int threads, unsigned long long stream) {
-  if (!launch_ok("clip", ctx, args->channel, "phase", phase, 2, dtype, blocks, threads)) return -1;
+  if (!launch_ok("clip", ctx, args->channel, "phase", phase, 2, dtype, blocks, threads) ||
+      !size_ok("clip", "n", args->n, vec_elems(dtype)))
+    return -1;
   cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
   return launched("clip", with_dtype(dtype, [&](auto tag) {
     using T = typename decltype(tag)::type;
@@ -1076,7 +1092,9 @@ int b200dp_comm_lw_bucket(const CommCtx* ctx, const ARArgs* args, const LwArgs* 
 // algo: 0 one-shot, 1 two-shot, 2 NVLS.  dtype: 0 fp32, 1 bf16, 2 fp16.
 int b200dp_comm_allreduce(const CommCtx* ctx, const ARArgs* args, int algo, int dtype, int blocks,
                           int threads, unsigned long long stream) {
-  if (!launch_ok("allreduce", ctx, args->channel, "algo", algo, 3, dtype, blocks, threads)) return -1;
+  if (!launch_ok("allreduce", ctx, args->channel, "algo", algo, 3, dtype, blocks, threads) ||
+      !size_ok("allreduce", "n", args->n, vec_elems(dtype)))
+    return -1;
   cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
   return launched("allreduce", with_dtype(dtype, [&](auto tag) {
     using T = typename decltype(tag)::type;
@@ -1090,7 +1108,9 @@ int b200dp_comm_allreduce(const CommCtx* ctx, const ARArgs* args, int algo, int 
 // mode: 0 reduce-scatter, 1 all-gather, 2 all-to-all.  dtype as in b200dp_comm_allreduce (reduce-scatter only).
 int b200dp_comm_collective(const CommCtx* ctx, const CollArgs* args, int mode, int dtype, int blocks, int threads,
                            unsigned long long stream) {
-  if (!launch_ok("collective", ctx, args->channel, "mode", mode, 3, dtype, blocks, threads)) return -1;
+  if (!launch_ok("collective", ctx, args->channel, "mode", mode, 3, dtype, blocks, threads) ||
+      (mode == 0 && !size_ok("collective", "chunk", args->chunk, vec_elems(dtype))))
+    return -1;
   cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
   if (mode == 1) {
     allgather_kernel<<<blocks, threads, 0, st>>>(*ctx, *args);
@@ -1111,7 +1131,9 @@ int b200dp_comm_coll_bytes() { return (int)sizeof(CollArgs); }
 
 int b200dp_comm_broadcast(const CommCtx* ctx, const BcastArgs* args, int blocks, int threads,
                           unsigned long long stream) {
-  if (!launch_ok("broadcast", ctx, args->channel, "-", 0, 1, 0, blocks, threads)) return -1;
+  if (!launch_ok("broadcast", ctx, args->channel, "-", 0, 1, 0, blocks, threads) ||
+      !size_ok("broadcast", "nbytes", args->nbytes, 16))
+    return -1;
   broadcast_kernel<<<blocks, threads, 0, (cudaStream_t)(uintptr_t)stream>>>(*ctx, *args);
   return launched("broadcast", cudaGetLastError());
 }

@@ -21,27 +21,29 @@ def comm():
     return lib, S
 
 
-GOOD = dict(blocks=4, threads=512, world=1, channel=1, sel=0, dtype=0)
+# size: ARArgs.n (all-reduce, clip), CollArgs.chunk (collectives, elements for reduce-scatter) or BcastArgs.nbytes
+GOOD = dict(blocks=4, threads=512, rank=0, world=1, channel=1, sel=0, dtype=0, size=64)
 BAD = [
     ("blocks", 0), ("blocks", 129),
     ("threads", 31), ("threads", 48), ("threads", 513),
-    ("world", 9), ("channel", 4), ("channel", -1),
+    ("world", 9), ("world", 0), ("rank", -1), ("rank", 1), ("channel", 4), ("channel", -1),
     ("sel", 3), ("sel", -1), ("dtype", 3), ("dtype", -1),
+    ("size", 6),      # not whole fp32 vectors (4 elements) nor whole 16-byte broadcast vectors
 ]
 
 
 def _call(lib, S, entry, cfg):
     """Launch ``entry`` with the configuration ``cfg`` (``sel``: algo, phase or collective mode)."""
     ctx = S.CommCtx()
-    ctx.world = cfg["world"]
+    ctx.rank, ctx.world = cfg["rank"], cfg["world"]
     b = ctypes.byref
     if entry == "allreduce":
         a = S.ARArgs()
-        a.channel = cfg["channel"]
+        a.channel, a.n = cfg["channel"], cfg["size"]
         return lib.b200dp_comm_allreduce(b(ctx), b(a), cfg["sel"], cfg["dtype"], cfg["blocks"], cfg["threads"], 0)
     if entry == "clip_bucket":
         a, k = S.ARArgs(), S.ClipArgs()
-        a.channel = cfg["channel"]
+        a.channel, a.n = cfg["channel"], cfg["size"]
         return lib.b200dp_comm_clip_bucket(b(ctx), b(a), b(k), cfg["sel"], cfg["dtype"], cfg["blocks"],
                                            cfg["threads"], 0)
     if entry == "lw_bucket":
@@ -52,10 +54,10 @@ def _call(lib, S, entry, cfg):
                                          cfg["threads"], 0)
     if entry == "collective":
         a = S.CollArgs()
-        a.channel = cfg["channel"]
+        a.channel, a.chunk = cfg["channel"], cfg["size"]
         return lib.b200dp_comm_collective(b(ctx), b(a), cfg["sel"], cfg["dtype"], cfg["blocks"], cfg["threads"], 0)
     a = S.BcastArgs()
-    a.channel = cfg["channel"]
+    a.channel, a.nbytes = cfg["channel"], cfg["size"]
     return lib.b200dp_comm_broadcast(b(ctx), b(a), cfg["blocks"], cfg["threads"], 0)
 
 
@@ -69,6 +71,8 @@ def test_bad_launch_config_is_rejected(comm, entry, field, value):
     lib, S = comm
     if entry == "broadcast" and field in ("sel", "dtype"):
         pytest.skip("broadcast takes no selector or dtype")
+    if entry == "lw_bucket" and field == "size":
+        pytest.skip("the layer-wise kernels walk the chunk table, not n")
     if field == "sel" and value == 3:
         value = SEL_LIMIT[entry]
     cfg = dict(GOOD, **{field: value})
@@ -84,3 +88,15 @@ def test_layerwise_rejects_other_optimizers_and_negative_chunks(comm, kind, nchu
     assert _call(lib, S, "lw_bucket", cfg) == -1
     msg = lib.b200dp_comm_last_error().decode()
     assert msg.startswith("bad layer-wise launch") and f"kind={getattr(S, kind)}" in msg, msg
+
+
+@pytest.mark.parametrize("entry", ["allreduce", "clip_bucket", "collective"])
+@pytest.mark.parametrize("dtype", [1, 2])
+def test_sixteen_bit_sizes_must_be_whole_vectors(comm, entry, dtype):
+    """bf16 and fp16 vectors hold 8 elements: 12 elements (whole fp32 vectors) are refused, for reduce-scatter
+    too."""
+    lib, S = comm
+    cfg = dict(GOOD, dtype=dtype, size=12)
+    assert _call(lib, S, entry, cfg) == -1
+    msg = lib.b200dp_comm_last_error().decode()
+    assert msg.startswith("bad ") and "is not a multiple of 8" in msg, msg
