@@ -141,14 +141,18 @@ __device__ __forceinline__ void st_param(void* p, int c, int bf16, float v) {
 }
 
 // gamma/beta/running_* are the module's tensors in their own dtype (fp32 or bf16: `pbf16`).
+// DEV_COUNT (SyncBatchNorm): `count` is the row count summed over all ranks, read from `count_dev` on the device.
+// A template argument, so that the plain instantiation compiles to the same instructions (and bits) as without it.
+template <bool DEV_COUNT>
 __global__ void bn_finalize_kernel(float* sum, float* sumsq, const void* gamma,
                                    const void* beta, float* mean, float* invstd, float* a, float* b,
                                    void* running_mean, void* running_var, float count, float eps,
                                    float momentum, int C, int pbf16, int rezero = 0,
-                                   long long* num_batches_tracked = nullptr) {
+                                   long long* num_batches_tracked = nullptr, const float* count_dev = nullptr) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c == 0 && num_batches_tracked != nullptr) *num_batches_tracked += 1;   // nn.BatchNorm2d bookkeeping
   if (c >= C) return;
+  if constexpr (DEV_COUNT) count = *count_dev;
   const float m = sum[c] / count;
   const float var = fmaxf(sumsq[c] / count - m * m, 0.f);
   if (rezero) {      // persistent accumulators filled by the producing GEMM / conv epilogue: ready for the next step
@@ -267,12 +271,15 @@ __global__ void __launch_bounds__(RTHREADS, 1) bn_bwd_reduce_kernel(
 }
 
 // ---- backward apply: dx = a*(dz - sum_dy/M - xhat*sum_dy_xhat/M), dres = dz ------------------------
+// DEV_COUNT (SyncBatchNorm): 1/M from the global row count `count_dev` on the device instead of `inv_count`.  A
+// template argument, so that the plain instantiation compiles to the same instructions (and bits) as without it.
+template <bool DEV_COUNT>
 __global__ void __launch_bounds__(THREADS, 4) bn_bwd_apply_kernel(
     const uint4* __restrict__ dy, const uint4* __restrict__ x, const uint8_t* __restrict__ mask, uint4* dx,
     uint4* dres, const float* __restrict__ mean, const float* __restrict__ invstd,
     const float* __restrict__ scale_a, const float* __restrict__ sum_dy,
     const float* __restrict__ sum_dy_xhat, float inv_count, long long nvec, int V, int relu,
-    void* dgamma, void* dbeta, int pbf16) {
+    void* dgamma, void* dbeta, int pbf16, const float* __restrict__ count_dev = nullptr) {
   constexpr int U = 2;
   const long long stride = (long long)gridDim.x * THREADS;
   const long long i0 = (long long)blockIdx.x * THREADS + threadIdx.x;
@@ -283,6 +290,8 @@ __global__ void __launch_bounds__(THREADS, 4) bn_bwd_apply_kernel(
     }
   }
   if (i0 >= nvec) return;
+  // 1 / (global row count) in double rounded to fp32, as the host computes inv_count
+  if constexpr (DEV_COUNT) inv_count = (float)(1.0 / (double)*count_dev);
   const int cg = (int)(i0 % V);
   float mv[8], iv[8], k1[8], k2[8], sc[8];
 #pragma unroll
@@ -861,7 +870,7 @@ int b200dp_bn_fwd(const void* x, const void* res, void* y, const void* gamma, co
     if (e != cudaSuccess) return fail("memset", e);
     bn_stats_kernel<<<reduce_grid(), RTHREADS, 0, st>>>((const uint4*)x, stats, stats + C, nvec, V);
   }
-  bn_finalize_kernel<<<(C + 127) / 128, 128, 0, st>>>(stats, stats + C, gamma, beta, mean, invstd, a, b,
+  bn_finalize_kernel<false><<<(C + 127) / 128, 128, 0, st>>>(stats, stats + C, gamma, beta, mean, invstd, a, b,
                                                       running_mean, running_var, (float)M, eps, momentum, C,
                                                       param_bf16, have_stats == 2 ? 1 : 0,
                                                       (long long*)num_batches_tracked);
@@ -886,18 +895,19 @@ int b200dp_bn_stats(const void* x, float* stats, long long M, int C, unsigned lo
   return 0;
 }
 
-// finalize + apply with statistics that were summed over all ranks: `count` = global number of rows
+// finalize + apply with statistics that were summed over all ranks: `count` = the global number of rows, a
+// device fp32 (the all-reduced stats[2*C]), so ranks may hold different numbers of rows, none included
 int b200dp_bn_fwd_sync(const void* x, const void* res, void* y, const void* gamma, const void* beta,
                        const float* stats, float* mean, float* invstd, float* a, float* b, void* running_mean,
-                       void* running_var, long long M_local, double count, int C, float eps, float momentum,
+                       void* running_var, long long M_local, const float* count, int C, float eps, float momentum,
                        int relu, int param_bf16, void* relu_mask, unsigned long long stream) {
   if (!shape_ok(C)) return -1;
   cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
   const int V = C / 8;
   const long long nvec = M_local * V;
-  bn_finalize_kernel<<<(C + 127) / 128, 128, 0, st>>>(const_cast<float*>(stats), const_cast<float*>(stats) + C, gamma,
+  bn_finalize_kernel<true><<<(C + 127) / 128, 128, 0, st>>>(const_cast<float*>(stats), const_cast<float*>(stats) + C, gamma,
                                                       beta, mean, invstd, a, b, running_mean, running_var,
-                                                      (float)count, eps, momentum, C, param_bf16);
+                                                      0.f, eps, momentum, C, param_bf16, 0, nullptr, count);
   bn_apply_kernel<<<grid_for(nvec, V), THREADS, 0, st>>>((const uint4*)x, (const uint4*)res, (uint4*)y, a, b, nvec,
                                                          V, relu, (uint8_t*)relu_mask);
   cudaError_t e = cudaGetLastError();
@@ -920,16 +930,16 @@ int b200dp_bn_bwd_reduce(const void* dy, const void* x, const void* relu_mask, c
   return 0;
 }
 
-// backward, pass 2 with globally summed `sums` and the global row count
+// backward, pass 2 with globally summed `sums` and the global row count (device fp32, as in b200dp_bn_fwd_sync)
 int b200dp_bn_bwd_apply(const void* dy, const void* x, const void* relu_mask, void* dx, void* dres,
                         const float* scale_a, const float* mean, const float* invstd, const float* sums,
-                        double count, long long M, int C, int relu, unsigned long long stream) {
+                        const float* count, long long M, int C, int relu, unsigned long long stream) {
   if (!shape_ok(C)) return -1;
   const int V = C / 8;
   const long long nvec = M * V;
-  bn_bwd_apply_kernel<<<grid_for(nvec, V), THREADS, 0, (cudaStream_t)(uintptr_t)stream>>>(
+  bn_bwd_apply_kernel<true><<<grid_for(nvec, V), THREADS, 0, (cudaStream_t)(uintptr_t)stream>>>(
       (const uint4*)dy, (const uint4*)x, (const uint8_t*)relu_mask, (uint4*)dx, (uint4*)dres, mean, invstd, scale_a,
-      sums, sums + C, (float)(1.0 / count), nvec, V, relu, nullptr, nullptr, 0);
+      sums, sums + C, 0.f, nvec, V, relu, nullptr, nullptr, 0, count);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail("bn_bwd_apply launch", e);
   return 0;
@@ -963,7 +973,7 @@ int b200dp_bn_bwd(const void* dy, const void* x, const void* relu_mask, void* dx
   bn_bwd_reduce_kernel<<<reduce_grid(), RTHREADS, 0, st>>>((const uint4*)dy, (const uint4*)x,
                                                            (const uint8_t*)relu_mask, mean, sums, sums + C,
                                                            nvec, V, relu);
-  bn_bwd_apply_kernel<<<grid, THREADS, 0, st>>>((const uint4*)dy, (const uint4*)x, (const uint8_t*)relu_mask,
+  bn_bwd_apply_kernel<false><<<grid, THREADS, 0, st>>>((const uint4*)dy, (const uint4*)x, (const uint8_t*)relu_mask,
                                                 (uint4*)dx, (uint4*)dres, mean, invstd, scale_a, sums,
                                                 sums + C, 1.0f / (float)M, nvec, V, relu, dgamma, dbeta,
                                                 param_bf16);

@@ -35,11 +35,10 @@ def register(lib, have):
     lib.b200dp_bn_bwd.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i, ll, i, i, u64]
     lib.b200dp_bn_supported.argtypes = [i]
     if hasattr(lib, "b200dp_bn_fwd_sync"):
-        d = ctypes.c_double
         lib.b200dp_bn_stats.argtypes = [vp, vp, ll, i, u64]
-        lib.b200dp_bn_fwd_sync.argtypes = [vp] * 12 + [ll, d, i, f, f, i, i, vp, u64]
+        lib.b200dp_bn_fwd_sync.argtypes = [vp] * 12 + [ll, vp, i, f, f, i, i, vp, u64]
         lib.b200dp_bn_bwd_reduce.argtypes = [vp, vp, vp, vp, vp, ll, i, i, u64]
-        lib.b200dp_bn_bwd_apply.argtypes = [vp] * 9 + [d, ll, i, i, u64]
+        lib.b200dp_bn_bwd_apply.argtypes = [vp] * 10 + [ll, i, i, u64]
     lib.b200dp_ew_last_error.restype = ctypes.c_char_p
     have["bn_act"] = True
     have["conv_bn_act"] = True

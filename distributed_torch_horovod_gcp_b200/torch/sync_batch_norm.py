@@ -30,7 +30,7 @@ class _SyncBNFn(torch.autograd.Function):
         stats = torch.empty(2 * C + 1, dtype=torch.float32, device=x.device)
         stats[:C] = xf.sum(dims)
         stats[C:2 * C] = (xf * xf).sum(dims)
-        stats[2 * C] = float(n_local)
+        stats[2 * C:].fill_(float(n_local))        # a fill kernel: item assignment would copy from the host
         stats = mpi_ops.allreduce(stats, op=mpi_ops.Sum, name=None)
         n = stats[2 * C]
         mean = stats[:C] / n
@@ -87,9 +87,9 @@ class _SyncBNKernelFn(torch.autograd.Function):
         st = torch.cuda.current_stream(dev).cuda_stream
         stats = torch.empty(2 * C + 1, dtype=torch.float32, device=dev)
         B._ck(lib.b200dp_bn_stats(x.data_ptr(), stats.data_ptr(), M, C, st))
-        stats[2 * C] = float(M)
+        stats[2 * C:].fill_(float(M))           # a fill kernel: item assignment would copy from the host
         stats = mpi_ops.allreduce(stats, op=mpi_ops.Sum, name=None)
-        count = float(M) * _state.size()        # every rank contributes the same local shape in DP
+        count = stats[2 * C:]                   # global row count: ranks may hold different numbers of rows
         y = torch.empty_like(x, memory_format=torch.channels_last)
         ws = torch.empty(4 * C, dtype=torch.float32, device=dev)
         mean, invstd, a, b = ws[:C], ws[C:2 * C], ws[2 * C:3 * C], ws[3 * C:]
@@ -98,17 +98,17 @@ class _SyncBNKernelFn(torch.autograd.Function):
                                      b.data_ptr(),
                                      running_mean.data_ptr() if running_mean is not None else None,
                                      running_var.data_ptr() if running_var is not None else None,
-                                     M, count, C, float(eps), float(momentum), 0,
+                                     M, count.data_ptr(), C, float(eps), float(momentum), 0,
                                      int(weight.dtype == torch.bfloat16), None, st))
-        ctx.save_for_backward(x, mean, invstd, a)
-        ctx.count, ctx.pdtype = count, weight.dtype
+        ctx.save_for_backward(x, mean, invstd, a, count)
+        ctx.pdtype = weight.dtype
         return y
 
     @staticmethod
     def backward(ctx, dy):
         from ..ops import bn as B
         lib = B._lib
-        x, mean, invstd, a = ctx.saved_tensors
+        x, mean, invstd, a, count = ctx.saved_tensors
         N, C, H, W = x.shape
         M = N * H * W
         if not dy.is_contiguous(memory_format=torch.channels_last):
@@ -123,12 +123,17 @@ class _SyncBNKernelFn(torch.autograd.Function):
         g = mpi_ops.allreduce(sums, op=mpi_ops.Sum, name=None)
         dx = torch.empty_like(x, memory_format=torch.channels_last)
         B._ck(lib.b200dp_bn_bwd_apply(dy.data_ptr(), x.data_ptr(), None, dx.data_ptr(), None, a.data_ptr(),
-                                      mean.data_ptr(), invstd.data_ptr(), g.data_ptr(), ctx.count, M, C, 0, st))
+                                      mean.data_ptr(), invstd.data_ptr(), g.data_ptr(), count.data_ptr(), M, C, 0,
+                                      st))
         return dx, dgamma, dbeta, None, None, None, None
 
 
-def _kernel_path_ok(x, weight, bias) -> bool:
+def _kernel_path_ok(x, weight, bias, running_mean=None, running_var=None) -> bool:
     if not (x.is_cuda and x.dim() == 4 and x.dtype == torch.bfloat16 and weight is not None and bias is not None):
+        return False
+    # the kernels read (and write) every parameter in one dtype, chosen by `weight`
+    params = [t for t in (weight, bias, running_mean, running_var) if t is not None]
+    if weight.dtype not in (torch.bfloat16, torch.float32) or any(t.dtype != weight.dtype for t in params):
         return False
     try:
         from ..ops import kernels, bn as B
@@ -158,7 +163,7 @@ class SyncBatchNorm(_BatchNorm):
             return torch.nn.functional.batch_norm(
                 input, self.running_mean, self.running_var, self.weight, self.bias,
                 use_batch, momentum if momentum is not None else 0.0, self.eps)
-        if _kernel_path_ok(input, self.weight, self.bias):
+        if _kernel_path_ok(input, self.weight, self.bias, self.running_mean, self.running_var):
             return _SyncBNKernelFn.apply(input, self.weight, self.bias, self.running_mean,
                                          self.running_var, self.eps, momentum)
         return _SyncBNFn.apply(input, self.weight, self.bias, self.running_mean,

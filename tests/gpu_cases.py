@@ -313,23 +313,28 @@ def native_collectives_match_nccl(hvd):
 
 
 def sync_bn_kernel_path(hvd):
-    """SyncBatchNorm on NHWC bf16: fused BN kernels + one-shot allreduce == fp32 BN over the global batch."""
+    """SyncBatchNorm on NHWC bf16: fused BN kernels + one-shot allreduce == fp32 BN over the global batch.  Rank r
+    holds 4 + r images, so the global row count is not the local one times the world size."""
     s = _symm(hvd)
     r, n = hvd.rank(), hvd.size()
     dev = s.device
     from distributed_torch_horovod_gcp_b200.ops import counters, kernels
+    from distributed_torch_horovod_gcp_b200.torch import sync_batch_norm as sbn
     assert kernels.has("bn_act")
     torch.manual_seed(5)
     C = 64
-    full = torch.randn(n * 4, C, 8, 8, device=dev)
-    gfull = torch.randn(n * 4, C, 8, 8, device=dev)
+    lo, hi = sum(4 + q for q in range(r)), sum(4 + q for q in range(r + 1))
+    total = sum(4 + q for q in range(n))
+    full = torch.randn(total, C, 8, 8, device=dev)
+    gfull = torch.randn(total, C, 8, 8, device=dev)
     bn = hvd.SyncBatchNorm(C).to(dev).to(torch.bfloat16)
     with torch.no_grad():
         bn.weight.copy_(torch.rand(C) + 0.5)
         bn.bias.copy_(torch.randn(C) * 0.1)
-    x = full[r * 4:(r + 1) * 4].to(torch.bfloat16).contiguous(memory_format=torch.channels_last).requires_grad_(True)
+    x = full[lo:hi].to(torch.bfloat16).contiguous(memory_format=torch.channels_last).requires_grad_(True)
+    assert sbn._kernel_path_ok(x, bn.weight, bn.bias, bn.running_mean, bn.running_var)
     y = bn(x)
-    y.backward(gfull[r * 4:(r + 1) * 4].to(torch.bfloat16).contiguous(memory_format=torch.channels_last))
+    y.backward(gfull[lo:hi].to(torch.bfloat16).contiguous(memory_format=torch.channels_last))
     # oracle: plain BN in fp32 over the whole batch (bf16-rounded inputs)
     ref = torch.nn.BatchNorm2d(C).to(dev)
     with torch.no_grad():
@@ -339,8 +344,8 @@ def sync_bn_kernel_path(hvd):
     yr = ref(xf)
     yr.backward(gfull.to(torch.bfloat16).float())
     rel = lambda a, b: ((a.float() - b.float()).norm() / b.float().norm().clamp_min(1e-6)).item()
-    assert rel(y, yr[r * 4:(r + 1) * 4]) < 1e-2
-    assert rel(x.grad, xf.grad[r * 4:(r + 1) * 4]) < 2e-2
+    assert rel(y, yr[lo:hi]) < 1e-2
+    assert rel(x.grad, xf.grad[lo:hi]) < 2e-2
     # local parameter gradients sum (over ranks) to the global ones
     gw = hvd.allreduce(bn.weight.grad.float(), op=hvd.Sum)
     assert rel(gw, ref.weight.grad) < 2e-2

@@ -544,6 +544,22 @@ def bn_bwd_bounds(x2, dz2, gamma, D_f, D_b, pbf16, eps=BN_EPS):
     return (dx, bf16_store(dxb, dx)), (dg, dgb), (db, dbb)
 
 
+def running_stats_bounds(rm0, rv0, m, var, Em, Evar, M, mom, pbf16):
+    """running_mean / running_var after one step of ``bn_finalize_kernel`` over M rows: fl((1 - mom) r + mom s) in
+    fp32, s = m~ or the unbiased var~ M / max(M - 1, 1), then the store in the parameter dtype.  Against the float64
+    update of rm0 / rv0 with the exact statistics: the error of s times mom, and 5 u of the terms for fl32(mom), the
+    two products and the sum.  Returns (rm, Erm, rv, Erv)."""
+    c = M / max(M - 1, 1)
+    rm = (1 - mom) * rm0 + mom * m
+    Erm = mom * Em * (1 + U32) + 5 * U32 * ((1 - mom) * rm0.abs() + mom * (m.abs() + Em))
+    rv = (1 - mom) * rv0 + mom * var * c
+    Eunb = c * (Evar + 2.02 * U32 * (var + Evar))
+    Erv = mom * Eunb * (1 + U32) + 5 * U32 * ((1 - mom) * rv0.abs() + mom * (var * c + Eunb))
+    if pbf16:
+        Erm, Erv = bf16_store(Erm, rm), bf16_store(Erv, rv)
+    return rm, Erm, rv, Erv
+
+
 def bn_inputs(M, C, seed, D=0):
     """x [M, C]: per channel, c % 4 == 0: zero mean; 1: |mean| / std = 8; 2: |mean| / std = 64; 3: constant
     (var = 0, invstd = rsqrt(eps)) of a value with at most 4 significant bits, 0 included (a dead ReLU channel);
@@ -679,14 +695,7 @@ def test_bn_train_fwd_bwd_vs_fp64(C, M, src, pdtype, with_res, relu):
         assert bool((bits[sure] == (pre[sure] > 0)).all()), "ReLU mask bit disagrees with the sign of y"
         assert bool((_to2(y)[~bits] == 0).all()), "y nonzero where the mask bit is clear"
     # running statistics (param dtype), momentum 0.1, unbiased variance
-    c = M / max(M - 1, 1)
-    rm = (1 - BN_MOM) * rm0 + BN_MOM * m
-    Erm = BN_MOM * Em * (1 + U32) + 5 * U32 * ((1 - BN_MOM) * rm0.abs() + BN_MOM * (m.abs() + Em))
-    rv = (1 - BN_MOM) * rv0 + BN_MOM * var * c
-    Eunb = c * (Evar + 2.02 * U32 * (var + Evar))
-    Erv = BN_MOM * Eunb * (1 + U32) + 5 * U32 * ((1 - BN_MOM) * rv0.abs() + BN_MOM * (var * c + Eunb))
-    if pdtype == torch.bfloat16:
-        Erm, Erv = bf16_store(Erm, rm), bf16_store(Erv, rv)
+    rm, Erm, rv, Erv = running_stats_bounds(rm0, rv0, m, var, Em, Evar, M, BN_MOM, pdtype == torch.bfloat16)
     _check(bn.running_mean, rm, Erm, "bn running_mean")
     _check(bn.running_var, rv, Erv, "bn running_var (unbiased)")
     assert int(bn.num_batches_tracked) == nbt0 + 1
