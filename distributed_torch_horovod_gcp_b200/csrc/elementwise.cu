@@ -9,6 +9,7 @@
 //             the residual-branch gradient together.
 // Statistics accumulate in fp32 (vector registers -> shared -> one slot per block, summed in block order
 // by the last block: see block_reduce_to_global).
+#include <initializer_list>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -797,6 +798,17 @@ bool shape_ok(int C) {
   return C % 8 == 0 && V >= 1 && V <= THREADS && (THREADS % V) == 0;   // V | 256 | 1024
 }
 
+// The activation tensors of the BatchNorm and LayerNorm kernels are read and written as 16-byte vectors (uint4):
+// -1 with a message naming `what` unless every pointer given is 16-byte aligned (nullptr: absent, accepted).
+int check_vec16(const char* what, std::initializer_list<const void*> ptrs) {
+  for (const void* p : ptrs)
+    if ((uintptr_t)p & 15) {
+      snprintf(g_err, sizeof(g_err), "%s: every activation tensor must be 16-byte aligned", what);
+      return -1;
+    }
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -860,6 +872,11 @@ int b200dp_bn_fwd(const void* x, const void* res, void* y, const void* gamma, co
     snprintf(g_err, sizeof(g_err), "unsupported channel count %d", C);
     return -1;
   }
+  if (M < 1) {   // the batch statistics of no rows are undefined, and the running statistics must not take them
+    snprintf(g_err, sizeof(g_err), "bn_fwd: needs at least one row");
+    return -1;
+  }
+  if (check_vec16("bn_fwd", {x, res, y})) return -1;
   cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
   const int V = C / 8;
   const long long nvec = M * V;
@@ -884,7 +901,7 @@ int b200dp_bn_fwd(const void* x, const void* res, void* y, const void* gamma, co
 // ---- SyncBatchNorm building blocks: the same kernels with the cross-rank reduction between the passes ----
 // local statistics only: stats[2*C] = sum | sum of squares over this rank's M rows
 int b200dp_bn_stats(const void* x, float* stats, long long M, int C, unsigned long long stream) {
-  if (!shape_ok(C)) return -1;
+  if (!shape_ok(C) || check_vec16("bn_stats", {x})) return -1;
   cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
   cudaError_t e = cudaMemsetAsync(stats, 0, sizeof(float) * 2 * C, st);
   if (e != cudaSuccess) return fail("memset", e);
@@ -901,7 +918,7 @@ int b200dp_bn_fwd_sync(const void* x, const void* res, void* y, const void* gamm
                        const float* stats, float* mean, float* invstd, float* a, float* b, void* running_mean,
                        void* running_var, long long M_local, const float* count, int C, float eps, float momentum,
                        int relu, int param_bf16, void* relu_mask, unsigned long long stream) {
-  if (!shape_ok(C)) return -1;
+  if (!shape_ok(C) || check_vec16("bn_fwd_sync", {x, res, y})) return -1;
   cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
   const int V = C / 8;
   const long long nvec = M_local * V;
@@ -918,7 +935,7 @@ int b200dp_bn_fwd_sync(const void* x, const void* res, void* y, const void* gamm
 // backward, pass 1: local sums[2*C] = sum dz | sum dz*(x - mean)     (dz = dy masked by the ReLU)
 int b200dp_bn_bwd_reduce(const void* dy, const void* x, const void* relu_mask, const float* mean, float* sums,
                          long long M, int C, int relu, unsigned long long stream) {
-  if (!shape_ok(C)) return -1;
+  if (!shape_ok(C) || check_vec16("bn_bwd_reduce", {dy, x})) return -1;
   cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
   cudaError_t e = cudaMemsetAsync(sums, 0, sizeof(float) * 2 * C, st);
   if (e != cudaSuccess) return fail("memset", e);
@@ -934,7 +951,7 @@ int b200dp_bn_bwd_reduce(const void* dy, const void* x, const void* relu_mask, c
 int b200dp_bn_bwd_apply(const void* dy, const void* x, const void* relu_mask, void* dx, void* dres,
                         const float* scale_a, const float* mean, const float* invstd, const float* sums,
                         const float* count, long long M, int C, int relu, unsigned long long stream) {
-  if (!shape_ok(C)) return -1;
+  if (!shape_ok(C) || check_vec16("bn_bwd_apply", {dy, x, dx, dres})) return -1;
   const int V = C / 8;
   const long long nvec = M * V;
   bn_bwd_apply_kernel<true><<<grid_for(nvec, V), THREADS, 0, (cudaStream_t)(uintptr_t)stream>>>(
@@ -948,7 +965,8 @@ int b200dp_bn_bwd_apply(const void* dy, const void* x, const void* relu_mask, vo
 // Inference / frozen-statistics apply: y = relu(x*a + b + res) with caller-provided a, b.
 int b200dp_bn_apply(const void* x, const void* res, void* y, const float* a, const float* b, long long M,
                     int C, int relu, unsigned long long stream) {
-  if (!shape_ok(C)) return -1;
+  if (!shape_ok(C) || check_vec16("bn_apply", {x, res, y})) return -1;
+  if (M == 0) return 0;
   const int V = C / 8;
   const long long nvec = M * V;
   bn_apply_kernel<<<grid_for(nvec, V), THREADS, 0, (cudaStream_t)(uintptr_t)stream>>>(
@@ -963,7 +981,11 @@ int b200dp_bn_apply(const void* x, const void* res, void* y, const float* a, con
 int b200dp_bn_bwd(const void* dy, const void* x, const void* relu_mask, void* dx, void* dres, const float* scale_a,
                   const float* mean, const float* invstd, float* sums, void* dgamma, void* dbeta,
                   int param_bf16, long long M, int C, int relu, unsigned long long stream) {
-  if (!shape_ok(C)) return -1;
+  if (!shape_ok(C) || check_vec16("bn_bwd", {dy, x, dx, dres})) return -1;
+  if (M < 1) {
+    snprintf(g_err, sizeof(g_err), "bn_bwd: needs at least one row");
+    return -1;
+  }
   cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
   const int V = C / 8;
   const long long nvec = M * V;
@@ -1064,7 +1086,8 @@ int b200dp_ln_supported(int C) { return (C % 256 == 0 && C / 256 >= 1 && C / 256
 
 int b200dp_ln_fwd(const void* x, void* y, const void* gamma, const void* beta, float* mean, float* rstd,
                   long long rows, int C, float eps, int param_bf16, unsigned long long stream) {
-  if (!b200dp_ln_supported(C)) return -1;
+  if (!b200dp_ln_supported(C) || check_vec16("ln_fwd", {x, y})) return -1;
+  if (rows == 0) return 0;
   cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
   long long blocks = (rows + LN_WARPS - 1) / LN_WARPS;
   if (blocks > reduce_grid() * 4) blocks = reduce_grid() * 4;
@@ -1080,10 +1103,15 @@ int b200dp_ln_fwd(const void* x, void* y, const void* gamma, const void* beta, f
 int b200dp_ln_bwd(const void* dy, const void* x, void* dx, const void* gamma, const float* mean,
                   const float* rstd, float* sums, void* dgamma, void* dbeta, long long rows, int C,
                   int param_bf16, unsigned long long stream) {
-  if (!b200dp_ln_supported(C)) return -1;
+  if (!b200dp_ln_supported(C) || check_vec16("ln_bwd", {dy, x, dx})) return -1;
   cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
   cudaError_t e = cudaMemsetAsync(sums, 0, sizeof(float) * 2 * C, st);
   if (e != cudaSuccess) return fail("memset", e);
+  if (rows == 0) {   // no rows: zero parameter gradients, no row kernel
+    ln_param_grad_kernel<<<(C + 255) / 256, 256, 0, st>>>(sums, dgamma, dbeta, C, param_bf16);
+    e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : fail("ln_bwd launch", e);
+  }
   long long blocks = (rows + LN_WARPS - 1) / LN_WARPS;
   if (blocks > reduce_grid() * 2) blocks = reduce_grid() * 2;
   const size_t smem = sizeof(float) * LN_WARPS * C;

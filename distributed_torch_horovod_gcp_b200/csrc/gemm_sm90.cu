@@ -113,7 +113,7 @@ const char* b200dp_gemm_last_error() { return g_err; }
 // C's dtype (out_bf16: bf16, else fp32), rounded once from fp32.  With splits > 1 (out_mode 1/2 only) the last
 // split to finish a tile sums the partials of all splits in split order.
 // Requirements: K % 8 == 0 for K-major operands, M % 8 (A) / N % 8 (B) == 0 for MN-major, N % 8 == 0,
-// 16-byte aligned base pointers and leading dimensions.
+// 16-byte aligned base pointers and leading dimensions, residual included; preact 4-byte aligned.
 int b200dp_gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, int lda, int ldb, int ldc,
                      int a_mn, int b_mn, const void* bias_bf16, const void* bias_f32, const void* residual,
                      void* preact, int act, int out_mode, int out_bf16, float alpha, int splits, int block_n,
@@ -123,6 +123,10 @@ int b200dp_gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K,
   if ((N % 8) || (lda % 8) || (ldb % 8) || (ldc % 4) || ((out_mode == 0 || out_bf16) && (ldc % 8)))
     return fail("alignment: N, lda, ldb, ldc must be multiples of 8");
   if (((uintptr_t)A | (uintptr_t)B | (uintptr_t)C) & 15) return fail("pointers must be 16-byte aligned");
+  // the epilogue loads the residual in 16-byte vectors and stores the pre-activation in bf16 pairs
+  if ((uintptr_t)residual & 15) return fail("residual must be 16-byte aligned");
+  if ((uintptr_t)preact & 3) return fail("preact must be 4-byte aligned");
+  if (((uintptr_t)bias_bf16 & 1) || ((uintptr_t)bias_f32 & 3)) return fail("bias must be aligned to its element");
   const int BN = pick_bn(N, block_n);
   if (BN < 0) return -1;
   GemmParams p{};

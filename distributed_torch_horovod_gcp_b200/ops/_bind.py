@@ -35,8 +35,8 @@ def register(lib, have: Dict[str, bool]) -> None:
     _dropout.register(lib, have)
 
 
-def linear_supported(x, weight) -> bool:
-    return _gemm.supported(x, weight)
+def linear_supported(x, weight, bias=None, residual=None, w2=None, b2=None) -> bool:
+    return _gemm.supported(x, weight, bias, residual, w2, b2)
 
 
 def layer_norm_supported(x, weight, bias) -> bool:

@@ -70,7 +70,35 @@ def bn_supported(x: torch.Tensor, C: int) -> bool:
 
 
 def _cl(t: torch.Tensor) -> torch.Tensor:
-    return t if t.is_contiguous(memory_format=torch.channels_last) else t.contiguous(memory_format=torch.channels_last)
+    """``t`` as a dense channels_last tensor with a 16-byte aligned base (``contiguous`` keeps a dense view at an
+    unaligned storage offset as it is)."""
+    if t.is_contiguous(memory_format=torch.channels_last) and t.data_ptr() % 16 == 0:
+        return t
+    return t.clone(memory_format=torch.channels_last)
+
+
+def params_ok(weight, bias, running_mean=None, running_var=None) -> bool:
+    """The BN kernels read (and write back) gamma, beta and the running statistics in one dtype, chosen by gamma
+    (``param_bf16``): gamma and beta must be present, and every one present must be a dense [C] tensor of that
+    dtype, bf16 or fp32."""
+    if weight is None or bias is None or weight.dtype not in (torch.bfloat16, torch.float32):
+        return False
+    C = weight.shape[0] if weight.dim() == 1 else -1
+    return all(t.dtype == weight.dtype and t.device == weight.device and tuple(t.shape) == (C,) and t.stride(0) == 1
+               for t in (weight, bias, running_mean, running_var) if t is not None)
+
+
+def module_ok(bn, C: int, rows: int) -> bool:
+    """Whether ``bn`` (a BatchNorm2d over ``C`` channels and ``rows`` = N H W positions) can run on the fused
+    kernels: ``params_ok``; in training, a constant ``momentum`` (``None``, the cumulative average, takes torch's
+    path) and more than one value per channel (torch refuses one); in eval mode, running statistics to apply."""
+    if _lib is None or bn.num_features != C or not bool(_lib.b200dp_bn_supported(C)):
+        return False
+    if not params_ok(bn.weight, bn.bias, bn.running_mean, bn.running_var):
+        return False
+    if bn.training:
+        return bn.momentum is not None and rows > 1
+    return bn.track_running_stats and bn.running_mean is not None and bn.running_var is not None and rows > 0
 
 
 def bn_forward(x, bn: torch.nn.BatchNorm2d, residual, relu: bool, stats_in=None, grads=(True, True)):
@@ -85,7 +113,7 @@ def bn_forward(x, bn: torch.nn.BatchNorm2d, residual, relu: bool, stats_in=None,
     gamma, beta = bn.weight, bn.bias
     nbt = bn.num_batches_tracked if (bn.track_running_stats and bn.num_batches_tracked is not None
                                      and bn.num_batches_tracked.is_cuda) else None   # += 1 inside bn_finalize
-    mom = bn.momentum if bn.momentum is not None else 0.1
+    mom = bn.momentum                  # not None: module_ok sends the cumulative average to torch's path
     y = torch.empty_like(x, memory_format=torch.channels_last)
     ws = torch.empty(6 * C, dtype=torch.float32, device=dev)
     stats, mean, invstd, a, b = ws[:2 * C], ws[2 * C:3 * C], ws[3 * C:4 * C], ws[4 * C:5 * C], ws[5 * C:]
@@ -264,7 +292,8 @@ def conv2d(x, conv: torch.nn.Conv2d, stats=None):
     from . import conv as _conv
     if conv.bias is None and _conv.supported(x, w, conv.stride, conv.padding, conv.dilation, conv.groups):
         return _conv.conv2d(x, w, conv.stride[0], conv.padding[0], stats), stats is not None
-    return F.conv2d(x, w, conv.bias, conv.stride, conv.padding, conv.dilation, conv.groups), False
+    b = conv.bias.to(x.dtype) if conv.bias is not None else None
+    return F.conv2d(x, w.to(x.dtype), b, conv.stride, conv.padding, conv.dilation, conv.groups), False
 
 
 def _stats_buffer(bn, C: int, device):
@@ -282,15 +311,28 @@ def fused_stats(bn, C: int, device) -> Optional[torch.Tensor]:
     return _stats_buffer(bn, C, device) if _FUSE_STATS and bn.training and C <= 2048 else None
 
 
+def _out_rows(x, conv) -> int:
+    """N * OH * OW of the convolution's output."""
+    N, _, H, W = x.shape
+    (R, S), (sh, sw), (ph, pw), (dh, dw) = conv.kernel_size, conv.stride, conv.padding, conv.dilation
+    return N * max((H + 2 * ph - dh * (R - 1) - 1) // sh + 1, 0) * max((W + 2 * pw - dw * (S - 1) - 1) // sw + 1, 0)
+
+
+def _wants_grad(*ts) -> bool:
+    return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in ts)
+
+
 def conv_bn_act(x, conv, bn, relu: bool, residual=None):
     C = conv.out_channels
-    fused_bn = _lib is not None and bn.weight is not None and bool(_lib.b200dp_bn_supported(C)) and \
+    fused_bn = x.dim() == 4 and isinstance(conv.padding, tuple) and module_ok(bn, C, _out_rows(x, conv)) and \
         (residual is None or residual.dtype == torch.bfloat16)
     stats = fused_stats(bn, C, x.device) if fused_bn and x.dtype == torch.bfloat16 else None
     y, filled = conv2d(x, conv, stats=stats)
     if stats is not None and not filled:
         stats = None
-    if fused_bn and bn_supported(y, C):
+    # eval mode: the fused apply pass is no autograd node, so only where nothing needs a gradient
+    if fused_bn and bn_supported(y, C) and (residual is None or residual.shape == y.shape) and \
+            (bn.training or not _wants_grad(y, residual, bn.weight, bn.bias)):
         return bn_act(y, bn, relu, residual, stats=stats)
     if stats is not None:
         stats.zero_()          # filled but not consumed by the fused BN: keep the accumulator clean

@@ -24,13 +24,15 @@ def _units(block):
 
 
 def supported(x: torch.Tensor, block) -> bool:
-    """NHWC bf16 ``x``; every BN in training mode with the fused kernel for its channel count; conv1 and
+    """NHWC bf16 ``x``; every BN in training mode and on the fused kernels (``ops.bn.module_ok``); conv1 and
     conv3 on the 1x1 GEMM, conv2 and the downsample on the GEMM or the implicit-GEMM kernel.  The
     activations inside the block are fresh NHWC bf16 tensors like ``x``, so ``x`` stands in for them."""
     if _bn._lib is None or not _bn._nhwc_ok(x):
         return False
+    rows1 = x.shape[0] * x.shape[2] * x.shape[3]
+    rows2 = _bn._out_rows(x, block.conv2)           # conv2, the downsample and conv3 share its output grid
     for conv, bn in _units(block):
-        if not (bn.training and bn.weight is not None and _bn._lib.b200dp_bn_supported(conv.out_channels)):
+        if not (bn.training and _bn.module_ok(bn, conv.out_channels, rows1 if conv is block.conv1 else rows2)):
             return False
         if not _bn._is_gemm_conv(x, conv) and (conv in (block.conv1, block.conv3) or conv.bias is not None or
                                                not _conv.supported(x, conv.weight, conv.stride, conv.padding,

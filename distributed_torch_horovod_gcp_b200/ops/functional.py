@@ -90,7 +90,7 @@ def linear_reference(x, weight, bias=None, act: Optional[str] = None, residual=N
 
 def linear(x, weight, bias=None, act: Optional[str] = None, residual=None):
     k = _kernels(x)
-    if k is not None and k.has("linear") and k.linear_supported(x, weight):
+    if k is not None and k.has("linear") and k.linear_supported(x, weight, bias, residual):
         return k.linear(x, weight, bias, act, residual)
     return linear_reference(x, weight, bias, act, residual)
 
@@ -98,8 +98,8 @@ def linear(x, weight, bias=None, act: Optional[str] = None, residual=None):
 def mlp(x, w1, b1, w2, b2, residual=None):
     """Transformer MLP: fc2(gelu(fc1(x))) + residual (one fused autograd node on the kernel path)."""
     k = _kernels(x)
-    if k is not None and k.has("linear") and k.linear_supported(x, w1) and b1 is not None \
-            and b2 is not None and w2.shape[0] % 8 == 0:
+    if k is not None and k.has("linear") and b1 is not None and b2 is not None \
+            and k.linear_supported(x, w1, b1, residual, w2=w2, b2=b2):
         return k.mlp(x, w1, b1, w2, b2, residual)
     return linear_reference(linear_reference(x, w1, b1, act="gelu"), w2, b2, residual=residual)
 
@@ -136,7 +136,8 @@ def layer_norm(x, weight, bias, eps: float = 1e-6):
     k = _kernels(x)
     if k is not None and k.has("layer_norm") and k.layer_norm_supported(x, weight, bias):
         return k.layer_norm(x, weight, bias, eps)
-    return F.layer_norm(x, (x.shape[-1],), weight.to(x.dtype), None if bias is None else bias.to(x.dtype), eps)
+    return F.layer_norm(x, (x.shape[-1],), None if weight is None else weight.to(x.dtype),
+                        None if bias is None else bias.to(x.dtype), eps)
 
 
 # ------------------------------------------------------------------ attention
@@ -153,10 +154,8 @@ def attention_reference(qkv, heads: int, causal: bool = False, dropout_p: float 
 
 
 def attention(qkv, heads: int, causal: bool = False, dropout_p: float = 0.0):
-    dropout_p = _check_p(dropout_p)
-    k = _kernels(qkv)
-    if k is not None and k.has("attention"):
-        return k.attention(qkv, heads, causal, dropout_p)
+    """Self-attention of a packed ``[B, S, 3 D]`` tensor: always the SDPA composition.  The flash-attention
+    kernels take q, k and v as the three dense projection outputs ``qkv_attention`` makes."""
     return attention_reference(qkv, heads, causal, dropout_p)
 
 
@@ -167,7 +166,8 @@ def qkv_attention(x, weight, bias, heads: int, causal: bool = False, dropout_p: 
     Kernel path: q, k, v are produced as three dense matrices (no un-pack / re-pack copies)."""
     dropout_p = _check_p(dropout_p)
     k = _kernels(x)
-    if k is not None and k.has("linear") and k.linear_supported(x, weight) and weight.shape[0] % 24 == 0 \
+    if k is not None and k.has("linear") and k.linear_supported(x, weight, bias) and x.dim() == 3 \
+            and weight.shape[0] == 3 * x.shape[-1] and weight.shape[0] % 24 == 0 and x.shape[-1] % heads == 0 \
             and os.environ.get("B200DP_SPLIT_QKV", "1") == "1":
         B, S, D = x.shape
         hd = D // heads

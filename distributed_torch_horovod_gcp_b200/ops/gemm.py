@@ -70,11 +70,50 @@ def gemm(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor, M: int, N: int, K:
     return out
 
 
-def supported(x: torch.Tensor, weight: torch.Tensor) -> bool:
-    if _lib is None or x.dtype != torch.bfloat16 or weight.dtype != torch.bfloat16:
+def _weight_ok(w: torch.Tensor, dev) -> bool:
+    """A bf16 [N, K] operand the TMA descriptor takes as it is: unit column stride, 16-byte rows and base."""
+    return (w.dtype == torch.bfloat16 and w.dim() == 2 and w.device == dev and w.shape[0] % 8 == 0
+            and w.shape[1] % 8 == 0 and w.stride(1) == 1 and w.stride(0) % 8 == 0 and w.data_ptr() % 16 == 0)
+
+
+def _bias_ok(bias: Optional[torch.Tensor], N: int, dev) -> bool:
+    """The epilogue reads ``bias[col]`` for col < N in bf16 or fp32 (any other dtype would not be passed)."""
+    return bias is None or (bias.dtype in (torch.bfloat16, torch.float32) and bias.device == dev
+                            and tuple(bias.shape) == (N,) and bias.stride(0) == 1)
+
+
+def _residual_ok(residual: Optional[torch.Tensor], shape, dev) -> bool:
+    """The epilogue reads the residual as a bf16 [M, N] matrix, so it must be one of the output's shape (no
+    broadcasting).  A misaligned or strided one is copied into a dense tensor first (``_dense``)."""
+    return residual is None or (residual.dtype == torch.bfloat16 and residual.device == dev
+                                and tuple(residual.shape) == tuple(shape))
+
+
+def supported(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] = None,
+              residual: Optional[torch.Tensor] = None, w2: Optional[torch.Tensor] = None,
+              b2: Optional[torch.Tensor] = None) -> bool:
+    """Whether ``linear(x, weight, bias, residual=residual)`` (or ``qkv_proj``) runs on the kernel: bf16 ``x``
+    with at least one row and bf16 weights of whole 16-byte rows, a bias of N elements in bf16 or fp32, and a bf16
+    residual of the output's shape.  With ``w2`` (``mlp``): fc1 = (weight, bias) and fc2 = (w2, b2), and the
+    residual is added to fc2's output."""
+    if _lib is None or x.dtype != torch.bfloat16 or x.dim() < 1 or not _weight_ok(weight, x.device):
         return False
     N, K = weight.shape
-    return N % 8 == 0 and K % 8 == 0 and x.shape[-1] == K and x.numel() // K >= 1
+    if x.shape[-1] != K or x.numel() // K < 1 or not _bias_ok(bias, N, x.device):
+        return False
+    if w2 is not None:
+        if not (_weight_ok(w2, x.device) and w2.shape[1] == N and _bias_ok(b2, w2.shape[0], x.device)):
+            return False
+        N = w2.shape[0]
+    return _residual_ok(residual, (*x.shape[:-1], N), x.device)
+
+
+def _dense(t: torch.Tensor) -> torch.Tensor:
+    """``t`` as a contiguous matrix with a 16-byte aligned base (``contiguous`` keeps a contiguous view at an
+    unaligned storage offset as it is)."""
+    if t.is_contiguous() and t.data_ptr() % 16 == 0:
+        return t
+    return t.clone(memory_format=torch.contiguous_format)
 
 
 def _splits_for(M_out: int, N_out: int, K_red: int, sms: int = 132) -> int:
@@ -149,16 +188,14 @@ class _LinearFn(torch.autograd.Function):
         N = weight.shape[0]
         x2 = x.reshape(-1, K)
         if x2.stride(-1) != 1 or (x2.stride(0) % 8) or (x2.data_ptr() % 16):
-            x2 = x2.contiguous()
+            x2 = x2.clone(memory_format=torch.contiguous_format)
         M = x2.shape[0]
         y = torch.empty((M, N), dtype=torch.bfloat16, device=x.device)
         need_z = act != 0 and any(ctx.needs_input_grad[0:3])      # dz feeds dx, dW and db; not dres
         z = torch.empty_like(y) if need_z else None
         r2 = None
         if residual is not None:
-            r2 = residual.reshape(-1, N)
-            if not r2.is_contiguous():
-                r2 = r2.contiguous()
+            r2 = _dense(residual.reshape(-1, N))
         gemm(x2, weight, y, M, N, K, bias=bias, residual=r2, preact=z, act=act, stats=stats)
         ctx.save_for_backward(x2, weight, z)
         ctx.act, ctx.has_bias, ctx.has_res = act, bias is not None, residual is not None
@@ -171,9 +208,7 @@ class _LinearFn(torch.autograd.Function):
         x2, weight, z = ctx.saved_tensors
         N, K = weight.shape
         M = x2.shape[0]
-        dy2 = dy.reshape(M, N)
-        if not dy2.is_contiguous():
-            dy2 = dy2.contiguous()
+        dy2 = _dense(dy.reshape(M, N))
         dres = dy2.view(*ctx.x_shape[:-1], N) if ctx.has_res else None
         if ctx.act != 0 and any(ctx.needs_input_grad[0:3]):
             dz = act_backward(dy2, z, ctx.act)
@@ -206,18 +241,14 @@ class _MLPFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, w1, b1, w2, b2, residual):
         D, Hd = w1.shape[1], w1.shape[0]
-        x2 = x.reshape(-1, D)
-        if not x2.is_contiguous():
-            x2 = x2.contiguous()
+        x2 = _dense(x.reshape(-1, D))
         M = x2.shape[0]
         dev = x.device
         z = torch.empty((M, Hd), dtype=torch.bfloat16, device=dev)
         h = torch.empty((M, Hd), dtype=torch.bfloat16, device=dev)
         gemm(x2, w1, h, M, Hd, D, bias=b1, preact=z, act=2)
         out = torch.empty((M, w2.shape[0]), dtype=torch.bfloat16, device=dev)
-        r2 = residual.reshape(M, -1) if residual is not None else None
-        if r2 is not None and not r2.is_contiguous():
-            r2 = r2.contiguous()
+        r2 = _dense(residual.reshape(M, -1)) if residual is not None else None
         gemm(h, w2, out, M, w2.shape[0], Hd, bias=b2, residual=r2)
         ctx.save_for_backward(x2, w1, w2, z, h)
         ctx.owners = (w1, w2)
@@ -234,9 +265,7 @@ class _MLPFn(torch.autograd.Function):
         x2, w1, w2, z, h = ctx.saved_tensors
         M, D = x2.shape
         Hd, Do = w1.shape[0], w2.shape[0]
-        dy2 = dy.reshape(M, Do)
-        if not dy2.is_contiguous():
-            dy2 = dy2.contiguous()
+        dy2 = _dense(dy.reshape(M, Do))
         dev = dy.device
         dz = torch.empty((M, Hd), dtype=torch.bfloat16, device=dev)
         gemm(dy2, w2, dz, M, Hd, Do, b_mn=True, residual=z, act=3)        # (dy @ W2) * gelu'(z)
@@ -266,9 +295,7 @@ class _QKVFn(torch.autograd.Function):
     def forward(ctx, x, weight, bias):
         D3, D = weight.shape
         Dh = D3 // 3
-        x2 = x.reshape(-1, D)
-        if not x2.is_contiguous():
-            x2 = x2.contiguous()
+        x2 = _dense(x.reshape(-1, D))
         M = x2.shape[0]
         outs = []
         for i in range(3):
@@ -290,10 +317,7 @@ class _QKVFn(torch.autograd.Function):
         dev = x2.device
         gs = []
         for g in (dq, dk, dv):
-            g2 = g.reshape(M, Dh)
-            if not g2.is_contiguous() or g2.data_ptr() % 16:
-                g2 = g2.contiguous()
-            gs.append(g2)
+            gs.append(_dense(g.reshape(M, Dh)))
         dx = None
         if ctx.needs_input_grad[0]:
             for i, g2 in enumerate(gs):

@@ -23,12 +23,17 @@ def register(lib, have):
     have["layer_norm"] = True
 
 
-def supported(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor) -> bool:
-    """The kernels read gamma and beta in one dtype (``pbf16``), so both must have it."""
+def supported(x: torch.Tensor, weight, bias) -> bool:
+    """bf16 ``x`` with at least one row and a 16-byte aligned base (the kernels load it in 16-byte vectors), and
+    gamma and beta of C elements in one dtype, bf16 or fp32 (the kernels read both in the dtype ``pbf16`` names)."""
+    if _lib is None or weight is None or bias is None or x.dim() < 1:
+        return False
     C = x.shape[-1]
-    return (_lib is not None and x.dtype == torch.bfloat16 and x.is_cuda
-            and weight.dtype in (torch.bfloat16, torch.float32) and bias is not None
-            and bias.dtype == weight.dtype and bool(_lib.b200dp_ln_supported(C)))
+    return (x.dtype == torch.bfloat16 and x.is_cuda and x.numel() > 0 and x.data_ptr() % 16 == 0
+            and weight.dtype in (torch.bfloat16, torch.float32) and bias.dtype == weight.dtype
+            and tuple(weight.shape) == (C,) and tuple(bias.shape) == (C,) and weight.stride(0) == 1
+            and bias.stride(0) == 1 and weight.device == x.device and bias.device == x.device
+            and bool(_lib.b200dp_ln_supported(C)))
 
 
 class _LayerNormFn(torch.autograd.Function):
@@ -57,8 +62,8 @@ class _LayerNormFn(torch.autograd.Function):
         x2, weight, stats = ctx.saved_tensors
         R, C = x2.shape
         dy2 = dy.reshape(R, C)
-        if not dy2.is_contiguous():
-            dy2 = dy2.contiguous()
+        if not dy2.is_contiguous() or dy2.data_ptr() % 16:
+            dy2 = dy2.clone(memory_format=torch.contiguous_format)
         dx = torch.empty_like(x2)
         sums = torch.empty(2 * C, dtype=torch.float32, device=dy.device)
         dgb = torch.empty(2 * C, dtype=weight.dtype, device=dy.device)

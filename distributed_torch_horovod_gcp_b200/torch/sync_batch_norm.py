@@ -129,14 +129,13 @@ class _SyncBNKernelFn(torch.autograd.Function):
 
 
 def _kernel_path_ok(x, weight, bias, running_mean=None, running_var=None) -> bool:
-    if not (x.is_cuda and x.dim() == 4 and x.dtype == torch.bfloat16 and weight is not None and bias is not None):
-        return False
-    # the kernels read (and write) every parameter in one dtype, chosen by `weight`
-    params = [t for t in (weight, bias, running_mean, running_var) if t is not None]
-    if weight.dtype not in (torch.bfloat16, torch.float32) or any(t.dtype != weight.dtype for t in params):
+    if not (x.is_cuda and x.dim() == 4 and x.dtype == torch.bfloat16):
         return False
     try:
         from ..ops import kernels, bn as B
+        # the kernels read (and write) every parameter in one dtype, chosen by `weight`
+        if not B.params_ok(weight, bias, running_mean, running_var):
+            return False
         if not kernels.has("bn_act") or not hasattr(B._lib, "b200dp_bn_fwd_sync"):
             return False
         return B.bn_supported(x, x.shape[1])
