@@ -85,6 +85,11 @@ def parse_args(argv=None):
                         "the GPT models AdamW, see gpt_optimizer); "
                         "'lars' / 'lamb' = hvd.LARS / hvd.LAMB with biases and norm-layer parameters in a "
                         "group with adaptive=False and no weight decay")
+    p.add_argument("--sequence-parallel", action="store_true",
+                   default=env("B200DP_SEQUENCE_PARALLEL", "0") == "1",
+                   help="GPT models: split each sequence across the ranks (zigzag shards, sequence-parallel "
+                        "attention) instead of giving each rank its own batch; every rank draws the same tokens "
+                        "and keeps its shard, and the printed losses are the rank averages")
     args = p.parse_args(argv)
     if args.optimizer != "default" and args.model.lower() == "lstm":
         p.error("--optimizer lars|lamb applies to the image models")
@@ -92,6 +97,14 @@ def parse_args(argv=None):
         p.error(f"--dropout must be in [0, 1], got {args.dropout}")
     if args.dropout and not (is_gpt(args.model) or is_vit(args.model)):
         p.error("--dropout applies to the GPT and ViT models (the LSTM has --lstm-dropout)")
+    if args.sequence_parallel:
+        if not is_gpt(args.model):
+            p.error("--sequence-parallel applies to the GPT models")
+        if args.dropout:
+            p.error("--sequence-parallel does not support --dropout")
+        if args.cuda_graph:
+            p.error("--sequence-parallel cannot be combined with --cuda-graph: the sequence-parallel attention's "
+                    "collectives are not captured in CUDA graphs")
     return args
 
 
@@ -204,18 +217,29 @@ if __name__ == "__main__":
         optimizer = torch.optim.Adam(model.parameters(), lr=args.lr)
         loss_fn = nn.MSELoss(reduction="mean")
     elif is_gpt(args.model):
-        model = build_model(args.model, **dropout_kw(args)).to(_DEVICE)
+        sp_kw = {"sequence_parallel": True} if args.sequence_parallel else {}
+        model = build_model(args.model, **dropout_kw(args), **sp_kw).to(_DEVICE)
         if compute_dtype != torch.float32:
             model = model.to(compute_dtype)
         seq_len = args.seq_len or model.context
-        tokens = SyntheticTokenBatches(args.batch_size, seq_len, model.vocab, _DEVICE, seed=hvd.rank())
+        # sequence parallelism: one batch for the world, each rank keeps its zigzag shard of every sequence
+        tokens = SyntheticTokenBatches(args.batch_size, seq_len, model.vocab, _DEVICE,
+                                       seed=0 if args.sequence_parallel else hvd.rank())
+
+        def _next_tokens():
+            inputs, labels = tokens.next()
+            if not args.sequence_parallel:
+                return inputs, labels
+            from distributed_torch_horovod_gcp_b200.ops.seq_parallel import zigzag_shard
+            shard = (lambda t: zigzag_shard(t, 1, hvd.rank(), hvd.size()))
+            return shard(inputs), shard(labels.view(inputs.shape)).reshape(-1)
 
         class _TokenLoader:
             def __iter__(self_inner):
                 for _ in range(args.steps_per_epoch):
-                    yield tokens.next()
+                    yield _next_tokens()
         train_loader = _TokenLoader()
-        test_loader = [tokens.next()]
+        test_loader = [_next_tokens()]
         lr = args.lr if args.lr != 1e-6 else 6e-4
         optimizer = gpt_optimizer(model, lr) if args.optimizer == "default" else \
             image_optimizer(model, args.optimizer, lr)
@@ -286,6 +310,8 @@ if __name__ == "__main__":
                 loss = train_step(inputs, labels)
             if args.max_steps and i + 1 >= args.max_steps:
                 break
+        if args.sequence_parallel:
+            loss = hvd.allreduce(loss, average=True)      # each rank's loss is the mean over its own tokens
         # write stats if running on main
         if device == 0:
             print(f"epoch: {epoch}, train_loss: {loss}", flush=True)
@@ -296,6 +322,8 @@ if __name__ == "__main__":
             test_inputs, test_labels = test_data[0].to(_DEVICE), test_data[1].to(_DEVICE)
             test_pred = model(test_inputs)
             test_loss = loss_fn(test_pred.float(), test_labels)
+        if args.sequence_parallel:
+            test_loss = hvd.allreduce(test_loss.detach(), average=True)
         if device == 0:
             print(f"epoch: {epoch}, test_loss: {test_loss}", flush=True)
 

@@ -45,6 +45,21 @@
 //   fragment layout above attn_fwd_kernel; S = Q K^T has the same layout in the backward), so each thread
 //   draws each Philox output once: 8 calls per 128 x 128 tile.
 //
+// Sequence parallelism (SP = true; CAUSAL or not, never DROPOUT): "rank r of W" holds a zigzag shard of the
+// sequence.  The global sequence is 2W chunks of c tiles (S_glob = 2 W c 128); rank r holds chunks r and
+// 2W - 1 - r, in that order, as its local rows (S_loc = 2 c 128), so under the causal mask every rank has the
+// same number of (query tile, key tile) pairs.  zz_global / zz_local map a local tile to its global tile and
+// back.  The operands owned by other ranks arrive as gathered [W][B][S_loc][H][64] views (what an all-gather
+// of each rank's tensor delivers), loaded through 5D tensor maps {64 d, S_loc, H, B, W}; the kernels reach other
+// ranks' data only through those buffers (no peer pointers, no barriers), so one GPU can run any rank.
+//   Forward: one CTA per (batch, head, local query tile) visits the key tiles in global order (0..its global
+//   tile when causal) from the gathered K / V; the mask is on global positions.  Each CTA computes exactly
+//   what the full-sequence kernel computes for that query tile, so O and LSE are bit-identical to it.
+//   Backward: one CTA per (batch, head, local key block) loops over the query tiles of all ranks in global
+//   order, reading the gathered Q, dO, LSE and delta, so dK / dV are bit-identical to the full-sequence
+//   kernel's; dQ partials go by fp32 RED.ADD into a [W][B][S_loc][H][64] workspace (row block of each query's
+//   owner), which the caller reduce-scatters.
+//
 // Replaces F.scaled_dot_product_attention (cuDNN / flash library kernels) on the ViT-B/16 and GPT paths.
 // The reference application has no attention.
 #include <cuda.h>
@@ -73,6 +88,7 @@ struct AttnFwdParams {
   const unsigned long long* seed;    // DROPOUT: Philox key, offset (2 words in device memory)
   uint32_t drop_thr;                 // DROPOUT: keep when the element's 16 bits are below this (t)
   float drop_scale;                  // DROPOUT: 2^16 / t (0 when t = 0)
+  int sp_rank, sp_world, sp_c;       // SP: this rank, the world, tiles per zigzag chunk
 };
 
 __device__ __forceinline__ float ex2(float x) {
@@ -96,6 +112,24 @@ __device__ __forceinline__ uint32_t pack2(float lo, float hi) {
   asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(v) : "f"(hi), "f"(lo));
   return v;
 }
+// SP zigzag map (see the header): global tile of local tile lt on rank r, and owner / local tile of global tile g.
+__device__ __forceinline__ int zz_global(int lt, int r, int W, int c) {
+  return lt < c ? r * c + lt : (2 * W - 1 - r) * c + (lt - c);
+}
+__device__ __forceinline__ void zz_local(int g, int W, int c, int& r, int& lt) {
+  const int ch = g / c, w = g - ch * c;
+  r = ch < W ? ch : 2 * W - 1 - ch;
+  lt = ch < W ? w : c + w;
+}
+__device__ __forceinline__ void tma_load_5d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1, int c2,
+                                            int c3, int c4) {
+  asm volatile(
+      "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], "
+      "[%1, {%3, %4, %5, %6, %7}], [%2];" ::"r"(smem_u32(dst)),
+      "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
+      : "memory");
+}
+
 __device__ __forceinline__ float quad_max(float v) {
   v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
   return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
@@ -130,7 +164,7 @@ constexpr int FW_SMEM = TILE_BYTES * (1 + FW_RING) + 2 * TILE_BYTES /*P*/ + 1024
 
 // Fragment of an m64 x N wgmma accumulator held by thread t of a warpgroup: element 4j + e is row
 // 16 (t / 32) + (t % 32) / 4 + 8 (e / 2), column 8 j + 2 (t % 4) + e % 2.
-template <bool CAUSAL, bool DROPOUT>
+template <bool CAUSAL, bool DROPOUT, bool SP = false>
 __global__ void __launch_bounds__(AT, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                 const __grid_constant__ CUtensorMap map_v, const AttnFwdParams p) {
@@ -150,7 +184,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
   const int qt = CAUSAL ? p.q_tiles - 1 - blockIdx.x / BH : blockIdx.x % p.q_tiles;
   const int bh = CAUSAL ? blockIdx.x % BH : blockIdx.x / p.q_tiles;
   const int h = bh % p.H, b = bh / p.H;
-  const int nb = CAUSAL ? qt + 1 : p.kv_blocks;
+  static_assert(!(SP && DROPOUT), "no dropout under sequence parallelism");
+  const int qg = SP ? zz_global(qt, p.sp_rank, p.sp_world, p.sp_c) : qt;   // global query tile (SP: local qt)
+  const int nb = CAUSAL ? qg + 1 : p.kv_blocks;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_q);
@@ -173,7 +209,13 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
         const int st = t % FW_RING;
         mbar_wait(&kv_empty[st], ((t / FW_RING) & 1) ^ 1);
         mbar_expect_tx(&kv_full[st], TILE_BYTES);
-        tma_load_4d((t & 1) ? &map_v : &map_k, &kv_full[st], sT + st * TILE_BYTES, 0, (t >> 1) * TILE, h, b);
+        if constexpr (SP) {
+          int r, lt;
+          zz_local(t >> 1, p.sp_world, p.sp_c, r, lt);
+          tma_load_5d((t & 1) ? &map_v : &map_k, &kv_full[st], sT + st * TILE_BYTES, 0, lt * TILE, h, b, r);
+        } else {
+          tma_load_4d((t & 1) ? &map_v : &map_k, &kv_full[st], sT + st * TILE_BYTES, 0, (t >> 1) * TILE, h, b);
+        }
       }
     }
   } else {
@@ -192,7 +234,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
     for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
     mbar_wait(q_full, 0);
     for (int j = 0; j < nb; ++j) {
-      const int valid = min(TILE, p.S - j * TILE);
+      const int valid = SP ? TILE : min(TILE, p.S - j * TILE);   // SP: S_loc is a multiple of 2 tiles
       // ---- S_j = Q K_j^T
       int t = 2 * j, st = t % FW_RING;
       mbar_wait(&kv_full[st], (t / FW_RING) & 1);
@@ -208,7 +250,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
       }
       if (leader) mbar_arrive(&kv_empty[st]);
       // ---- online softmax on the fragment
-      const bool diag = CAUSAL && j == qt;                // causal diagonal tile: key column <= query row
+      const bool diag = CAUSAL && j == qg;                // causal diagonal tile: key column <= query row
       float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
       for (int jj = 0; jj < TILE / 8; ++jj)
@@ -296,6 +338,8 @@ struct AttnBwdParams {
   const unsigned long long* seed;    // DROPOUT: as in AttnFwdParams
   uint32_t drop_thr;
   float drop_scale;
+  int sp_rank, sp_world, sp_c;       // SP: as in AttnFwdParams
+  long long lse_sw, dq_sw;           // SP: rank strides (elements) of the gathered lse / delta and of dq_acc
 };
 
 // delta[b][h][s] = sum_d dO * O   (8 lanes per row: one 16-byte load of each tensor per lane)
@@ -329,7 +373,7 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const __nv_bfloat16* __
 constexpr int BW_RING = 2;
 constexpr int BW_SMEM = TILE_BYTES * (2 + 2 * BW_RING) + 4 * TILE_BYTES + 1024 + 256;
 
-template <bool CAUSAL, bool DROPOUT>
+template <bool CAUSAL, bool DROPOUT, bool SP = false>
 __global__ void __launch_bounds__(AT, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                 const __grid_constant__ CUtensorMap map_v, const __grid_constant__ CUtensorMap map_do,
@@ -353,8 +397,10 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
   const int bh = CAUSAL ? blockIdx.x % BH : blockIdx.x / p.kv_blocks;
   const int h = bh % p.H, b = bh / p.H;
   const int nq = p.q_tiles;
-  const int i0 = CAUSAL ? kb : 0;                        // first query tile that sees this key block
-  const int kvalid = min(TILE, p.S - kb * TILE);
+  static_assert(!(SP && DROPOUT), "no dropout under sequence parallelism");
+  const int kg = SP ? zz_global(kb, p.sp_rank, p.sp_world, p.sp_c) : kb;   // global key block (SP: local kb)
+  const int i0 = CAUSAL ? kg : 0;                        // first query tile that sees this key block
+  const int kvalid = SP ? TILE : min(TILE, p.S - kb * TILE);
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_q);
@@ -379,8 +425,15 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
         const int st = (i - i0) % BW_RING;
         mbar_wait(&r_empty[st], (((i - i0) / BW_RING) & 1) ^ 1);
         mbar_expect_tx(&r_full[st], 2 * TILE_BYTES);
-        tma_load_4d(&map_q, &r_full[st], sR + (2 * st) * TILE_BYTES, 0, i * TILE, h, b);
-        tma_load_4d(&map_do, &r_full[st], sR + (2 * st + 1) * TILE_BYTES, 0, i * TILE, h, b);
+        if constexpr (SP) {
+          int r, lt;
+          zz_local(i, p.sp_world, p.sp_c, r, lt);
+          tma_load_5d(&map_q, &r_full[st], sR + (2 * st) * TILE_BYTES, 0, lt * TILE, h, b, r);
+          tma_load_5d(&map_do, &r_full[st], sR + (2 * st + 1) * TILE_BYTES, 0, lt * TILE, h, b, r);
+        } else {
+          tma_load_4d(&map_q, &r_full[st], sR + (2 * st) * TILE_BYTES, 0, i * TILE, h, b);
+          tma_load_4d(&map_do, &r_full[st], sR + (2 * st + 1) * TILE_BYTES, 0, i * TILE, h, b);
+        }
       }
     }
   } else {
@@ -426,13 +479,16 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
       // ---- P = exp2(S c - LSE), dS = P (dP - D) / sqrt(d) -> bf16 smem
       float lse2[2], dl[2];
       bool qok[2];
-      const bool diag = CAUSAL && i == kb;                // causal diagonal tile: key column <= query row
+      const bool diag = CAUSAL && i == kg;                // causal diagonal tile: key column <= query row
+      int qr = 0, ql = i;                                // SP: the owner of query tile i and its local tile there
+      if constexpr (SP) zz_local(i, p.sp_world, p.sp_c, qr, ql);
+      const size_t row_off = SP ? (size_t)qr * p.lse_sw + bh_off : bh_off;
 #pragma unroll
       for (int h2 = 0; h2 < 2; ++h2) {
-        const int qrow = i * TILE + r0 + 8 * h2;
+        const int qrow = ql * TILE + r0 + 8 * h2;
         qok[h2] = qrow < p.S;
-        lse2[h2] = qok[h2] ? p.lse[bh_off + qrow] * 1.4426950408889634f : 0.f;
-        dl[h2] = qok[h2] ? p.delta[bh_off + qrow] : 0.f;
+        lse2[h2] = qok[h2] ? p.lse[row_off + qrow] * 1.4426950408889634f : 0.f;
+        dl[h2] = qok[h2] ? p.delta[row_off + qrow] : 0.f;
       }
       uint4 rnd;
 #pragma unroll
@@ -488,7 +544,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
 #pragma unroll
       for (int h2 = 0; h2 < 2; ++h2) {
         if (qok[h2]) {
-          float* dst = p.dq_acc + (size_t)b * p.dq_sb + (size_t)h * p.dq_sh + (size_t)(i * TILE + r0 + 8 * h2) * p.dq_ss;
+          float* dst = p.dq_acc + (SP ? (size_t)qr * p.dq_sw : 0) + (size_t)b * p.dq_sb + (size_t)h * p.dq_sh +
+                       (size_t)(ql * TILE + r0 + 8 * h2) * p.dq_ss;
 #pragma unroll
           for (int jj = 0; jj < HD / 8; ++jj)
             asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst + 8 * jj + cq), "f"(dqv[4 * jj + 2 * h2]),
@@ -540,16 +597,47 @@ int check_mode(int causal, const unsigned long long* seed, float drop_p, Params&
   return 0;
 }
 
-template <bool CAUSAL, bool DROPOUT, typename... Args>
+template <bool CAUSAL, bool DROPOUT, bool SP = false, typename... Args>
 int launch_fwd(dim3 grid, cudaStream_t st, Args... args) {
-  if (smem_attr_once<attn_fwd_kernel<CAUSAL, DROPOUT>>(FW_SMEM)) return -1;
-  attn_fwd_kernel<CAUSAL, DROPOUT><<<grid, AT, FW_SMEM, st>>>(args...);
+  if (smem_attr_once<attn_fwd_kernel<CAUSAL, DROPOUT, SP>>(FW_SMEM)) return -1;
+  attn_fwd_kernel<CAUSAL, DROPOUT, SP><<<grid, AT, FW_SMEM, st>>>(args...);
   return 0;
 }
-template <bool CAUSAL, bool DROPOUT, typename... Args>
+template <bool CAUSAL, bool DROPOUT, bool SP = false, typename... Args>
 int launch_bwd(dim3 grid, cudaStream_t st, Args... args) {
-  if (smem_attr_once<attn_bwd_kernel<CAUSAL, DROPOUT>>(BW_SMEM)) return -1;
-  attn_bwd_kernel<CAUSAL, DROPOUT><<<grid, AT, BW_SMEM, st>>>(args...);
+  if (smem_attr_once<attn_bwd_kernel<CAUSAL, DROPOUT, SP>>(BW_SMEM)) return -1;
+  attn_bwd_kernel<CAUSAL, DROPOUT, SP><<<grid, AT, BW_SMEM, st>>>(args...);
+  return 0;
+}
+
+// SP: a gathered [W][B][S][H][64] operand as a {64 d, S, H, B, W} map with element strides s = {w, b, h, s};
+// box {64, 128, 1, 1, 1}
+int make_gathered_map(CUtensorMap* m, const void* ptr, int W, int B, int H, int S, const long long* s) {
+  if ((s[0] % 8) || (s[1] % 8) || (s[2] % 8) || (s[3] % 8) || ((uintptr_t)ptr & 15))
+    return fail("gathered attention operands must be 16-byte aligned");
+  const cuuint64_t dims[5] = {(cuuint64_t)HD, (cuuint64_t)S, (cuuint64_t)H, (cuuint64_t)B, (cuuint64_t)W};
+  const cuuint64_t strides[4] = {(cuuint64_t)s[3] * 2, (cuuint64_t)s[2] * 2, (cuuint64_t)s[1] * 2, (cuuint64_t)s[0] * 2};
+  const cuuint32_t box[5] = {64, TILE, 1, 1, 1};
+  const cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+  CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<void*>(ptr), dims, strides, box, estr,
+                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled failed", (int)r);
+  return 0;
+}
+
+// SP arguments shared by the forward and the backward; fills the zigzag fields of the params
+template <typename Params>
+int check_sp(int B, int H, int S, int D, int causal, int rank, int world, Params& p) {
+  if (D != HD) return fail("head dim must be 64");
+  if (causal != 0 && causal != 1) return fail("causal must be 0 or 1");
+  if (B < 1 || H < 1) return fail("attention shapes must be positive");
+  if (world < 1 || rank < 0 || rank >= world) return fail("sequence parallelism needs 0 <= rank < world");
+  if (S < 2 * TILE || S % (2 * TILE)) return fail("sequence-parallel shards must be a positive multiple of 256 rows");
+  if ((long long)S * world > (1 << 30)) return fail("sequence too long");
+  p.B = B; p.H = H; p.S = S;
+  p.sp_rank = rank; p.sp_world = world; p.sp_c = S / (2 * TILE);
+  p.seed = nullptr; p.drop_thr = 0; p.drop_scale = 1.f;
   return 0;
 }
 
@@ -649,6 +737,85 @@ int b200dp_attn_bwd_dropout(const void* q, const void* k, const void* v, const v
                                 : launch_bwd<true, false>(grid, st, mq, mk, mv, mdo, p))
                         : (drop ? launch_bwd<false, true>(grid, st, mq, mk, mv, mdo, p)
                                 : launch_bwd<false, false>(grid, st, mq, mk, mv, mdo, p));
+  return rc ? rc : launched();
+}
+
+// delta[b][h][s] = sum_d dO * O (the backward's first pass on its own).  o, dout: [B, H, S, 64] with element
+// strides os / dos {batch, head, seq}; delta: [B][H][S] fp32.
+int b200dp_attn_delta(const void* o, const void* dout, float* delta, int B, int H, int S, int D, const long long* os,
+                      const long long* dos, unsigned long long stream) {
+  if (D != HD) return fail("head dim must be 64");
+  if (B < 1 || H < 1 || S < 1) return fail("attention shapes must be positive");
+  if ((os[0] % 8) || (os[1] % 8) || (os[2] % 8) || ((uintptr_t)o & 15) || (dos[0] % 8) || (dos[1] % 8) ||
+      (dos[2] % 8) || ((uintptr_t)dout & 15))
+    return fail("attention delta operands must be 16-byte aligned");
+  const long long rows = (long long)B * H * S;
+  attn_delta_kernel<<<(unsigned)((rows + 31) / 32), 256, 0, (cudaStream_t)(uintptr_t)stream>>>(
+      reinterpret_cast<const __nv_bfloat16*>(o), reinterpret_cast<const __nv_bfloat16*>(dout), delta, B, H, S, os[0],
+      os[1], os[2], dos[0], dos[1], dos[2]);
+  return launched();
+}
+
+// Sequence-parallel forward (see the header): rank `rank` of `world`, S = S_loc rows per rank (a multiple of 256).
+// q, o: this rank's [B, H, S, 64] shard, strides {batch, head, seq}; k, v: the gathered [W, B, H, S, 64] views,
+// strides {rank, batch, head, seq}; lse: [B][H][S] (nullptr: not saved).  No dropout.
+int b200dp_attn_sp_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int B, int H, int S, int D,
+                       const long long* qs, const long long* ks, const long long* vs, const long long* os, float scale,
+                       int causal, int rank, int world, unsigned long long stream) {
+  if (ensure_init()) return -1;
+  AttnFwdParams p;
+  if (check_sp(B, H, S, D, causal, rank, world, p)) return -1;
+  CUtensorMap mq, mk, mv;
+  if (make_qkv_map(&mq, q, B, H, S, qs[0], qs[1], qs[2]) || make_gathered_map(&mk, k, world, B, H, S, ks) ||
+      make_gathered_map(&mv, v, world, B, H, S, vs))
+    return -1;
+  if ((os[0] % 8) || (os[1] % 8) || (os[2] % 8) || ((uintptr_t)o & 15)) return fail("output must be 16-byte aligned");
+  p.q_tiles = S / TILE;                                  // local query tiles
+  p.kv_blocks = world * (S / TILE);                      // global key tiles
+  p.scale_log2 = scale * 1.4426950408889634f;
+  p.o = reinterpret_cast<__nv_bfloat16*>(o);
+  p.o_sb = os[0]; p.o_sh = os[1]; p.o_ss = os[2];
+  p.lse = lse;
+  const dim3 grid(B * H * p.q_tiles);
+  cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
+  const int rc = causal ? launch_fwd<true, false, true>(grid, st, mq, mk, mv, p)
+                        : launch_fwd<false, false, true>(grid, st, mq, mk, mv, p);
+  return rc ? rc : launched();
+}
+
+// Sequence-parallel backward: k, v, dk, dv: this rank's [B, H, S, 64] shard (strides {batch, head, seq}); q, dout:
+// gathered [W, B, H, S, 64] views (strides {rank, batch, head, seq}); lse, delta: gathered [W][B][H][S] fp32 with
+// rank stride ld_sw elements (delta from b200dp_attn_delta on each rank); dq_acc: fp32 [W, B, H, S, 64] workspace
+// (strides dqs {rank, batch, head, seq}, 64 contiguous) zeroed by the caller, which gets this rank's partial dQ of
+// every rank's queries.
+int b200dp_attn_sp_bwd(const void* q, const void* k, const void* v, const void* dout, const float* lse,
+                       const float* delta, float* dq_acc, void* dk, void* dv, int B, int H, int S, int D,
+                       const long long* qs, const long long* ks, const long long* vs, const long long* dos,
+                       const long long* dqs, const long long* dks, const long long* dvs, long long ld_sw, float scale,
+                       int causal, int rank, int world, unsigned long long stream) {
+  if (ensure_init()) return -1;
+  AttnBwdParams p;
+  if (check_sp(B, H, S, D, causal, rank, world, p)) return -1;
+  CUtensorMap mq, mk, mv, mdo;
+  if (make_gathered_map(&mq, q, world, B, H, S, qs) || make_qkv_map(&mk, k, B, H, S, ks[0], ks[1], ks[2]) ||
+      make_qkv_map(&mv, v, B, H, S, vs[0], vs[1], vs[2]) || make_gathered_map(&mdo, dout, world, B, H, S, dos))
+    return -1;
+  if ((dqs[0] % 4) || (dqs[1] % 4) || (dqs[2] % 4) || (dqs[3] % 4)) return fail("dq workspace strides must be multiples of 4");
+  if (ld_sw < (long long)B * H * S) return fail("lse / delta rank stride is shorter than one rank's rows");
+  p.q_tiles = world * (S / TILE);                        // global query tiles
+  p.kv_blocks = S / TILE;                                // local key blocks
+  p.scale = scale;
+  p.scale_log2 = scale * 1.4426950408889634f;
+  p.lse = lse; p.delta = delta; p.dq_acc = dq_acc;
+  p.lse_sw = ld_sw;
+  p.dq_sw = dqs[0]; p.dq_sb = dqs[1]; p.dq_sh = dqs[2]; p.dq_ss = dqs[3];
+  p.dk = reinterpret_cast<__nv_bfloat16*>(dk); p.dv = reinterpret_cast<__nv_bfloat16*>(dv);
+  p.dk_sb = dks[0]; p.dk_sh = dks[1]; p.dk_ss = dks[2];
+  p.dv_sb = dvs[0]; p.dv_sh = dvs[1]; p.dv_ss = dvs[2];
+  const dim3 grid(B * H * p.kv_blocks);
+  cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
+  const int rc = causal ? launch_bwd<true, false, true>(grid, st, mq, mk, mv, mdo, p)
+                        : launch_bwd<false, false, true>(grid, st, mq, mk, mv, mdo, p);
   return rc ? rc : launched();
 }
 

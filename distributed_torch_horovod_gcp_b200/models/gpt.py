@@ -10,6 +10,13 @@ N(0, 0.02) everywhere, with the residual projections (``proj``, ``fc2``) at 0.02
 value, as nanoGPT's ``dropout``: in training mode it drops the embedding sum, the attention probabilities and
 the output of each residual branch.  Nothing is dropped inside the fused MLP node.
 
+``sequence_parallel=True`` (world size > 1) splits each sequence across the ranks: ``forward`` takes this
+rank's zigzag shard of the tokens (``ops.seq_parallel.zigzag_shard``), looks the position embedding up at the
+shard's global positions, runs attention through ``sp_attention`` over every rank's keys and values, and
+returns this rank's logits or the mean loss over its own tokens.  With equal shards, averaging the gradients
+over the ranks (``DistributedOptimizer``) gives the full-sequence gradient.  At world size 1 the model is the
+same as without it.
+
 The MLP is the fused node's exact (erf) GELU, not GPT-2's tanh approximation, so weights trained by the
 original GPT-2 code would see a slightly different activation here.
 """
@@ -26,10 +33,13 @@ from .vit import EncoderBlock
 
 class GPT(nn.Module):
     def __init__(self, vocab: int = 50304, context: int = 1024, depth: int = 12, heads: int = 12,
-                 dim: int = 768, mlp_dim: int = 3072, dropout: float = 0.0):
+                 dim: int = 768, mlp_dim: int = 3072, dropout: float = 0.0, sequence_parallel: bool = False):
         super().__init__()
         if not 0.0 <= dropout <= 1.0:
             raise ValueError(f"dropout must be in [0, 1], got {dropout}")
+        if sequence_parallel and dropout > 0.0:
+            raise ValueError("dropout is not supported with sequence_parallel=True")
+        self.sequence_parallel = bool(sequence_parallel)
         self.vocab, self.context, self.dim = vocab, context, dim
         self.dropout = float(dropout)
         self.wte = nn.Embedding(vocab, dim)
@@ -51,22 +61,36 @@ class GPT(nn.Module):
         """``idx``: [B, S] int64 token ids, S <= context.  Without ``targets``: the logits [B * S, vocab] (rows
         in (b, s) order, ready for ``nn.CrossEntropyLoss`` against targets of shape [B * S]).  With ``targets``
         ([B, S] or [B * S]): the mean cross-entropy loss, through ``linear_cross_entropy`` on the LM head, which
-        never materialises the logits on the kernel path."""
+        never materialises the logits on the kernel path.  Under sequence parallelism ``idx`` and ``targets`` are
+        this rank's zigzag shards, and S the local length."""
         B, S = idx.shape
-        if S > self.context:
-            raise ValueError(f"sequence length {S} exceeds the model's context of {self.context}")
+        rank, world = self._sp_rank_world()
+        if S * world > self.context:
+            raise ValueError(f"sequence length {S * world} exceeds the model's context of {self.context}")
         # the token embedding is also the LM head: two uses, so its gradient is summed by autograd
         # rather than written straight into the gradient bucket by the LM head's GEMM
         grad_sink.note_forward(self.wte.weight)
-        x = self.wte(idx) + self.wpe.weight[:S]
+        if world > 1:
+            from ..ops.seq_parallel import zigzag_positions
+            x = self.wte(idx) + self.wpe.weight[zigzag_positions(S * world, rank, world, idx.device)]
+        else:
+            x = self.wte(idx) + self.wpe.weight[:S]
         if self.training and self.dropout > 0.0:
             x = F2.dropout_add(x, None, self.dropout)
         for blk in self.layers:
-            x = blk(x)
+            x = blk(x, sequence_parallel=True) if world > 1 else blk(x)
         x = F2.layer_norm(x, self.ln_f.weight, self.ln_f.bias, self.ln_f.eps)
         if targets is not None:
             return F2.linear_cross_entropy(x.reshape(B * S, self.dim), self.wte.weight, targets.reshape(-1))
         return F2.linear(x.reshape(B * S, self.dim), self.wte.weight)
+
+    def _sp_rank_world(self):
+        """(rank, world) of the sequence split: (0, 1) unless ``sequence_parallel`` with world size > 1."""
+        if not self.sequence_parallel:
+            return 0, 1
+        from .. import _state
+        rt = _state.runtime()
+        return (rt.rank, rt.size) if rt.initialized else (0, 1)
 
 
 def gpt2(**kw):

@@ -36,6 +36,10 @@ def register(lib, have):
     lib.b200dp_attn_bwd.argtypes = [vp] * 10 + [i, i, i, i] + [lp] * 8 + [f, i, u64]
     lib.b200dp_attn_fwd_dropout.argtypes = [vp, vp, vp, vp, vp, i, i, i, i, lp, lp, lp, lp, f, i, vp, f, u64]
     lib.b200dp_attn_bwd_dropout.argtypes = [vp] * 10 + [i, i, i, i] + [lp] * 8 + [f, i, vp, f, u64]
+    if hasattr(lib, "b200dp_attn_sp_fwd"):           # sequence parallelism (ops/seq_parallel.py)
+        lib.b200dp_attn_delta.argtypes = [vp, vp, vp, i, i, i, i, lp, lp, u64]
+        lib.b200dp_attn_sp_fwd.argtypes = [vp] * 5 + [i] * 4 + [lp] * 4 + [f, i, i, i, u64]
+        lib.b200dp_attn_sp_bwd.argtypes = [vp] * 9 + [i] * 4 + [lp] * 7 + [ctypes.c_longlong, f, i, i, i, u64]
     lib.b200dp_attn_last_error.restype = ctypes.c_char_p
     if hasattr(lib, "b200dp_cast_acc_zero"):
         lib.b200dp_cast_acc_zero.argtypes = [vp, vp, ctypes.c_longlong, i, i, i, u64]

@@ -159,12 +159,17 @@ def attention(qkv, heads: int, causal: bool = False, dropout_p: float = 0.0):
     return attention_reference(qkv, heads, causal, dropout_p)
 
 
-def qkv_attention(x, weight, bias, heads: int, causal: bool = False, dropout_p: float = 0.0):
+def qkv_attention(x, weight, bias, heads: int, causal: bool = False, dropout_p: float = 0.0,
+                  sequence_parallel: bool = False):
     """Multi-head self-attention input stage: packed QKV projection + scaled-dot-product attention
     (``causal=True``: position i attends to positions 0..i only, as in a decoder; ``dropout_p``: dropout on
     the attention probabilities, drawn inside the flash-attention kernels on the kernel path).
-    Kernel path: q, k, v are produced as three dense matrices (no un-pack / re-pack copies)."""
+    Kernel path: q, k, v are produced as three dense matrices (no un-pack / re-pack copies).
+    ``sequence_parallel=True``: ``x`` is this rank's zigzag shard of the sequence and attention runs through
+    ``seq_parallel.sp_attention`` over every rank's keys and values."""
     dropout_p = _check_p(dropout_p)
+    if sequence_parallel:
+        return _sp_qkv_attention(x, weight, bias, heads, causal, dropout_p)
     k = _kernels(x)
     if k is not None and k.has("linear") and k.linear_supported(x, weight, bias) and x.dim() == 3 \
             and weight.shape[0] == 3 * x.shape[-1] and weight.shape[0] % 24 == 0 and x.shape[-1] % heads == 0 \
@@ -181,6 +186,19 @@ def qkv_attention(x, weight, bias, heads: int, causal: bool = False, dropout_p: 
         o = F.scaled_dot_product_attention(q, kk, v, dropout_p=dropout_p, is_causal=causal)
         return o.transpose(1, 2).reshape(B, S, D)
     return attention(linear(x, weight, bias), heads, causal, dropout_p)
+
+
+def _sp_qkv_attention(x, weight, bias, heads, causal, dropout_p):
+    from .seq_parallel import sp_attention
+    B, S, D = x.shape
+    hd = D // heads
+    k = _kernels(x)
+    if k is not None and k.has("linear") and k.linear_supported(x, weight, bias) and weight.shape[0] == 3 * D \
+            and weight.shape[0] % 24 == 0 and D % heads == 0:
+        q, kk, v = [t.view(B, S, heads, hd).transpose(1, 2) for t in k.qkv_proj(x, weight, bias)]
+    else:
+        q, kk, v = linear(x, weight, bias).view(B, S, 3, heads, hd).permute(2, 0, 3, 1, 4)
+    return sp_attention(q, kk, v, causal, dropout_p).transpose(1, 2).reshape(B, S, D)
 
 
 # ------------------------------------------------------------------ LM head + cross-entropy
