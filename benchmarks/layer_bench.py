@@ -33,7 +33,7 @@ def main():
     ap.add_argument("--out", default=None, help="also write the rows to this JSON file")
     args = ap.parse_args()
     from distributed_torch_horovod_gcp_b200.models import resnet50
-    from distributed_torch_horovod_gcp_b200.ops import kernels, bn as B
+    from distributed_torch_horovod_gcp_b200.ops import kernels, conv as CV
     assert kernels.has("conv_implicit_gemm")
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     hbm, tf = 3350.0, 989.0      # H100 SXM data sheet (not measured); MEASURED_PEAKS.json overrides
@@ -87,7 +87,7 @@ def main():
         stats = torch.zeros(2 * co, dtype=torch.float32, device=dev)
         def fwd():
             stats.zero_()
-            return B.conv2d(x, conv, stats=stats)[0]
+            return CV.conv2d(x, conv, stats=stats)
         y = fwd()
         dy = torch.randn_like(y)
         oh = y.shape[2]

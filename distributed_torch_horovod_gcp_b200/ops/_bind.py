@@ -17,7 +17,7 @@ from .attention import attention_fused  # noqa: F401
 from .dropout import dropout_add  # noqa: F401
 from .xent import linear_cross_entropy  # noqa: F401
 from .lstm_rec import lstm_recurrent  # noqa: F401
-from .conv import conv3x3, conv2d as conv2d_implicit  # noqa: F401
+from .conv import conv3x3, conv2d_implicit  # noqa: F401
 from .ln import layer_norm  # noqa: F401
 from .gemm import linear, mlp, qkv_proj  # noqa: F401  (re-exported as kernels.linear / .mlp / .qkv_proj)
 from .bn import conv_bn_act, bn_act, max_pool_3x3_s2, global_avg_pool  # noqa: F401

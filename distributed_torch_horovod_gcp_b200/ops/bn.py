@@ -1,8 +1,5 @@
-"""Fused NHWC BatchNorm(+residual)(+ReLU) (csrc/elementwise.cu) and the conv+BN+act unit used by
-the ResNet blocks.  1x1 stride-1 convolutions run on the wgmma GEMM (an NHWC activation is a
-row-major [N*H*W, C] matrix), the 7x7 stem on im2col + that GEMM, and 3x3 / strided 1x1 convolutions
-on the implicit-GEMM kernel (ops/conv.py, csrc/conv_sm90.cu); cuDNN is only the fallback for shapes
-none of these cover (e.g. a 3-channel 3x3 stem).
+"""Fused NHWC BatchNorm(+residual)(+ReLU), max / average pooling (csrc/elementwise.cu) and the conv+BN+act unit
+used by the ResNet blocks, whose convolution runs on the kernel ``ops.conv.kind`` chooses.
 
 The batch-statistics reductions (here and in the producing GEMM / convolution epilogue) sum per-CTA
 partials in a fixed order through one per-library set of slots, so they are bit-reproducible but must
@@ -17,11 +14,9 @@ import torch
 import torch.nn.functional as F
 
 from . import counters
-from . import gemm as _gemm
 from . import grad_sink
 
 _lib = None
-_USE_GEMM_1X1 = os.environ.get("B200DP_CONV1X1_GEMM", "1") == "1"
 
 
 def register(lib, have):
@@ -61,7 +56,9 @@ def _ck(rc):
 
 
 def _nhwc_ok(x: torch.Tensor) -> bool:
-    return x.dim() == 4 and x.dtype == torch.bfloat16 and \
+    """An activation the NHWC kernels take as it is: a dense channels_last bf16 CUDA tensor with a 16-byte
+    aligned base."""
+    return x.dim() == 4 and x.dtype == torch.bfloat16 and x.is_cuda and \
         x.is_contiguous(memory_format=torch.channels_last) and x.data_ptr() % 16 == 0
 
 
@@ -213,87 +210,7 @@ def bn_act(x, bn: torch.nn.BatchNorm2d, relu: bool, residual: Optional[torch.Ten
     return y
 
 
-def _is_gemm_conv(x, conv) -> bool:
-    w = conv.weight
-    return (_USE_GEMM_1X1 and _gemm._lib is not None and conv.kernel_size == (1, 1)
-            and conv.stride == (1, 1) and conv.padding == (0, 0) and conv.groups == 1
-            and conv.bias is None and w.dtype == torch.bfloat16 and _nhwc_ok(x)
-            and w.shape[0] % 8 == 0 and w.shape[1] % 8 == 0)
-
-
-_USE_STEM_GEMM = os.environ.get("B200DP_STEM_GEMM", "1") == "1"
-STEM_KP = 168          # k = kh*24 + kw*3 + c (21 real + 3 zero-weighted columns per kernel row)
-
-
-class _StemConvFn(torch.autograd.Function):
-    """ResNet stem (7x7, stride 2, pad 3, 3 input channels) as im2col + wgmma GEMM.  The im2col
-    matrix ([N*112*112, 168] bf16, about 1 GB at batch 256) is kept for the weight gradient instead
-    of being rebuilt: it fits easily in an 80 GB H100, and HBM bandwidth, not capacity, bounds
-    the step."""
-
-    @staticmethod
-    def forward(ctx, x, weight, stats=None):
-        N, C, H, W = x.shape
-        OH, OW = H // 2, W // 2
-        M = N * OH * OW
-        cols = torch.empty((M, STEM_KP), dtype=torch.bfloat16, device=x.device)
-        _ck(_lib.b200dp_stem_im2col(x.data_ptr(), cols.data_ptr(), N, H, W,
-                                    torch.cuda.current_stream(x.device).cuda_stream))
-        counters.bump("stem_im2col")
-        Cout = weight.shape[0]
-        wp = torch.zeros((Cout, 7, 24), dtype=torch.bfloat16, device=x.device)
-        wp[:, :, :21] = weight.permute(0, 2, 3, 1).reshape(Cout, 7, 21)  # [Cout][kh][kw*3 + c]
-        wp = wp.view(Cout, STEM_KP)
-        y = torch.empty((M, Cout), dtype=torch.bfloat16, device=x.device)
-        _gemm.gemm(cols, wp, y, M, Cout, STEM_KP, stats=stats)
-        ctx.save_for_backward(cols)
-        ctx.wshape = weight.shape
-        return y.view(N, OH, OW, Cout).permute(0, 3, 1, 2)
-
-    @staticmethod
-    def backward(ctx, dy):
-        (cols,) = ctx.saved_tensors
-        Cout = ctx.wshape[0]
-        M = cols.shape[0]
-        dy2 = dy.permute(0, 2, 3, 1).reshape(M, Cout)
-        if not dy2.is_contiguous():
-            dy2 = dy2.contiguous()
-        acc = torch.zeros((Cout, STEM_KP), dtype=torch.float32, device=dy.device)
-        _gemm.gemm(dy2, cols, acc, Cout, STEM_KP, M, a_mn=True, b_mn=True, out_mode=1,
-                   splits=_gemm._splits_for(Cout, STEM_KP, M))
-        dw = acc.view(Cout, 7, 24)[:, :, :21].reshape(Cout, 7, 7, 3).permute(0, 3, 1, 2).to(torch.bfloat16)
-        return None, dw.contiguous(memory_format=torch.channels_last), None
-
-
-def _is_stem_conv(x, conv) -> bool:
-    return (_USE_STEM_GEMM and _gemm._lib is not None and hasattr(_lib, "b200dp_stem_im2col")
-            and conv.kernel_size == (7, 7) and conv.stride == (2, 2) and conv.padding == (3, 3)
-            and conv.groups == 1 and conv.bias is None and conv.in_channels == 3
-            and conv.weight.dtype == torch.bfloat16 and _nhwc_ok(x) and not x.requires_grad
-            and x.shape[2] % 2 == 0 and x.shape[3] % 8 == 0 and conv.out_channels % 8 == 0)
-
-
 _FUSE_STATS = os.environ.get("B200DP_BN_STATS_IN_EPILOGUE", "1") == "1"
-
-
-def conv2d(x, conv: torch.nn.Conv2d, stats=None):
-    """Convolution of an NHWC bf16 activation; 1x1/stride-1 and the 7x7 stem -> wgmma GEMM, 3x3 and
-    strided 1x1 -> implicit-GEMM kernel.  Returns ``(y, stats_filled)``: when ``stats`` (fp32 [2*Cout]
-    accumulator) is given and the kernel that ran supports it, its epilogue has added the output's
-    per-channel sum / sum of squares."""
-    w = conv.weight
-    if _is_gemm_conv(x, conv):
-        N, C, H, W = x.shape
-        x2 = x.permute(0, 2, 3, 1).reshape(N * H * W, C)             # view: NHWC rows
-        y2 = _gemm.linear(x2, w.reshape(w.shape[0], C), owner=w, stats=stats)     # [M, Cout]
-        return y2.view(N, H, W, w.shape[0]).permute(0, 3, 1, 2), stats is not None   # logical NCHW, NHWC memory
-    if _is_stem_conv(x, conv):
-        return _StemConvFn.apply(x, w, stats), stats is not None
-    from . import conv as _conv
-    if conv.bias is None and _conv.supported(x, w, conv.stride, conv.padding, conv.dilation, conv.groups):
-        return _conv.conv2d(x, w, conv.stride[0], conv.padding[0], stats), stats is not None
-    b = conv.bias.to(x.dtype) if conv.bias is not None else None
-    return F.conv2d(x, w.to(x.dtype), b, conv.stride, conv.padding, conv.dilation, conv.groups), False
 
 
 def _stats_buffer(bn, C: int, device):
@@ -311,11 +228,12 @@ def fused_stats(bn, C: int, device) -> Optional[torch.Tensor]:
     return _stats_buffer(bn, C, device) if _FUSE_STATS and bn.training and C <= 2048 else None
 
 
-def _out_rows(x, conv) -> int:
-    """N * OH * OW of the convolution's output."""
+def _out_shape(x, conv):
+    """The shape [N, Cout, OH, OW] of the convolution's output."""
     N, _, H, W = x.shape
     (R, S), (sh, sw), (ph, pw), (dh, dw) = conv.kernel_size, conv.stride, conv.padding, conv.dilation
-    return N * max((H + 2 * ph - dh * (R - 1) - 1) // sh + 1, 0) * max((W + 2 * pw - dw * (S - 1) - 1) // sw + 1, 0)
+    return (N, conv.out_channels, max((H + 2 * ph - dh * (R - 1) - 1) // sh + 1, 0),
+            max((W + 2 * pw - dw * (S - 1) - 1) // sw + 1, 0))
 
 
 def _wants_grad(*ts) -> bool:
@@ -323,19 +241,18 @@ def _wants_grad(*ts) -> bool:
 
 
 def conv_bn_act(x, conv, bn, relu: bool, residual=None):
+    from . import conv as _conv
     C = conv.out_channels
-    fused_bn = x.dim() == 4 and isinstance(conv.padding, tuple) and module_ok(bn, C, _out_rows(x, conv)) and \
-        (residual is None or residual.dtype == torch.bfloat16)
-    stats = fused_stats(bn, C, x.device) if fused_bn and x.dtype == torch.bfloat16 else None
-    y, filled = conv2d(x, conv, stats=stats)
-    if stats is not None and not filled:
-        stats = None
+    shape = _out_shape(x, conv) if x.dim() == 4 and isinstance(conv.padding, tuple) else None
     # eval mode: the fused apply pass is no autograd node, so only where nothing needs a gradient
-    if fused_bn and bn_supported(y, C) and (residual is None or residual.shape == y.shape) and \
-            (bn.training or not _wants_grad(y, residual, bn.weight, bn.bias)):
+    fused_bn = shape is not None and module_ok(bn, C, shape[0] * shape[2] * shape[3]) and \
+        (residual is None or (residual.dtype == torch.bfloat16 and residual.shape == shape)) and \
+        (bn.training or not _wants_grad(x, conv.weight, conv.bias, residual, bn.weight, bn.bias))
+    # a kernel's output is a fresh NHWC bf16 tensor, which the fused BN takes: it consumes these statistics
+    stats = fused_stats(bn, C, x.device) if fused_bn and _conv.kind(x, conv) is not None else None
+    y = _conv.conv2d(x, conv, stats)
+    if fused_bn and bn_supported(y, C):
         return bn_act(y, bn, relu, residual, stats=stats)
-    if stats is not None:
-        stats.zero_()          # filled but not consumed by the fused BN: keep the accumulator clean
     y = bn(y)
     if residual is not None:
         y = y + residual

@@ -13,7 +13,6 @@ import torch
 
 from . import bn as _bn
 from . import conv as _conv
-from . import gemm as _gemm
 from . import grad_sink
 
 
@@ -25,43 +24,29 @@ def _units(block):
 
 def supported(x: torch.Tensor, block) -> bool:
     """NHWC bf16 ``x``; every BN in training mode and on the fused kernels (``ops.bn.module_ok``); conv1 and
-    conv3 on the 1x1 GEMM, conv2 and the downsample on the GEMM or the implicit-GEMM kernel.  The
-    activations inside the block are fresh NHWC bf16 tensors like ``x``, so ``x`` stands in for them."""
+    conv3 on the 1x1 GEMM, conv2 and the downsample on the GEMM or the implicit-GEMM kernel (``ops.conv.kind``).
+    The activations inside the block are fresh NHWC bf16 tensors like ``x``, so ``x`` stands in for them."""
     if _bn._lib is None or not _bn._nhwc_ok(x):
         return False
     rows1 = x.shape[0] * x.shape[2] * x.shape[3]
-    rows2 = _bn._out_rows(x, block.conv2)           # conv2, the downsample and conv3 share its output grid
+    N, _, OH, OW = _bn._out_shape(x, block.conv2)   # conv2, the downsample and conv3 share its output grid
+    rows2 = N * OH * OW
     for conv, bn in _units(block):
         if not (bn.training and _bn.module_ok(bn, conv.out_channels, rows1 if conv is block.conv1 else rows2)):
             return False
-        if not _bn._is_gemm_conv(x, conv) and (conv in (block.conv1, block.conv3) or conv.bias is not None or
-                                               not _conv.supported(x, conv.weight, conv.stride, conv.padding,
-                                                                   conv.dilation, conv.groups)):
+        k = _conv.kind(x, conv)
+        if k != "gemm" and (conv in (block.conv1, block.conv3) or k != "implicit"):
             return False
     return True
 
 
-def _rows(t: torch.Tensor) -> torch.Tensor:
-    """A channels_last [N, C, H, W] activation as its [N*H*W, C] matrix (a view)."""
-    N, C, H, W = t.shape
-    return t.permute(0, 2, 3, 1).reshape(N * H * W, C)
-
-
-def _unit_forward(x, conv, bn, relu, residual, need):
-    """conv + BN(+residual)(+ReLU); ``need``: whether the conv weight, γ and β need gradients.  Returns the
-    output and (conv input, weight as the kernel reads it, BN input, ReLU sign bits, mean, invstd, a)."""
-    C = conv.out_channels
-    stats = _bn.fused_stats(bn, C, x.device)
+def _unit_forward(x, conv, bn, k, relu, residual, need):
+    """conv (of kind ``k``) + BN(+residual)(+ReLU); ``need``: whether the conv weight, γ and β need gradients.
+    Returns the output and (conv input, weight as the kernel reads it, BN input, ReLU sign bits, mean, invstd, a)."""
+    stats = _bn.fused_stats(bn, conv.out_channels, x.device)
     if need[0]:
         grad_sink.note_forward(conv.weight)
-    if _bn._is_gemm_conv(x, conv):              # 1x1 stride 1: the GEMM on the NHWC rows
-        N, _, H, W = x.shape
-        w = conv.weight.reshape(C, x.shape[1])
-        y = _gemm.gemm(_rows(x), w, torch.empty((N * H * W, C), dtype=torch.bfloat16, device=x.device),
-                       N * H * W, C, x.shape[1], stats=stats).view(N, H, W, C).permute(0, 3, 1, 2)
-    else:
-        w = _conv._krsc(conv.weight)
-        y = _conv.conv_fprop(x, w, conv.stride[0], conv.padding[0], stats)
+    y, w, _ = _conv.forward(x, conv.weight, k, conv.stride[0], conv.padding[0], stats)
     out, mask, ws = _bn.bn_forward(y, bn, residual, relu, stats, need[1:])
     return out, (x, w, y, mask, *ws)
 
@@ -73,10 +58,11 @@ class _BottleneckFn(torch.autograd.Function):
     def forward(ctx, block, x, *params):
         units = _units(block)
         need = [ctx.needs_input_grad[2 + 3 * i:5 + 3 * i] for i in range(len(units))]
-        h, s1 = _unit_forward(x, *units[0], True, None, need[0])
-        h, s2 = _unit_forward(h, *units[1], True, None, need[1])
-        identity, sd = _unit_forward(x, *units[2], False, None, need[2]) if len(units) == 4 else (x, ())
-        y, s3 = _unit_forward(h, *units[-1], True, identity, need[-1])
+        k = ctx.kinds = [_conv.kind(x, conv) for conv, _ in units]
+        h, s1 = _unit_forward(x, *units[0], k[0], True, None, need[0])
+        h, s2 = _unit_forward(h, *units[1], k[1], True, None, need[1])
+        identity, sd = _unit_forward(x, *units[2], k[2], False, None, need[2]) if len(units) == 4 else (x, ())
+        y, s3 = _unit_forward(h, *units[-1], k[-1], True, identity, need[-1])
         ctx.save_for_backward(*s1, *s2, *sd, *s3)
         ctx.block = block
         return y
@@ -90,28 +76,18 @@ class _BottleneckFn(torch.autograd.Function):
 
         def unit(i, dout, mask, want_dx, residual=None, res_mask=None):
             """BN backward applying ``mask``, then the conv's dgrad (+ ``residual``; GEMM only) and wgrad."""
-            (conv, bn), (x, w, y, _, *ws), need_dw = units[i], saved[i], need[2 + 3 * i]
+            (conv, bn), (x, w, y, _, *ws), k = units[i], saved[i], ctx.kinds[i]
+            stride, pad = conv.stride[0], conv.padding[0]
             dz, dgamma, dbeta, _ = _bn.bn_backward(dout, bn, y, mask, ws)
-            dx = dw = None
-            if w.dim() == 2:
-                N, C, H, W = x.shape
-                if want_dx:
-                    dx = _gemm.dgrad(_rows(dz), w, residual, res_mask).view(N, H, W, C).permute(0, 3, 1, 2)
-                if need_dw:
-                    dw = _gemm.wgrad(_rows(dz), _rows(x), w.shape[0], C, N * H * W, w.dtype, owner=conv.weight)
-                    dw = dw.view(conv.weight.shape) if dw is not None else None
-            else:
-                if want_dx:
-                    dx = _conv.conv_dgrad(dz, w, x.shape, conv.stride[0], conv.padding[0])
-                if need_dw:
-                    dw = _conv.conv_wgrad(dz, x, conv.weight, conv.stride[0], conv.padding[0])
+            dx = _conv.dgrad(dz, w, k, x.shape, stride, pad, residual, res_mask) if want_dx else None
+            dw = _conv.wgrad(dz, x, conv.weight, k, stride, pad) if need[2 + 3 * i] else None
             grads[i] = (dw, dgamma, dbeta)
             return dx
 
         dy, mask3 = _bn._cl(dy), saved[-1][3]
         d = unit(1, unit(n - 1, dy, mask3, True), saved[1][3], True)
         skip, skip_mask = (unit(2, dy, mask3, need[1]), None) if n == 4 else (dy, mask3)
-        dx = unit(0, d, saved[0][3], need[1], _rows(skip) if need[1] else None, skip_mask)
+        dx = unit(0, d, saved[0][3], need[1], skip, skip_mask)
         return (None, dx) + tuple(g for unit_grads in grads for g in unit_grads)
 
 

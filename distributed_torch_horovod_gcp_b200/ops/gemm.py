@@ -180,11 +180,10 @@ def dgrad(dz: torch.Tensor, weight: torch.Tensor, residual: Optional[torch.Tenso
 
 class _LinearFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, weight, bias, act, residual, owner=None, stats=None):
+    def forward(ctx, x, weight, bias, act, residual):
         K = weight.shape[1]
-        ctx.owner = owner if owner is not None else weight
         if ctx.needs_input_grad[1]:
-            grad_sink.note_forward(ctx.owner)
+            grad_sink.note_forward(weight)
         N = weight.shape[0]
         x2 = x.reshape(-1, K)
         if x2.stride(-1) != 1 or (x2.stride(0) % 8) or (x2.data_ptr() % 16):
@@ -196,7 +195,7 @@ class _LinearFn(torch.autograd.Function):
         r2 = None
         if residual is not None:
             r2 = _dense(residual.reshape(-1, N))
-        gemm(x2, weight, y, M, N, K, bias=bias, residual=r2, preact=z, act=act, stats=stats)
+        gemm(x2, weight, y, M, N, K, bias=bias, residual=r2, preact=z, act=act)
         ctx.save_for_backward(x2, weight, z)
         ctx.act, ctx.has_bias, ctx.has_res = act, bias is not None, residual is not None
         ctx.x_shape = x.shape
@@ -218,10 +217,10 @@ class _LinearFn(torch.autograd.Function):
         if ctx.needs_input_grad[0]:
             dx = dgrad(dz, weight).view(ctx.x_shape)                       # dx = dz @ W
         if ctx.needs_input_grad[1]:
-            dw = wgrad(dz, x2, N, K, M, weight.dtype, owner=ctx.owner)     # dW = dz^T @ x
+            dw = wgrad(dz, x2, N, K, M, weight.dtype, owner=weight)        # dW = dz^T @ x
         if ctx.has_bias and ctx.needs_input_grad[2]:
             db = bias_grad(dz, N, M, ctx.bias_dtype)
-        return dx, dw, db, None, dres, None, None
+        return dx, dw, db, None, dres
 
 
 def act_backward(dy2: torch.Tensor, z: torch.Tensor, act: int) -> torch.Tensor:
@@ -339,7 +338,5 @@ def qkv_proj(x, weight, bias):
     return _QKVFn.apply(x, weight, bias)
 
 
-def linear(x, weight, bias=None, act: Optional[str] = None, residual=None, owner=None, stats=None):
-    """``owner``: the parameter whose storage ``weight`` is a 2D view of (a 1x1 conv weight), so the
-    weight gradient can be written into its gradient-bucket slot directly."""
-    return _LinearFn.apply(x, weight, bias, ACT[act], residual, owner, stats)
+def linear(x, weight, bias=None, act: Optional[str] = None, residual=None):
+    return _LinearFn.apply(x, weight, bias, ACT[act], residual)

@@ -894,7 +894,7 @@ def _dgrad_of(spy, weight):
 @pytest.mark.parametrize("kind,planes,batch,hw", [("identity", 16, 3, 7), ("proj_s1", 64, 3, 7),
                                                   ("proj_s2", 16, 3, 14), ("proj_s2", 64, 2, 2)])
 def test_per_op_chain_stages(kind, planes, batch, hw, monkeypatch):
-    """The same blocks through ``conv_bn_act`` (``_LinearFn`` for the 1x1 stride-1 convolutions, ``_ConvFn``,
+    """The same blocks through ``conv_bn_act`` (``_ConvFn`` on the 1x1 GEMM and the implicit-GEMM kernel,
     ``_BNActFn``): every launch against float64, bn3's dres is its masked dy, the downsample BN reads that dres, and
     x.grad is autograd's bf16 sum of conv1's dgrad and the skip gradient."""
     from distributed_torch_horovod_gcp_b200.ops import functional as F2

@@ -486,11 +486,11 @@ def _state(bn):
 
 
 def _torch_bn_unit(x, conv, bn, relu, residual=None):
-    """What ``conv_bn_act`` means when its BatchNorm is not on the kernels: the convolution as ``ops.bn.conv2d``
+    """What ``conv_bn_act`` means when its BatchNorm is not on the kernels: the convolution as ``ops.conv.conv2d``
     runs it (the implicit-GEMM / 1x1 GEMM kernels for bf16 NHWC, else ``F.conv2d``), then the torch module."""
-    from distributed_torch_horovod_gcp_b200.ops import bn as B
+    from distributed_torch_horovod_gcp_b200.ops import conv as CV
     if x.dtype == BF16 and x.is_contiguous(memory_format=torch.channels_last):
-        y = bn(B.conv2d(x, conv)[0])
+        y = bn(CV.conv2d(x, conv))
     else:
         y = bn(F.conv2d(x, conv.weight.to(x.dtype), None, conv.stride, conv.padding))
     if residual is not None:
@@ -575,12 +575,12 @@ def test_conv_bn_act_reference_path(cid, bkw, res, train, xf, env):
     _same_sides(sides)
     if cid == "momentum-None":
         # the cumulative average, mom = 1 / num_batches_tracked at every step, against float64 of each batch
-        from distributed_torch_horovod_gcp_b200.ops import bn as B
+        from distributed_torch_horovod_gcp_b200.ops import conv as CV
         rm0, rv0 = [t.double() for t in _state(_bn(C, seed=62, **bkw))[:2]]
         for s, (out, grads, state, args) in enumerate(sides[0]):
             assert int(state[2]) == s + 1
             with torch.no_grad():
-                y2 = B.conv2d(args[0].detach(), conv)[0].permute(0, 2, 3, 1).reshape(-1, C)
+                y2 = CV.conv2d(args[0].detach(), conv).permute(0, 2, 3, 1).reshape(-1, C)
             m, var, _, Em, Evar, _ = bn_stat_bounds(y2, D=y2.shape[0])
             rm, Erm, rv, Erv = running_stats_bounds(rm0, rv0, m, var, Em, Evar, y2.shape[0], 1.0 / (s + 1), False)
             assert_within_bound(state[0], rm, group="momentum=None running_mean", terms=[(1.0, Erm)])

@@ -190,15 +190,15 @@ def test_maxpool_matches_torch():
 
 
 def test_stem_conv_matches_cudnn():
-    from distributed_torch_horovod_gcp_b200.ops import kernels, bn as B
+    from distributed_torch_horovod_gcp_b200.ops import kernels, conv as CV
     assert kernels.has("stem_conv")
     torch.manual_seed(8)
     conv = torch.nn.Conv2d(3, 64, 7, 2, 3, bias=False).cuda().to(torch.bfloat16).to(
         memory_format=torch.channels_last)
     x = torch.randn(4, 3, 64, 96, device="cuda").to(torch.bfloat16).contiguous(
         memory_format=torch.channels_last)
-    assert B._is_stem_conv(x, conv)
-    y = B.conv2d(x, conv)[0]
+    assert CV.kind(x, conv) == "stem"
+    y = CV.conv2d(x, conv)
     ref = torch.nn.functional.conv2d(x.float(), conv.weight.float(), None, 2, 3)
     assert y.shape == ref.shape and _rel(y, ref) < 6e-3
     gy = torch.randn_like(y)

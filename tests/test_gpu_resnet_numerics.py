@@ -620,7 +620,7 @@ def _run_bn_train(x, bn, res, relu, src):
     """The training forward with statistics from the stand-alone pass, or from the epilogue of a 1x1 (GEMM) or 3x3
     (implicit-GEMM) convolution whose weights pass x through unchanged (y = bf16(x * 1) = x), as conv_bn_act runs
     it.  Returns the BN output, its mask bits, the saved (mean, invstd, a), and the depth of the statistics sums."""
-    from distributed_torch_horovod_gcp_b200.ops import bn as B
+    from distributed_torch_horovod_gcp_b200.ops import bn as B, conv as CV
     N, C, H, W = x.shape
     M = N * H * W
     if src == "standalone":
@@ -635,8 +635,9 @@ def _run_bn_train(x, bn, res, relu, src):
     stats = B.fused_stats(bn, C, x.device)
     assert stats is not None
     before = stats.clone()
-    y0, filled = B.conv2d(x, conv, stats=stats)
-    assert filled and bool((stats != before).any() or M == 0)
+    assert CV.kind(x, conv) == ("gemm" if src == "gemm" else "implicit")
+    y0 = CV.conv2d(x, conv, stats=stats)
+    assert bool((stats != before).any() or M == 0)
     assert torch.equal(y0, x), "pass-through convolution changed its input"
     y, mask, ws = B.bn_forward(y0.contiguous(memory_format=torch.channels_last), bn, res, relu, stats_in=stats)
     assert float(stats.abs().max()) == 0.0, "bn_finalize did not re-zero the epilogue accumulator"
@@ -899,20 +900,20 @@ def test_stem_im2col_and_gemm_vs_fp64(N, H, W):
     bit.  Output: a GEMM over 168 columns (three zero-weighted per kernel row, K zero-filled to 192), bf16 store.
     Weight gradient: split-K fp32 sums of 64 ceil(M / 64) products per split, s splits added to a zeroed buffer,
     then one bf16 rounding."""
-    from distributed_torch_horovod_gcp_b200.ops import bn as B, gemm as G
+    from distributed_torch_horovod_gcp_b200.ops import conv as CV, gemm as G
     lib = _bn_lib()
     g = torch.Generator(device="cuda").manual_seed(N * H * W)
     x = _nhwc(torch.randn(N, 3, H, W, device="cuda", generator=g))
     OH, OW = H // 2, W // 2
     M = N * OH * OW
-    cols = torch.empty(M, B.STEM_KP, device="cuda", dtype=torch.bfloat16)
+    cols = torch.empty(M, CV.STEM_KP, device="cuda", dtype=torch.bfloat16)
     assert lib.b200dp_stem_im2col(x.data_ptr(), cols.data_ptr(), N, H, W, _stream()) == 0
     torch.cuda.synchronize()
     ref = F.unfold(x.float(), 7, padding=3, stride=2).view(N, 3, 7, 7, OH * OW)      # [n, c, kh, kw, l]
     ref = ref.permute(0, 4, 2, 3, 1).reshape(M, 7, 21).bfloat16()
     assert torch.equal(cols.view(M, 7, 24)[:, :, :21], ref), "stem im2col differs from unfold"
     w = _nhwc(torch.randn(64, 3, 7, 7, device="cuda", generator=g) * 0.1).requires_grad_(True)
-    y = B._StemConvFn.apply(x, w, None)
+    y = CV._ConvFn.apply(x, w, "stem", 2, 3)
     dy = torch.randn(y.shape, device="cuda", generator=g).bfloat16()
     y.backward(dy)
     torch.cuda.synchronize()
@@ -921,7 +922,7 @@ def test_stem_im2col_and_gemm_vs_fp64(N, H, W):
     gw = torch.nn.grad.conv2d_weight
     dw64 = gw(x.double(), w.shape, dy.double(), 2, 3)
     dwm = gw(x.double().abs(), w.shape, dy.double().abs(), 2, 3)
-    s = G._splits_for(64, B.STEM_KP, M)
+    s = G._splits_for(64, CV.STEM_KP, M)
     _check(w.grad, dw64, bf16_store(2 * (_pad64(M) + s + 1) * U32 * dwm, dw64), "stem wgrad")
 
 
