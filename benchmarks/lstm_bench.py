@@ -49,13 +49,12 @@ def time_ms(fn, iters, warmup):
 
 
 def fwd_bwd(model, x, g):
+    from distributed_torch_horovod_gcp_b200.ops import functional as F2
+    lstm = F2.lstm_reference if model._fused is False else F2.lstm
+
     def run():
         h = model.init_hidden(x.shape[0])
-        if model._fused is False:
-            seq, _ = model.lstm(x, h)
-        else:
-            from distributed_torch_horovod_gcp_b200.ops import lstm_fused
-            seq, _ = lstm_fused.recurrence(model, x, h)
+        seq, _ = lstm(x, model.lstm, h)
         seq.backward(g)
     return run
 

@@ -11,13 +11,14 @@ moves the same 10 tensors / 1 480 196 bytes.
 H100-first changes (SURVEY.md §2.6 S2/S4, §7.3):
   * ``(h0, c0)`` come from the device generator (no CPU randn + pageable H2D + sync per
     step), the last-step gather is a slice (no host-built index tensor);
-  * on CUDA (fp32, hidden size 256, any number of layers, one or two directions, 1..512 input
-    features, inter-layer dropout in [0, 1]) forward/backward run on the persistent cluster LSTM
-    kernels (K5: ``ops/lstm_rec.py``, csrc/lstm_rec_sm90.cu — tf32 wgmma, W_hh resident in shared memory, h exchanged through
-    DSMEM; the two directions of a layer run as separate clusters of one launch) and, for batches
-    up to 1024, the chained-GEMM head (K6: ``ops/lstm_fused.py``; larger batches use torch's
-    linears).  Other hidden sizes, wider inputs and non-fp32 weights use cuDNN / cuBLAS, which is
-    also the numerics oracle.
+  * the recurrence and the head are ``ops.functional.lstm`` and ``ops.functional.lstm_head``, each of
+    which chooses its kernel.  On an sm_90 device (fp32, hidden size 256, any number of layers, one or two
+    directions, 1..512 input features, inter-layer dropout in [0, 1]) forward/backward run on the persistent
+    cluster LSTM kernels (K5: ``ops/lstm_rec.py``, csrc/lstm_rec_sm90.cu — tf32 wgmma, W_hh resident in shared
+    memory, h exchanged through DSMEM; the two directions of a layer run as separate clusters of one launch)
+    and, for batches up to 1024, the chained-GEMM head (K6: ``ops/lstm_fused.py``; larger batches use torch's
+    linears).  Other hidden sizes, wider inputs and non-fp32 weights use cuDNN / cuBLAS, which is also the
+    numerics oracle; ``fused=False`` takes cuDNN / cuBLAS for every shape.
 """
 from __future__ import annotations
 
@@ -26,6 +27,8 @@ from typing import Callable, Optional, Sequence
 
 import torch
 from torch import nn
+
+from ..ops import functional as F2
 
 
 class LSTM(nn.Module):
@@ -96,22 +99,11 @@ class LSTM(nn.Module):
         shape = (self.n_layers * self.directions, batch_size, self.h_size)
         return (torch.randn(shape, device=dev, dtype=dt), torch.randn(shape, device=dev, dtype=dt))
 
-    def _use_fused(self, x: torch.Tensor) -> bool:
-        if self._fused is False or not x.is_cuda:
-            return False
-        from ..ops import lstm_fused
-        return lstm_fused.available(self, x)
-
     def forward(self, input):
-        batch_size = input.size(0)
-        self.hidden = self.init_hidden(batch_size)
-        from ..ops import lstm_fused
-        if self._use_fused(input):
-            return lstm_fused.forward(self, input, self.hidden)
-        if self._fused is not False and input.is_cuda and input.dtype == torch.float32:
-            # batches beyond the fused head (the reference validates on the whole test split at once)
-            lstm_output, self.hidden = lstm_fused.recurrence(self, input, self.hidden)
+        self.hidden = self.init_hidden(input.size(0))
+        if self._fused is False:
+            lstm, head = F2.lstm_reference, F2.lstm_head_reference
         else:
-            lstm_output, self.hidden = self.lstm(input, self.hidden)
-        last_hidden_states = lstm_output[:, self.window_size - 1:self.window_size, :]
-        return self.linear3(self.linear2(self.linear(last_hidden_states)))
+            lstm, head = F2.lstm, F2.lstm_head
+        lstm_output, self.hidden = lstm(input, self.lstm, self.hidden)
+        return head(lstm_output, self.window_size - 1, self.linear, self.linear2, self.linear3)

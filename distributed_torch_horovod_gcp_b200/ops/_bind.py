@@ -17,6 +17,7 @@ from .attention import attention_fused  # noqa: F401
 from .dropout import dropout_add  # noqa: F401
 from .xent import linear_cross_entropy  # noqa: F401
 from .lstm_rec import lstm_recurrent  # noqa: F401
+from .lstm_fused import head as lstm_head  # noqa: F401
 from .conv import conv3x3, conv2d_implicit  # noqa: F401
 from .ln import layer_norm  # noqa: F401
 from .gemm import linear, mlp, qkv_proj  # noqa: F401  (re-exported as kernels.linear / .mlp / .qkv_proj)
@@ -49,3 +50,7 @@ def linear_cross_entropy_supported(x, weight, targets) -> bool:
 
 def dropout_add_supported(y, residual) -> bool:
     return _dropout.supported(y, residual)
+
+
+def lstm_head_supported(seq, t_index, l1, l2, l3) -> bool:
+    return _lstm.head_supported(seq, t_index, l1, l2, l3)

@@ -6,7 +6,8 @@ hand-written sm_90a kernels bound in ``ops.kernels``: wgmma GEMM with fused epil
 (ops/gemm.py), implicit-GEMM convolution (ops/conv.py), fused BN/ReLU/residual and max-pool
 (ops/bn.py), LayerNorm (ops/ln.py), flash attention forward/backward with optional dropout
 (ops/attention.py), the LM head fused with its cross-entropy loss (ops/xent.py), dropout fused with the
-residual add (ops/dropout.py).
+residual add (ops/dropout.py), the persistent LSTM recurrence (ops/lstm_rec.py) and the LSTM model's linear
+head (ops/lstm_fused.py).
 """
 from __future__ import annotations
 
@@ -228,6 +229,53 @@ def linear_cross_entropy(x, weight, targets, ignore_index: int = -100, reduction
     if k is not None and k.has("linear_cross_entropy") and k.linear_cross_entropy_supported(x, weight, targets):
         return k.linear_cross_entropy(x, weight, targets, ignore_index, reduction)
     return linear_cross_entropy_reference(x, weight, targets, ignore_index, reduction)
+
+
+# ------------------------------------------------------------------ LSTM recurrence and head
+def lstm_reference(x, module: nn.LSTM, hidden):
+    return module(x, hidden)
+
+
+_warned_cudnn = False
+
+
+def lstm(x, module: nn.LSTM, hidden):
+    """``module(x, hidden) -> (seq, (h_n, c_n))``.  Kernel path (hidden size 256, fp32, batch_first, biases,
+    1..512 input features, no projection): the persistent recurrence kernels for the whole stack, inter-layer
+    dropout included (ops/lstm_rec.py).  Any other LSTM takes cuDNN's RNN, logged once when it could have
+    taken the kernels but for its shape or dtype."""
+    k = _kernels(x)
+    if k is not None and k.has("lstm_recurrent"):
+        from . import lstm_rec
+        if lstm_rec.stack_supported(module, x):
+            return lstm_rec.lstm_stack(x, hidden[0], hidden[1], [w for ws in module.all_weights for w in ws],
+                                       module.num_layers, module.bidirectional,
+                                       dropout=module.dropout if module.training else 0.0)
+        global _warned_cudnn
+        if not _warned_cudnn:
+            _warned_cudnn = True
+            import logging
+            logging.getLogger("b200dp").warning(
+                "LSTM shape (layers=%d, hidden=%d, features=%d, bidirectional=%s, proj_size=%d, dtype=%s) is "
+                "outside the persistent recurrence kernels (hidden size 256, 1..512 features, fp32, no "
+                "projection): using the cuDNN RNN for this module",
+                module.num_layers, module.hidden_size, module.input_size, module.bidirectional,
+                module.proj_size, module.weight_hh_l0.dtype)
+    return lstm_reference(x, module, hidden)
+
+
+def lstm_head_reference(seq, t: int, l1: nn.Linear, l2: nn.Linear, l3: nn.Linear):
+    return l3(l2(l1(seq[:, t:t + 1])))
+
+
+def lstm_head(seq, t: int, l1: nn.Linear, l2: nn.Linear, l3: nn.Linear):
+    """``l3(l2(l1(seq[:, t:t + 1])))``, ``[B, 1, out3]``.  Kernel path (fp32, batch <= 1024, in + out1 + out2 +
+    out3 <= 12000, the six linear tensors dense fp32 on ``seq``'s device): the step gather and the three
+    linears as one forward and two backward kernels (ops/lstm_fused.py)."""
+    k = _kernels(seq)
+    if k is not None and k.has("lstm_fused") and k.lstm_head_supported(seq, t, l1, l2, l3):
+        return k.lstm_head(seq, t, l1, l2, l3)
+    return lstm_head_reference(seq, t, l1, l2, l3)
 
 
 # ------------------------------------------------------------------ ViT patch embedding

@@ -74,52 +74,19 @@ class _HeadFn(torch.autograd.Function):
         return dseq, None, dW1, db1, dW2, db2, dW3, db3
 
 
-def available(model, x: torch.Tensor) -> bool:
-    if _lib is None:
-        try:
-            from . import kernels
-            kernels.has("lstm_fused")        # triggers the lazy library load + register()
-        except Exception:
-            return False
-    p = model.linear.weight
-    return (_lib is not None and x.is_cuda and p.dtype == torch.float32 and x.dtype == torch.float32
-            and x.shape[0] <= 1024
-            and model.linear.in_features + model.linear.out_features + model.linear2.out_features
-            + model.linear3.out_features <= 12000)
+def head_supported(seq: torch.Tensor, t_index: int, l1, l2, l3) -> bool:
+    """Whether ``l3(l2(l1(seq[:, t_index:t_index + 1])))`` can run on K6: fp32 ``seq`` [B, T, H] with B <= 1024
+    and 0 <= ``t_index`` < T, three chained biased linears with H + out1 + out2 + out3 <= 12000, and all six
+    of their tensors dense fp32 on ``seq``'s device (the kernels read them by pointer)."""
+    tensors = (l1.weight, l1.bias, l2.weight, l2.bias, l3.weight, l3.bias)
+    return (_lib is not None and seq.dim() == 3 and seq.dtype == torch.float32 and seq.shape[0] <= 1024
+            and 0 <= t_index < seq.shape[1] and l1.in_features == seq.shape[2]
+            and l2.in_features == l1.out_features and l3.in_features == l2.out_features
+            and l1.in_features + l1.out_features + l2.out_features + l3.out_features <= 12000
+            and all(p is not None and p.dtype == torch.float32 and p.is_contiguous() and p.device == seq.device
+                    for p in tensors))
 
 
-_warned_cudnn = False
-
-
-def recurrence(model, x, hidden):
-    """The model's nn.LSTM on the persistent recurrence kernels (K5, ops/lstm_rec.py) for every shape they
-    cover, inter-layer dropout included; cuDNN only for the others (hidden size != 256, > 512 input features,
-    projections, non-fp32 weights)."""
-    from . import lstm_rec
-    lstm = model.lstm
-    if lstm_rec.stack_supported(lstm, x):
-        return lstm_rec.lstm_stack(x, hidden[0], hidden[1], [w for ws in lstm.all_weights for w in ws],
-                                   lstm.num_layers, lstm.bidirectional,
-                                   dropout=lstm.dropout if lstm.training else 0.0)
-    global _warned_cudnn
-    if not _warned_cudnn:
-        _warned_cudnn = True
-        import logging
-        logging.getLogger("b200dp").warning(
-            "LSTM shape (layers=%d, hidden=%d, features=%d, bidirectional=%s, proj_size=%d, dtype=%s) is "
-            "outside the persistent recurrence kernels (hidden size 256, 1..512 features, fp32, no "
-            "projection): using the cuDNN RNN for this module",
-            model.n_layers, model.h_size, model.n_features, model.directions == 2,
-            getattr(lstm, "proj_size", 0), lstm.weight_hh_l0.dtype)
-    return lstm(x, hidden)
-
-
-def forward(model, x, hidden):
-    """Persistent recurrence kernels (K5, ops/lstm_rec.py; cuDNN only for shapes they do not cover)
-    + fused head (K6)."""
-    seq, model.hidden = recurrence(model, x, hidden)
-    if not seq.is_contiguous():
-        seq = seq.contiguous()
-    return _HeadFn.apply(seq, model.window_size - 1, model.linear.weight, model.linear.bias,
-                         model.linear2.weight, model.linear2.bias, model.linear3.weight,
-                         model.linear3.bias)
+def head(seq: torch.Tensor, t_index: int, l1, l2, l3) -> torch.Tensor:
+    """``l3(l2(l1(seq[:, t_index:t_index + 1])))`` on K6, ``[B, 1, out3]``; ``head_supported`` must hold."""
+    return _HeadFn.apply(seq.contiguous(), t_index, l1.weight, l1.bias, l2.weight, l2.bias, l3.weight, l3.bias)

@@ -83,10 +83,11 @@ def test_app_script_cuda_single(tmp_path):
     assert r.stdout.count("train_loss") == 2 and "total training time in minutes" in r.stdout
 
 
-def test_lstm_fused_head_matches_torch():
+def test_lstm_head_kernel_matches_torch():
     """K6: fused last-step gather + 3 chained linears (fp32) vs the PyTorch composition."""
     import copy
     from distributed_torch_horovod_gcp_b200.models import LSTM
+    from distributed_torch_horovod_gcp_b200.ops import kernels
     dev = torch.device("cuda", 0)
     torch.manual_seed(0)
     m = LSTM(23, 10, 1, 256, device=dev)
@@ -94,7 +95,9 @@ def test_lstm_fused_head_matches_torch():
     ref._fused = False
     x = torch.randn(32, 10, 23, device=dev)
     y = torch.randn(32, 1, 1, device=dev)
-    assert m._use_fused(x), "fused head kernels not available"
+    seq = torch.empty(32, 10, 256, device=dev)
+    assert kernels.enabled_for(seq) and kernels.has("lstm_fused") \
+        and kernels.lstm_head_supported(seq, 9, m.linear, m.linear2, m.linear3), "fused head kernels not available"
     torch.manual_seed(1)
     out = m(x)
     torch.manual_seed(1)
