@@ -90,6 +90,11 @@ def parse_args(argv=None):
                    help="GPT models: split each sequence across the ranks (zigzag shards, sequence-parallel "
                         "attention) instead of giving each rank its own batch; every rank draws the same tokens "
                         "and keeps its shard, and the printed losses are the rank averages")
+    sp_size = env("B200DP_SEQUENCE_PARALLEL_SIZE")
+    p.add_argument("--sequence-parallel-size", type=int, default=int(sp_size) if sp_size else None, metavar="G",
+                   help="with --sequence-parallel: split each sequence across a group of G ranks (G divides the "
+                        "world size; groups are contiguous blocks of ranks) instead of the whole world; the ranks "
+                        "of a group draw the same tokens and different groups different ones")
     args = p.parse_args(argv)
     if args.optimizer != "default" and args.model.lower() == "lstm":
         p.error("--optimizer lars|lamb applies to the image models")
@@ -105,7 +110,21 @@ def parse_args(argv=None):
         if args.cuda_graph:
             p.error("--sequence-parallel cannot be combined with --cuda-graph: the sequence-parallel attention's "
                     "collectives are not captured in CUDA graphs")
+    if args.sequence_parallel_size is not None:
+        if not args.sequence_parallel:
+            p.error("--sequence-parallel-size needs --sequence-parallel")
+        from distributed_torch_horovod_gcp_b200._state import launch_size
+        world = launch_size()
+        if args.sequence_parallel_size < 1 or world % args.sequence_parallel_size:
+            p.error(f"--sequence-parallel-size {args.sequence_parallel_size} does not divide the world size {world}")
     return args
+
+
+def sp_split(args):
+    """(group index, rank in the group, group size) of the sequence split: groups of --sequence-parallel-size
+    contiguous ranks, or the whole world as one group."""
+    G = args.sequence_parallel_size or hvd.size()
+    return hvd.rank() // G, hvd.rank() % G, G
 
 
 def image_optimizer(model, kind, lr):
@@ -218,20 +237,23 @@ if __name__ == "__main__":
         loss_fn = nn.MSELoss(reduction="mean")
     elif is_gpt(args.model):
         sp_kw = {"sequence_parallel": True} if args.sequence_parallel else {}
+        if args.sequence_parallel_size is not None:
+            sp_kw["sequence_parallel_size"] = args.sequence_parallel_size
         model = build_model(args.model, **dropout_kw(args), **sp_kw).to(_DEVICE)
         if compute_dtype != torch.float32:
             model = model.to(compute_dtype)
         seq_len = args.seq_len or model.context
-        # sequence parallelism: one batch for the world, each rank keeps its zigzag shard of every sequence
-        tokens = SyntheticTokenBatches(args.batch_size, seq_len, model.vocab, _DEVICE,
-                                       seed=0 if args.sequence_parallel else hvd.rank())
+        # sequence parallelism: one batch per group (seeded by the group index), each rank keeps its zigzag shard
+        # of every sequence
+        sp_group, sp_rank, sp_world = sp_split(args) if args.sequence_parallel else (hvd.rank(), 0, 1)
+        tokens = SyntheticTokenBatches(args.batch_size, seq_len, model.vocab, _DEVICE, seed=sp_group)
 
         def _next_tokens():
             inputs, labels = tokens.next()
             if not args.sequence_parallel:
                 return inputs, labels
             from distributed_torch_horovod_gcp_b200.ops.seq_parallel import zigzag_shard
-            shard = (lambda t: zigzag_shard(t, 1, hvd.rank(), hvd.size()))
+            shard = (lambda t: zigzag_shard(t, 1, sp_rank, sp_world))
             return shard(inputs), shard(labels.view(inputs.shape)).reshape(-1)
 
         class _TokenLoader:

@@ -38,6 +38,11 @@ def _env_int(*names: str, default: Optional[int] = None) -> Optional[int]:
     return default
 
 
+def launch_size() -> int:
+    """The world size the launcher's environment gives (1 without a launcher): what ``init`` will use."""
+    return _env_int("HOROVOD_SIZE", "WORLD_SIZE", "OMPI_COMM_WORLD_SIZE", "PMI_SIZE", default=1)
+
+
 @dataclass
 class Runtime:
     initialized: bool = False
@@ -85,7 +90,7 @@ def init(comm=None, process_sets=None) -> None:
         if rt.initialized:
             return
         rank = _env_int("HOROVOD_RANK", "RANK", "OMPI_COMM_WORLD_RANK", "PMI_RANK", default=0)
-        size = _env_int("HOROVOD_SIZE", "WORLD_SIZE", "OMPI_COMM_WORLD_SIZE", "PMI_SIZE", default=1)
+        size = launch_size()
         local_rank = _env_int("HOROVOD_LOCAL_RANK", "LOCAL_RANK",
                               "OMPI_COMM_WORLD_LOCAL_RANK", default=None)
         local_size = _env_int("HOROVOD_LOCAL_SIZE", "LOCAL_WORLD_SIZE",

@@ -129,6 +129,15 @@ struct LwArgs {
   int pad_;
 };
 
+// reduce-scatter / all-gather among a group of ranks: `coll`'s pointers are indexed by group rank (the index in
+// `members`), and multicast is never used (the world's multicast object spans non-members' buffers too).
+struct GroupCollArgs {
+  CollArgs coll;                    // src[] / dst[] by group rank; use_mc must be 0
+  int members[B200DP_MAX_RANKS];    // world ranks of the group, ascending
+  int size;                         // ranks in the group
+  int index;                        // this rank's group rank: members[index] == CommCtx::rank
+};
+
 struct BcastArgs {
   void* buf[B200DP_MAX_RANKS];
   void* buf_mc;
@@ -201,6 +210,37 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
 }
 
 // ------------------------------------------------------------------ cross-rank block barrier
+// Spin until this rank's pad entry `mine` (written by world rank `peer`) reaches epoch `e`.  False after the
+// watchdog expires or another block has reported a failure; the first reporter records (1, peer, block, channel)
+// in the mailbox.
+__device__ __forceinline__ bool wait_for_peer(const CommCtx& c, const uint32_t* mine, uint32_t e, int peer,
+                                              int channel) {
+  unsigned long long t0 = 0;
+  unsigned spins = 0;
+  while ((int)(ld_acquire_sys(mine) - e) < 0) {
+    if (++spins > 4096u) {
+      spins = 0;
+      const unsigned long long now = globaltimer_ns();
+      if (t0 == 0) {
+        t0 = now;
+      } else if (now - t0 > c.timeout_ns || *(volatile int*)c.err != 0) {
+        volatile int* mb = c.err;     // host-mapped mailbox; benign race between reporters
+        if (mb[0] == 0) {
+          mb[1] = peer;
+          mb[2] = (int)blockIdx.x;
+          mb[3] = channel;
+          __threadfence_system();
+          mb[0] = 1;
+          __threadfence_system();
+        }
+        return false;
+      }
+      __nanosleep(64);
+    }
+  }
+  return true;
+}
+
 // Block b of every rank meets block b of every other rank.  acq_rel: writes made by this
 // block before the barrier (P2P / multimem stores) are visible to peers after it.
 __device__ __forceinline__ bool rank_barrier(const CommCtx& c, int channel) {
@@ -213,35 +253,49 @@ __device__ __forceinline__ bool rank_barrier(const CommCtx& c, int channel) {
     const uint32_t e = c.epoch[base + t] + 1u;
     c.epoch[base + t] = e;
     red_add_release_sys(c.sig[t] + base + c.rank, 1u);
-    const uint32_t* mine = c.sig[c.rank] + base + t;
-    unsigned long long t0 = 0;
-    unsigned spins = 0;
-    while ((int)(ld_acquire_sys(mine) - e) < 0) {
-      if (++spins > 4096u) {
-        spins = 0;
-        const unsigned long long now = globaltimer_ns();
-        if (t0 == 0) {
-          t0 = now;
-        } else if (now - t0 > c.timeout_ns || *(volatile int*)c.err != 0) {
-          volatile int* mb = c.err;     // host-mapped mailbox; benign race between reporters
-          if (mb[0] == 0) {
-            mb[1] = t;
-            mb[2] = (int)blockIdx.x;
-            mb[3] = channel;
-            __threadfence_system();
-            mb[0] = 1;
-            __threadfence_system();
-          }
-          s_failed = 1;
-          break;
-        }
-        __nanosleep(64);
-      }
-    }
+    if (!wait_for_peer(c, c.sig[c.rank] + base + t, e, t, channel)) s_failed = 1;
   }
   __syncthreads();
   return s_failed == 0;
 }
+
+// The same barrier among the members of a group only.  The pad and epoch entries stay indexed by WORLD rank, so
+// the counter of an ordered pair of ranks counts exactly the collectives both took part in, whether world or group
+// ones, and a channel can carry both.  (Indexed by group rank, world ranks 0 and 2 would both credit slot 0 of
+// rank 3's pad when they lead groups {0, 1, 3} and {2, 3}.)
+__device__ __forceinline__ bool group_barrier(const CommCtx& c, const GroupCollArgs& g, int channel) {
+  __shared__ int s_failed;
+  if (threadIdx.x == 0) s_failed = 0;
+  __syncthreads();
+  const int t = threadIdx.x;
+  if (g.size > 1 && t < g.size && t != g.index) {
+    const int peer = g.members[t];
+    const int base = (channel * B200DP_MAX_BLOCKS + (int)blockIdx.x) * B200DP_MAX_RANKS;
+    const uint32_t e = c.epoch[base + peer] + 1u;
+    c.epoch[base + peer] = e;
+    red_add_release_sys(c.sig[peer] + base + c.rank, 1u);
+    if (!wait_for_peer(c, c.sig[c.rank] + base + peer, e, peer, channel)) s_failed = 1;
+  }
+  __syncthreads();
+  return s_failed == 0;
+}
+
+// Who takes part in a collective: `rank()` of `size()` ranks, and their barrier.  The whole world, or a group whose
+// data pointers are indexed by group rank.
+struct WorldTeam {
+  const CommCtx& c;
+  __device__ __forceinline__ int rank() const { return c.rank; }
+  __device__ __forceinline__ int size() const { return c.world; }
+  __device__ __forceinline__ bool barrier(int channel) const { return rank_barrier(c, channel); }
+};
+
+struct GroupTeam {
+  const CommCtx& c;
+  const GroupCollArgs& g;
+  __device__ __forceinline__ int rank() const { return g.index; }
+  __device__ __forceinline__ int size() const { return g.size; }
+  __device__ __forceinline__ bool barrier(int channel) const { return group_barrier(c, g, channel); }
+};
 
 // After a watchdog expiry the data behind the barrier is incomplete: rank_barrier returns false and the
 // kernels return without reducing / writing anything (the host raises HorovodInternalError from the
@@ -860,15 +914,15 @@ __global__ void __launch_bounds__(512) allreduce_sliced_kernel(CommCtx c, ARArgs
 // the switch does the sum) and keeps scale * sum locally — (N-1)/N * S bytes in per rank instead of the
 // 2 * S an allreduce-then-slice moves.  All-gather: rank r pushes its chunk into slot r of every peer
 // (one multimem.st per 16 bytes with NVLS).  All-to-all: rank r pushes chunk j into slot r of peer j.
-template <typename T, bool kNVLS>
-__global__ void __launch_bounds__(512) reducescatter_kernel(CommCtx c, CollArgs a) {
+template <typename T, bool kNVLS, typename Team>
+__device__ __forceinline__ void reducescatter_body(const Team& m, const CollArgs& a) {
   constexpr int VN = Vec<T>::N;
   const size_t nvec = a.chunk / VN;
-  const size_t base = (size_t)c.rank * nvec;
+  const size_t base = (size_t)m.rank() * nvec;
   const size_t stride = (size_t)gridDim.x * blockDim.x;
   const size_t start = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  uint4* out = reinterpret_cast<uint4*>(a.dst[c.rank]);
-  if (!rank_barrier(c, a.channel)) return;
+  uint4* out = reinterpret_cast<uint4*>(a.dst[m.rank()]);
+  if (!m.barrier(a.channel)) return;
   constexpr int U = kNVLS ? 4 : 2;
   for (size_t v0 = start; v0 < nvec; v0 += U * stride) {
     float acc[U][VN];
@@ -888,7 +942,7 @@ __global__ void __launch_bounds__(512) reducescatter_kernel(CommCtx c, CollArgs 
         const size_t v = v0 + u * stride;
 #pragma unroll
         for (int r = 0; r < B200DP_MAX_RANKS; ++r)
-          if (r < c.world && v < nvec) raw[u][r] = ld_peer_v4(reinterpret_cast<const uint4*>(a.src[r]) + base + v);
+          if (r < m.size() && v < nvec) raw[u][r] = ld_peer_v4(reinterpret_cast<const uint4*>(a.src[r]) + base + v);
       }
 #pragma unroll
       for (int u = 0; u < U; ++u) {
@@ -897,7 +951,7 @@ __global__ void __launch_bounds__(512) reducescatter_kernel(CommCtx c, CollArgs 
         for (int i = 0; i < VN; ++i) acc[u][i] = 0.0f;
 #pragma unroll
         for (int r = 0; r < B200DP_MAX_RANKS; ++r) {   // fixed rank order
-          if (r < c.world) {
+          if (r < m.size()) {
             Vec<T>::unpack(raw[u][r], f);
 #pragma unroll
             for (int i = 0; i < VN; ++i) acc[u][i] += f[i];
@@ -914,27 +968,47 @@ __global__ void __launch_bounds__(512) reducescatter_kernel(CommCtx c, CollArgs 
       out[v] = Vec<T>::pack(acc[u]);
     }
   }
-  rank_barrier(c, a.channel);   // peers have finished reading my input
+  m.barrier(a.channel);   // peers have finished reading my input
 }
 
-__global__ void __launch_bounds__(512) allgather_kernel(CommCtx c, CollArgs a) {
+template <typename T, bool kNVLS>
+__global__ void __launch_bounds__(512) reducescatter_kernel(CommCtx c, CollArgs a) {
+  reducescatter_body<T, kNVLS>(WorldTeam{c}, a);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(512) reducescatter_group_kernel(CommCtx c, GroupCollArgs a) {
+  reducescatter_body<T, false>(GroupTeam{c, a}, a.coll);
+}
+
+// kMC: multicast when the argument block asks for it (world only).
+template <bool kMC, typename Team>
+__device__ __forceinline__ void allgather_body(const Team& m, const CollArgs& a) {
   const size_t nvec = a.chunk;   // chunk is given in 16-byte vectors for the copy collectives
   const size_t stride = (size_t)gridDim.x * blockDim.x;
   const size_t start = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const uint4* src = reinterpret_cast<const uint4*>(a.src[c.rank]);
-  const size_t slot = (size_t)c.rank * nvec;
-  if (!rank_barrier(c, a.channel)) return;   // every rank's output is free to overwrite
+  const uint4* src = reinterpret_cast<const uint4*>(a.src[m.rank()]);
+  const size_t slot = (size_t)m.rank() * nvec;
+  if (!m.barrier(a.channel)) return;   // every rank's output is free to overwrite
   for (size_t v = start; v < nvec; v += stride) {
     const uint4 x = src[v];
-    if (a.use_mc) {
+    if (kMC && a.use_mc) {
       mc_st_v4(reinterpret_cast<uint4*>(a.dst_mc) + slot + v, x);
     } else {
 #pragma unroll
       for (int r = 0; r < B200DP_MAX_RANKS; ++r)
-        if (r < c.world) st_peer_v4(reinterpret_cast<uint4*>(a.dst[r]) + slot + v, x);
+        if (r < m.size()) st_peer_v4(reinterpret_cast<uint4*>(a.dst[r]) + slot + v, x);
     }
   }
-  rank_barrier(c, a.channel);   // all pushes visible everywhere
+  m.barrier(a.channel);   // all pushes visible everywhere
+}
+
+__global__ void __launch_bounds__(512) allgather_kernel(CommCtx c, CollArgs a) {
+  allgather_body<true>(WorldTeam{c}, a);
+}
+
+__global__ void __launch_bounds__(512) allgather_group_kernel(CommCtx c, GroupCollArgs a) {
+  allgather_body<false>(GroupTeam{c, a}, a.coll);
 }
 
 __global__ void __launch_bounds__(512) alltoall_kernel(CommCtx c, CollArgs a) {
@@ -1128,6 +1202,50 @@ int b200dp_comm_collective(const CommCtx* ctx, const CollArgs* args, int mode, i
 }
 
 int b200dp_comm_coll_bytes() { return (int)sizeof(CollArgs); }
+
+int b200dp_comm_group_coll_bytes() { return (int)sizeof(GroupCollArgs); }
+
+// The member list of a group launch: 1..B200DP_MAX_RANKS world ranks, strictly ascending (sorted, no duplicates),
+// inside the world, with the caller at `index`; no multicast.  Sets the error message and returns false otherwise.
+static bool group_ok(const CommCtx* ctx, const GroupCollArgs* g) {
+  const char* why = nullptr;
+  if (g->size < 1 || g->size > B200DP_MAX_RANKS) {
+    why = "size";
+  } else if (g->index < 0 || g->index >= g->size || g->members[g->index] != ctx->rank) {
+    why = "the caller is not members[index]";
+  } else if (g->coll.use_mc) {
+    why = "multicast";
+  } else {
+    for (int i = 0; i < g->size && !why; ++i) {
+      if (g->members[i] < 0 || g->members[i] >= ctx->world) why = "a member outside the world";
+      else if (i > 0 && g->members[i] <= g->members[i - 1]) why = "members not strictly ascending";
+    }
+  }
+  if (!why) return true;
+  snprintf(g_comm_err, sizeof(g_comm_err), "bad group collective launch: %s (size=%d index=%d rank=%d world=%d)",
+           why, g->size, g->index, ctx->rank, ctx->world);
+  return false;
+}
+
+// mode: 0 reduce-scatter, 1 all-gather, among the members of `args` (the world collectives' layouts, indexed by
+// group rank).  dtype as in b200dp_comm_collective.
+int b200dp_comm_group_collective(const CommCtx* ctx, const GroupCollArgs* args, int mode, int dtype, int blocks,
+                                 int threads, unsigned long long stream) {
+  if (!launch_ok("group collective", ctx, args->coll.channel, "mode", mode, 2, dtype, blocks, threads) ||
+      !group_ok(ctx, args) ||
+      (mode == 0 && !size_ok("group collective", "chunk", args->coll.chunk, vec_elems(dtype))))
+    return -1;
+  cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
+  if (mode == 1) {
+    allgather_group_kernel<<<blocks, threads, 0, st>>>(*ctx, *args);
+    return launched("group all-gather", cudaGetLastError());
+  }
+  return launched("group reduce-scatter", with_dtype(dtype, [&](auto tag) {
+    using T = typename decltype(tag)::type;
+    reducescatter_group_kernel<T><<<blocks, threads, 0, st>>>(*ctx, *args);
+    return cudaGetLastError();
+  }));
+}
 
 int b200dp_comm_broadcast(const CommCtx* ctx, const BcastArgs* args, int blocks, int threads,
                           unsigned long long stream) {

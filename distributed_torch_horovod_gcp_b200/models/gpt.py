@@ -17,6 +17,12 @@ returns this rank's logits or the mean loss over its own tokens.  With equal sha
 over the ranks (``DistributedOptimizer``) gives the full-sequence gradient.  At world size 1 the model is the
 same as without it.
 
+``sequence_parallel_size=G`` (G divides the world size) splits each sequence across a group of G ranks instead
+of the whole world: the groups are the contiguous blocks of ranks [k G, (k + 1) G), a rank's sequence-parallel
+rank is its index in its group, and each group trains on its own batch (sequence and data parallelism at once).
+The constructor is then collective: for 1 < G < world it creates every group's ``hvd.ProcessSet``, in the same
+order on every rank, or reuses a set already registered with the same ranks.  G = 1 is plain data parallelism and G = world the whole-world split.
+
 The MLP is the fused node's exact (erf) GELU, not GPT-2's tanh approximation, so weights trained by the
 original GPT-2 code would see a slightly different activation here.
 """
@@ -33,13 +39,17 @@ from .vit import EncoderBlock
 
 class GPT(nn.Module):
     def __init__(self, vocab: int = 50304, context: int = 1024, depth: int = 12, heads: int = 12,
-                 dim: int = 768, mlp_dim: int = 3072, dropout: float = 0.0, sequence_parallel: bool = False):
+                 dim: int = 768, mlp_dim: int = 3072, dropout: float = 0.0, sequence_parallel: bool = False,
+                 sequence_parallel_size=None):
         super().__init__()
         if not 0.0 <= dropout <= 1.0:
             raise ValueError(f"dropout must be in [0, 1], got {dropout}")
         if sequence_parallel and dropout > 0.0:
             raise ValueError("dropout is not supported with sequence_parallel=True")
         self.sequence_parallel = bool(sequence_parallel)
+        self.sequence_parallel_size, self._sp_set = None, None
+        if sequence_parallel_size is not None:
+            self._sp_groups(int(sequence_parallel_size))
         self.vocab, self.context, self.dim = vocab, context, dim
         self.dropout = float(dropout)
         self.wte = nn.Embedding(vocab, dim)
@@ -78,19 +88,43 @@ class GPT(nn.Module):
         if self.training and self.dropout > 0.0:
             x = F2.dropout_add(x, None, self.dropout)
         for blk in self.layers:
-            x = blk(x, sequence_parallel=True) if world > 1 else blk(x)
+            x = blk(x, sequence_parallel=True, process_set=self._sp_set) if world > 1 else blk(x)
         x = F2.layer_norm(x, self.ln_f.weight, self.ln_f.bias, self.ln_f.eps)
         if targets is not None:
             return F2.linear_cross_entropy(x.reshape(B * S, self.dim), self.wte.weight, targets.reshape(-1))
         return F2.linear(x.reshape(B * S, self.dim), self.wte.weight)
 
+    def _sp_groups(self, G: int):
+        """Check ``sequence_parallel_size=G`` and take the process set of every group of G ranks (collective): a
+        set registered with exactly those ranks is reused, so building several models does not add groups."""
+        if not self.sequence_parallel:
+            raise ValueError("sequence_parallel_size needs sequence_parallel=True")
+        from .. import _state
+        rt = _state.runtime()
+        world = rt.size if rt.initialized else 1
+        if G < 1 or world % G:
+            raise ValueError(f"sequence_parallel_size must be a divisor of the world size {world}, got {G}")
+        self.sequence_parallel_size = G
+        if 1 < G < world:
+            from ..torch.process_sets import add_process_set
+            sets = []
+            for k in range(world // G):
+                ranks = list(range(k * G, (k + 1) * G))
+                known = [ps for ps in rt.process_sets.values() if ps.ranks == ranks]
+                sets.append(known[0] if known else add_process_set(ranks))
+            self._sp_set = sets[rt.rank // G]
+
     def _sp_rank_world(self):
-        """(rank, world) of the sequence split: (0, 1) unless ``sequence_parallel`` with world size > 1."""
+        """(rank, world) of the sequence split: (0, 1) unless ``sequence_parallel`` with world size > 1; with
+        ``sequence_parallel_size=G``, the rank's index in its group of G contiguous ranks and G."""
         if not self.sequence_parallel:
             return 0, 1
         from .. import _state
         rt = _state.runtime()
-        return (rt.rank, rt.size) if rt.initialized else (0, 1)
+        if not rt.initialized:
+            return 0, 1
+        G = self.sequence_parallel_size or rt.size
+        return rt.rank % G, G
 
 
 def gpt2(**kw):

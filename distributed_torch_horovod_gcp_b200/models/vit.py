@@ -38,14 +38,15 @@ class EncoderBlock(nn.Module):
         self.fc1 = nn.Linear(dim, mlp_dim)
         self.fc2 = nn.Linear(mlp_dim, dim)
 
-    def forward(self, x, sequence_parallel: bool = False):
-        """``sequence_parallel=True``: ``x`` is this rank's zigzag shard of the sequence (``ops.seq_parallel``)."""
+    def forward(self, x, sequence_parallel: bool = False, process_set=None):
+        """``sequence_parallel=True``: ``x`` is this rank's zigzag shard of the sequence (``ops.seq_parallel``),
+        split across the ranks of ``process_set`` (an ``hvd.ProcessSet``; None: the world)."""
         B, S, D = x.shape
         pa = self.attention_dropout if self.training else 0.0
         pr = self.dropout if self.training else 0.0
         h = F2.layer_norm(x, self.ln_1.weight, self.ln_1.bias, self.ln_1.eps)
         a = F2.qkv_attention(h, self.qkv.weight, self.qkv.bias, self.heads, self.causal, pa,
-                             sequence_parallel=sequence_parallel)   # [B,S,D]
+                             sequence_parallel=sequence_parallel, process_set=process_set)   # [B,S,D]
         if pr > 0.0:
             # the branch output is dropped before the add, so the GEMM epilogue adds no residual
             x = F2.dropout_add(F2.linear(a, self.proj.weight, self.proj.bias), x, pr)

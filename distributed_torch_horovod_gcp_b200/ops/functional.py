@@ -161,16 +161,17 @@ def attention(qkv, heads: int, causal: bool = False, dropout_p: float = 0.0):
 
 
 def qkv_attention(x, weight, bias, heads: int, causal: bool = False, dropout_p: float = 0.0,
-                  sequence_parallel: bool = False):
+                  sequence_parallel: bool = False, process_set=None):
     """Multi-head self-attention input stage: packed QKV projection + scaled-dot-product attention
     (``causal=True``: position i attends to positions 0..i only, as in a decoder; ``dropout_p``: dropout on
     the attention probabilities, drawn inside the flash-attention kernels on the kernel path).
     Kernel path: q, k, v are produced as three dense matrices (no un-pack / re-pack copies).
     ``sequence_parallel=True``: ``x`` is this rank's zigzag shard of the sequence and attention runs through
-    ``seq_parallel.sp_attention`` over every rank's keys and values."""
+    ``seq_parallel.sp_attention`` over every rank's keys and values (``process_set``: the ranks of that set
+    only)."""
     dropout_p = _check_p(dropout_p)
     if sequence_parallel:
-        return _sp_qkv_attention(x, weight, bias, heads, causal, dropout_p)
+        return _sp_qkv_attention(x, weight, bias, heads, causal, dropout_p, process_set)
     k = _kernels(x)
     if k is not None and k.has("linear") and k.linear_supported(x, weight, bias) and x.dim() == 3 \
             and weight.shape[0] == 3 * x.shape[-1] and weight.shape[0] % 24 == 0 and x.shape[-1] % heads == 0 \
@@ -189,7 +190,7 @@ def qkv_attention(x, weight, bias, heads: int, causal: bool = False, dropout_p: 
     return attention(linear(x, weight, bias), heads, causal, dropout_p)
 
 
-def _sp_qkv_attention(x, weight, bias, heads, causal, dropout_p):
+def _sp_qkv_attention(x, weight, bias, heads, causal, dropout_p, process_set=None):
     from .seq_parallel import sp_attention
     B, S, D = x.shape
     hd = D // heads
@@ -199,7 +200,7 @@ def _sp_qkv_attention(x, weight, bias, heads, causal, dropout_p):
         q, kk, v = [t.view(B, S, heads, hd).transpose(1, 2) for t in k.qkv_proj(x, weight, bias)]
     else:
         q, kk, v = linear(x, weight, bias).view(B, S, 3, heads, hd).permute(2, 0, 3, 1, 4)
-    return sp_attention(q, kk, v, causal, dropout_p).transpose(1, 2).reshape(B, S, D)
+    return sp_attention(q, kk, v, causal, dropout_p, process_set).transpose(1, 2).reshape(B, S, D)
 
 
 # ------------------------------------------------------------------ LM head + cross-entropy

@@ -20,9 +20,14 @@ fp32 sums.  Anywhere else (CPU / Gloo, other dtypes, head dims or lengths) the r
 differentiable ``torch.distributed`` all-gather of K and V and SDPA with a boolean mask built from the global
 positions.  At world size 1, ``sp_attention`` is ``attention_fused`` (or SDPA where the kernels do not apply).
 
-Not supported: attention dropout (the backward would need each query row owner's Philox seed), sequence-parallel
-groups smaller than the world, CUDA-graph capture of the kernel path (its collectives are launched with
-per-call host arguments)."""
+Groups.  ``sp_attention(..., process_set=ps)`` splits each sequence across the ranks of ``ps`` only: "rank" and
+"world" above are then the rank's index in the set and the set's size, the all-gathers and the reduce-scatter run
+among the set's members (``runtime.symm`` with ``members=``, never multicast) and the reference path uses the
+set's ``torch.distributed`` group.  Several disjoint sets (``models.gpt``: contiguous blocks of ranks) then train
+on different batches at once.  A set of one rank is plain attention; a set of the whole world is the world.
+
+Not supported: attention dropout (the backward would need each query row owner's Philox seed), CUDA-graph capture
+of the kernel path (its collectives are launched with per-call host arguments)."""
 from __future__ import annotations
 
 import ctypes
@@ -157,19 +162,20 @@ def cast_bf16(src32: torch.Tensor, out: torch.Tensor):
 
 class _SPAttnFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, q, k, v, causal, rank, world, symm):
+    def forward(ctx, q, k, v, causal, rank, world, symm, members=None):
         q, k, v = _attn._fix(q), _attn._fix(k), _attn._fix(v)
         B, H, S, D = q.shape
         dev = q.device
+        coll = {} if members is None else {"members": members}     # the group's ranks (world ranks), or the world
         g = torch.empty((world, 2, B, S, H, D), dtype=torch.bfloat16, device=dev)
-        symm.allgather(pack_kv(k, v), g)
+        symm.allgather(pack_kv(k, v), g, **coll)
         kg, vg = kv_views(g)
         o = torch.empty((B, S, H, D), dtype=torch.bfloat16, device=dev).permute(0, 2, 1, 3)
         lse = torch.empty((B, H, S), dtype=torch.float32, device=dev)
         sp_fwd(q, kg, vg, o, lse, causal, rank, world)
         counters.bump("attn_sp_fwd")
         ctx.save_for_backward(q, k, v, o, lse)
-        ctx.causal, ctx.rank, ctx.world, ctx.symm = causal, rank, world, symm
+        ctx.causal, ctx.rank, ctx.world, ctx.symm, ctx.coll = causal, rank, world, symm, coll
         return o
 
     @staticmethod
@@ -180,17 +186,17 @@ class _SPAttnFn(torch.autograd.Function):
         do = _attn._fix(do)
         pack = pack_bwd(q, do, o, lse)
         g = torch.empty((W, pack.numel()), dtype=torch.uint8, device=dev)
-        ctx.symm.allgather(pack, g)
+        ctx.symm.allgather(pack, g, **ctx.coll)
         qg, dog, lse_ptr, delta_ptr, ld_sw = bwd_views(g, B, H, S, D)
         acc = torch.zeros((W, B, S, H, D), dtype=torch.float32, device=dev)
         dk, dv = [torch.empty((B, S, H, D), dtype=torch.bfloat16, device=dev).permute(0, 2, 1, 3) for _ in range(2)]
         sp_bwd(qg, k, v, dog, lse_ptr, delta_ptr, ld_sw, acc.permute(0, 1, 3, 2, 4), dk, dv, ctx.causal, ctx.rank, W)
         dq32 = torch.empty((B, S, H, D), dtype=torch.float32, device=dev)
-        ctx.symm.reducescatter(acc, dq32)                  # rank r: sum over ranks of acc[r]
+        ctx.symm.reducescatter(acc, dq32, **ctx.coll)      # rank r: sum over ranks of acc[r]
         dq = torch.empty((B, S, H, D), dtype=torch.bfloat16, device=dev)
         cast_bf16(dq32, dq)
         counters.bump("attn_sp_bwd", 3)
-        return dq.permute(0, 2, 1, 3), dk, dv, None, None, None, None
+        return dq.permute(0, 2, 1, 3), dk, dv, None, None, None, None, None
 
 
 # ------------------------------------------------------------------ reference path
@@ -246,14 +252,24 @@ def _kernel_reason(q, k, v):
     return None
 
 
-def sp_attention(q, k, v, causal: bool = True, dropout_p: float = 0.0):
-    """softmax(q k^T / sqrt(d) [+ causal mask on global positions]) v for this rank's zigzag shard of the
-    queries against every rank's keys and values: q, k, v are [B, H, S_loc, d] shards (see the module
-    docstring); returns [B, H, S_loc, d] (kernel path: memory order [B, S_loc, H, d]).  ``dropout_p > 0`` is
-    only supported at world size 1."""
-    dropout_p = _attn.check_dropout_p(dropout_p)
+def _split(process_set):
+    """(rank, world, members, torch.distributed group) of the sequence split: this rank of the whole world
+    (members and group None), or its index in ``process_set`` and the set's size, world ranks and group."""
     rt = _state.runtime()
     rank, world = (rt.rank, rt.size) if rt.initialized else (0, 1)
+    if process_set is None or world == 1 or process_set.size() == world:
+        return rank, world, None, None
+    return process_set.rank(), process_set.size(), list(process_set.ranks), process_set.group
+
+
+def sp_attention(q, k, v, causal: bool = True, dropout_p: float = 0.0, process_set=None):
+    """softmax(q k^T / sqrt(d) [+ causal mask on global positions]) v for this rank's zigzag shard of the
+    queries against every rank's keys and values: q, k, v are [B, H, S_loc, d] shards (see the module
+    docstring); returns [B, H, S_loc, d] (kernel path: memory order [B, S_loc, H, d]).  ``process_set``: split
+    across the ranks of this ``hvd.ProcessSet`` only (None: the world).  ``dropout_p > 0`` is only supported
+    when the split has one rank."""
+    dropout_p = _attn.check_dropout_p(dropout_p)
+    rank, world, members, group = _split(process_set)
     if world == 1:
         if _attn._lib is not None and q.is_cuda and _attn.supported(q, k, v):
             return _attn.attention_fused(q, k, v, causal, dropout_p)
@@ -273,8 +289,8 @@ def sp_attention(q, k, v, causal: bool = True, dropout_p: float = 0.0):
         if symm is None:
             why = "the symmetric-memory runtime is unavailable"
     if why is None:
-        return _SPAttnFn.apply(q, k, v, bool(causal), rank, world, symm)
+        return _SPAttnFn.apply(q, k, v, bool(causal), rank, world, symm, members)
     if why not in _said:
         _said.add(why)
         log.warning("sp_attention: reference path (all-gather + SDPA with a mask) because %s", why)
-    return sp_attention_reference(q, k, v, bool(causal), rank, world)
+    return sp_attention_reference(q, k, v, bool(causal), rank, world, group)

@@ -92,6 +92,29 @@ class CollArgs(ctypes.Structure):
 COLL_REDUCE_SCATTER, COLL_ALLGATHER, COLL_ALLTOALL = 0, 1, 2
 
 
+class GroupCollArgs(ctypes.Structure):
+    _fields_ = [("coll", CollArgs), ("members", ctypes.c_int * MAX_RANKS), ("size", ctypes.c_int),
+                ("index", ctypes.c_int)]
+
+
+def group_coll_args(members, index: int, src, dst, chunk: int, scale: float = 1.0,
+                    channel: int = CH_USER) -> GroupCollArgs:
+    """Argument block of a group reduce-scatter or all-gather (``b200dp_comm_group_collective``).  ``members``:
+    the group's world ranks, ascending; ``index``: the caller's group rank; ``src`` / ``dst``: device pointers
+    indexed by group rank (0 where the kernel does not read them); ``chunk`` as in ``CollArgs`` (elements for
+    reduce-scatter, 16-byte vectors for all-gather).  Multicast stays off."""
+    a = GroupCollArgs()
+    for g, p in enumerate(src):
+        a.coll.src[g] = p
+    for g, p in enumerate(dst):
+        a.coll.dst[g] = p
+    a.coll.chunk, a.coll.scale, a.coll.channel = chunk, float(scale), channel
+    for g, w in enumerate(members):
+        a.members[g] = w
+    a.size, a.index = len(members), index
+    return a
+
+
 class _Raw:
     """Expose a raw device range through ``__cuda_array_interface__`` (zero-copy into torch)."""
 
@@ -293,6 +316,9 @@ class SymmRuntime(KernelLauncher):
             L.b200dp_comm_collective.argtypes = [P(CommCtx), P(CollArgs), i, i, i, i, u64]
             if L.b200dp_comm_coll_bytes() != ctypes.sizeof(CollArgs):
                 raise RuntimeError("ctypes/C struct layout mismatch: CollArgs")
+            L.b200dp_comm_group_collective.argtypes = [P(CommCtx), P(GroupCollArgs), i, i, i, i, u64]
+            if L.b200dp_comm_group_coll_bytes() != ctypes.sizeof(GroupCollArgs):
+                raise RuntimeError("ctypes/C struct layout mismatch: GroupCollArgs")
         lim = [ctypes.c_int() for _ in range(6)]
         L.b200dp_comm_limits(*[ctypes.byref(x) for x in lim])
         got = tuple(x.value for x in lim) + (L.b200dp_comm_clip_bytes(), L.b200dp_comm_lw_bytes())
@@ -540,16 +566,36 @@ class SymmRuntime(KernelLauncher):
 
     # ------------------------------------------------------------------ reduce-scatter / all-gather / all-to-all
     def _coll(self, mode: int, a: CollArgs, dtype, work_bytes: int, stream):
-        blocks = max(1, min((work_bytes + 512 * 16 * 2 - 1) // (512 * 16 * 2), self.max_blocks or 48))
+        blocks = self._coll_blocks(work_bytes)
         self._launched(self.lib.b200dp_comm_collective(ctypes.byref(self.ctx), ctypes.byref(a), mode,
                                                        _DTYPE_CODE.get(dtype, 0), blocks, 512, stream.cuda_stream))
 
-    def reducescatter(self, src: torch.Tensor, out: torch.Tensor, scale: float = 1.0) -> torch.cuda.Event:
+    def _coll_blocks(self, work_bytes: int) -> int:
+        return max(1, min((work_bytes + 512 * 16 * 2 - 1) // (512 * 16 * 2), self.max_blocks or 48))
+
+    def _group(self, members) -> Tuple[List[int], int]:
+        """(members as a list, this rank's index in it); the C entry point checks the rest of the list."""
+        members = [int(w) for w in members]
+        if self.rank not in members:
+            raise ValueError(f"rank {self.rank} is not a member of the group {members}")
+        return members, members.index(self.rank)
+
+    def _group_coll(self, mode: int, a: GroupCollArgs, dtype, work_bytes: int, stream):
+        self._launched(self.lib.b200dp_comm_group_collective(ctypes.byref(self.ctx), ctypes.byref(a), mode,
+                                                             _DTYPE_CODE.get(dtype, 0), self._coll_blocks(work_bytes),
+                                                             512, stream.cuda_stream))
+
+    def reducescatter(self, src: torch.Tensor, out: torch.Tensor, scale: float = 1.0,
+                      members=None) -> torch.cuda.Event:
         """``out`` (numel = src.numel() / world) = scale * sum over ranks of chunk ``rank`` of ``src``.
         ``src`` is staged into symmetric memory (chunk-major slabs when larger than the staging
-        buffer); each rank then reads ONLY its own chunk from every peer (or lets the switch sum it)."""
+        buffer); each rank then reads ONLY its own chunk from every peer (or lets the switch sum it).
+        ``members`` (world ranks, ascending): the same among those ranks only, with the group's size and this
+        rank's index in it in place of the world's; never multicast."""
         stream = torch.cuda.current_stream(self.device)
-        W, es = self.world, src.element_size()
+        if members is not None:
+            members, gi = self._group(members)
+        W, es = (self.world if members is None else len(members)), src.element_size()
         vec = 16 // es
         chunk = src.numel() // W
         assert src.numel() == chunk * W and out.numel() == chunk and chunk % vec == 0
@@ -559,10 +605,15 @@ class SymmRuntime(KernelLauncher):
         for lo in range(0, chunk, cap):
             m = min(cap, chunk - lo)
             st[: W * m].view(W, m).copy_(s2[:, lo:lo + m])
+            dst = o1[lo:lo + m]
+            if members is not None:
+                a = group_coll_args(members, gi, [self.stage.peer_ptrs[w] for w in members],
+                                    [dst.data_ptr() if g == gi else 0 for g in range(W)], m, scale)
+                self._group_coll(COLL_REDUCE_SCATTER, a, src.dtype, m * es, stream)
+                continue
             a = CollArgs()
             for r in range(W):
                 a.src[r] = self.stage.peer_ptrs[r]
-            dst = o1[lo:lo + m]
             a.dst[self.rank] = dst.data_ptr()
             a.chunk, a.scale, a.channel = m, float(scale), CH_USER
             a.use_mc = 1 if (self.stage.mc_ptr and m * es >= (64 << 10)) else 0
@@ -572,18 +623,22 @@ class SymmRuntime(KernelLauncher):
         ev.record(stream)
         return ev
 
-    def allgather(self, src: torch.Tensor, out: torch.Tensor) -> torch.cuda.Event:
+    def allgather(self, src: torch.Tensor, out: torch.Tensor, members=None) -> torch.cuda.Event:
         """``out`` (world * src.numel()) = concatenation of every rank's ``src`` (equal sizes, 16-byte
-        multiple).  Each rank pushes its chunk into slot ``rank`` of every peer's staging buffer."""
-        return self._push(COLL_ALLGATHER, src, out)
+        multiple).  Each rank pushes its chunk into slot ``rank`` of every peer's staging buffer.
+        ``members`` (world ranks, ascending): the concatenation over those ranks only, in group-rank order;
+        never multicast."""
+        return self._push(COLL_ALLGATHER, src, out, members)
 
     def alltoall(self, src: torch.Tensor, out: torch.Tensor) -> torch.cuda.Event:
         """Equal-split all-to-all: chunk j of ``src`` lands in slot ``rank`` of rank j's ``out``."""
         return self._push(COLL_ALLTOALL, src, out)
 
-    def _push(self, mode: int, src: torch.Tensor, out: torch.Tensor) -> torch.cuda.Event:
+    def _push(self, mode: int, src: torch.Tensor, out: torch.Tensor, members=None) -> torch.cuda.Event:
         stream = torch.cuda.current_stream(self.device)
-        W = self.world
+        if members is not None:
+            members, gi = self._group(members)
+        W = self.world if members is None else len(members)
         sb = src.reshape(-1).view(torch.uint8)
         ob = out.reshape(-1).view(torch.uint8)
         chunk = sb.numel() if mode == COLL_ALLGATHER else sb.numel() // W     # bytes per (src, dst) pair
@@ -593,18 +648,23 @@ class SymmRuntime(KernelLauncher):
         o2 = ob.view(W, chunk)
         for lo in range(0, chunk, cap):
             m = min(cap, chunk - lo)
-            a = CollArgs()
             if mode == COLL_ALLGATHER:
                 piece = sb[lo:lo + m]
             else:                                   # pack the W sub-chunks of this slab contiguously
                 piece = sb.view(W, chunk)[:, lo:lo + m].contiguous().view(-1)
-            a.src[self.rank] = piece.data_ptr()
-            for r in range(W):
-                a.dst[r] = self.stage.peer_ptrs[r]
-            a.chunk, a.channel = m // 16, CH_USER
-            a.use_mc = 1 if (mode == COLL_ALLGATHER and self.stage.mc_ptr and m >= (64 << 10)) else 0
-            a.dst_mc = self.stage.mc_ptr
-            self._coll(mode, a, torch.uint8, m, stream)
+            if members is None:
+                a = CollArgs()
+                a.src[self.rank] = piece.data_ptr()
+                for r in range(W):
+                    a.dst[r] = self.stage.peer_ptrs[r]
+                a.chunk, a.channel = m // 16, CH_USER
+                a.use_mc = 1 if (mode == COLL_ALLGATHER and self.stage.mc_ptr and m >= (64 << 10)) else 0
+                a.dst_mc = self.stage.mc_ptr
+                self._coll(mode, a, torch.uint8, m, stream)
+            else:
+                a = group_coll_args(members, gi, [piece.data_ptr() if g == gi else 0 for g in range(W)],
+                                    [self.stage.peer_ptrs[w] for w in members], m // 16)
+                self._group_coll(mode, a, torch.uint8, m, stream)
             o2[:, lo:lo + m].copy_(st[: W * m].view(W, m))
             piece.record_stream(stream) if piece.data_ptr() != sb.data_ptr() else None
         ev = torch.cuda.Event()
