@@ -80,11 +80,14 @@ def parse_args(argv=None):
     p.add_argument("--clip-grad-norm", type=float, default=float(env("B200DP_CLIP_GRAD_NORM", "0")),
                    help="clip the averaged gradient by its global L2 norm to at most this value before "
                         "each update (DistributedOptimizer max_grad_norm=; 0 = off, the reference)")
-    p.add_argument("--optimizer", default=env("B200DP_OPTIMIZER", "default"), choices=["default", "lars", "lamb"],
+    p.add_argument("--optimizer", default=env("B200DP_OPTIMIZER", "default"),
+                   choices=["default", "lars", "lamb", "muon"],
                    help="image models: 'default' = SGD momentum 0.9, wd 1e-4 (the LSTM always uses Adam; "
                         "the GPT models AdamW, see gpt_optimizer); "
                         "'lars' / 'lamb' = hvd.LARS / hvd.LAMB with biases and norm-layer parameters in a "
-                        "group with adaptive=False and no weight decay")
+                        "group with adaptive=False and no weight decay; "
+                        "'muon' (GPT models only) = hvd.Muon on the blocks' matrices, AdamW on the rest "
+                        "(see gpt_muon_optimizer)")
     p.add_argument("--sequence-parallel", action="store_true",
                    default=env("B200DP_SEQUENCE_PARALLEL", "0") == "1",
                    help="GPT models: split each sequence across the ranks (zigzag shards, sequence-parallel "
@@ -96,6 +99,8 @@ def parse_args(argv=None):
                         "world size; groups are contiguous blocks of ranks) instead of the whole world; the ranks "
                         "of a group draw the same tokens and different groups different ones")
     args = p.parse_args(argv)
+    if args.optimizer == "muon" and not is_gpt(args.model):
+        p.error("--optimizer muon applies to the GPT models")
     if args.optimizer != "default" and args.model.lower() == "lstm":
         p.error("--optimizer lars|lamb applies to the image models")
     if not 0.0 <= args.dropout <= 1.0:
@@ -163,6 +168,24 @@ def gpt_optimizer(model, lr):
     groups = [{"params": [p for p in model.parameters() if p.dim() >= 2], "weight_decay": 0.1},
               {"params": [p for p in model.parameters() if p.dim() < 2], "weight_decay": 0.0}]
     return torch.optim.AdamW(groups, lr=lr, betas=(0.9, 0.95))
+
+
+MUON_MATRICES = ("qkv.weight", "proj.weight", "fc1.weight", "fc2.weight")
+
+
+def gpt_muon_optimizer(model, lr):
+    """hvd.Muon on the transformer blocks' projection matrices (qkv, proj, fc1, fc2), with adjust_lr_fn
+    "match_rms_adamw" so that gpt_optimizer's learning rate and weight decay carry over; the embeddings, biases
+    and LayerNorm parameters keep gpt_optimizer's AdamW settings in use_muon=False groups."""
+    named = list(model.named_parameters())
+    muon = [p for n, p in named if n.startswith("layers.") and n.endswith(MUON_MATRICES)]
+    ids = {id(p) for p in muon}
+    rest = [p for _, p in named if id(p) not in ids]
+    groups = [{"params": muon, "weight_decay": 0.1},
+              {"params": [p for p in rest if p.dim() >= 2], "weight_decay": 0.1, "use_muon": False},
+              {"params": [p for p in rest if p.dim() < 2], "weight_decay": 0.0, "use_muon": False}]
+    return hvd.Muon([g for g in groups if g["params"]], lr=lr, betas=(0.9, 0.95),
+                    adjust_lr_fn="match_rms_adamw")
 
 
 if __name__ == "__main__":
@@ -263,8 +286,12 @@ if __name__ == "__main__":
         train_loader = _TokenLoader()
         test_loader = [_next_tokens()]
         lr = args.lr if args.lr != 1e-6 else 6e-4
-        optimizer = gpt_optimizer(model, lr) if args.optimizer == "default" else \
-            image_optimizer(model, args.optimizer, lr)
+        if args.optimizer == "default":
+            optimizer = gpt_optimizer(model, lr)
+        elif args.optimizer == "muon":
+            optimizer = gpt_muon_optimizer(model, lr)
+        else:
+            optimizer = image_optimizer(model, args.optimizer, lr)
         loss_fn = nn.CrossEntropyLoss()
     else:
         small = args.model.lower().replace("-", "").replace("_", "") == "resnet18" and not use_cuda

@@ -44,7 +44,7 @@ struct CommCtx {
   int world;
 };
 
-enum { OPT_NONE = 0, OPT_SGD = 1, OPT_ADAM = 2, OPT_LARS = 3, OPT_LAMB = 4 };
+enum { OPT_NONE = 0, OPT_SGD = 1, OPT_ADAM = 2, OPT_LARS = 3, OPT_LAMB = 4, OPT_MUON = 5 };
 
 struct OptHyper {
   int kind;        // OPT_*
@@ -127,6 +127,32 @@ struct LwArgs {
   int adaptive;            // 0: trust ratio 1 (biases, norm layers)
   float trust_coef;        // LARS eta; 1 for LAMB
   int pad_;
+};
+
+// Muon (h.kind OPT_MUON) on the one-shot path.  A bucket of matrices runs in three phases here, all launched from
+// the bucket-ready hook, around the Newton-Schulz GEMMs that the host launches on the wgmma kernel between phases 1
+// and 2: phase 0 (K12) reduces, updates the momentum buffer in s0, writes u to `r` and per-chunk sums of squares of
+// u; phase 1 (K13) folds each matrix's partials into its norm and writes X0 = bf16(u / max(norm, eps)), transposed
+// for tall matrices so that every NS operand has rows <= cols; phase 2 (K14) applies the decay and the NS result O.
+// The chunk table is LARS / LAMB's (LwChunk); `mats` gives the matrix of each chunk.
+struct MuonMat {
+  int rows;       // the parameter's shape
+  int cols;
+  int elem0;      // its first element in the bucket
+  int x0;         // first element of its NS operand in `x0` / `o`: [min(rows, cols)][max(rows, cols)] bf16
+};
+
+struct MuonArgs {
+  float* r;                  // fp32 u of this bucket (nesterov: g.lerp(buf, momentum), else buf)
+  float* part;               // per chunk: {sum of u^2, 0} (K12 writes, K13 reads)
+  const LwChunk* chunks;     // this bucket's chunk table
+  const MuonMat* mats;       // per chunk: the matrix the chunk belongs to
+  __nv_bfloat16* x0;         // K13: the bucket's NS inputs
+  const __nv_bfloat16* o;    // K14: the bucket's NS results, laid out as x0
+  int nchunks;
+  int nesterov;
+  int lr_mode;               // learning-rate factor f: 0 sqrt(max(1, rows / cols)), 1 0.2 sqrt(max(rows, cols))
+  float eps;                 // clamp of the norm
 };
 
 // reduce-scatter / all-gather among a group of ranks: `coll`'s pointers are indexed by group rank (the index in
@@ -829,6 +855,150 @@ __global__ void __launch_bounds__(512) lw_apply_kernel(CommCtx c, ARArgs a, LwAr
   finish_step(a);
 }
 
+// ------------------------------------------------------------------ K12 / K13 / K14: Muon
+// torch.lerp's formula: s + w (e - s) for |w| < 0.5, else e - (e - s)(1 - w).
+__device__ __forceinline__ float lerp_torch(float s, float e, float w) {
+  return fabsf(w) < 0.5f ? fmaf(w, e - s, s) : fmaf(-(e - s), 1.0f - w, e);
+}
+
+// K12: K1's reduction (same fixed rank order, same `scale * sum`), then buf.lerp_(g, 1 - momentum) into s0, u into
+// `k.r` and, per chunk, the fp32 sum of squares of u.  CTAs walk whole chunks as K10 does, so every rank holds the
+// same bits of u and of the partials.  Step counters are not touched.
+template <typename T>
+__global__ void __launch_bounds__(512) allreduce_oneshot_muon_kernel(CommCtx c, ARArgs a, MuonArgs k) {
+  constexpr int VN = Vec<T>::N;
+  const float mu = a.h.momentum, w = a.h.dampening;  // dampening carries Muon's lerp weight 1 - momentum
+
+  if (!rank_barrier(c, a.channel)) return;
+  for (int ch = blockIdx.x; ch < k.nchunks; ch += gridDim.x) {
+    const LwChunk q = k.chunks[ch];
+    float uu = 0.0f;
+    for (int v = q.first_vec + (int)threadIdx.x; v < q.first_vec + q.nvec; v += blockDim.x) {
+      uint4 raw[B200DP_MAX_RANKS];
+#pragma unroll
+      for (int r = 0; r < B200DP_MAX_RANKS; ++r)
+        if (r < c.world) raw[r] = ld_peer_v4(reinterpret_cast<const uint4*>(a.in[r]) + v);
+      float g[VN], f[VN], b[VN];
+#pragma unroll
+      for (int i = 0; i < VN; ++i) g[i] = 0.0f;
+#pragma unroll
+      for (int r = 0; r < B200DP_MAX_RANKS; ++r) {
+        if (r < c.world) {
+          Vec<T>::unpack(raw[r], f);
+#pragma unroll
+          for (int i = 0; i < VN; ++i) g[i] += f[i];
+        }
+      }
+      const size_t idx = (size_t)v * VN;
+      load_f32<VN>(a.s0 + idx, b);
+#pragma unroll
+      for (int i = 0; i < VN; ++i) {
+        g[i] = __fmul_rn(g[i], a.scale);  // rounded, as K1's scale * sum: never contracted into the lerp's e - s
+        b[i] = lerp_torch(b[i], g[i], w);
+        g[i] = k.nesterov ? lerp_torch(g[i], b[i], mu) : b[i];
+        uu = fmaf(g[i], g[i], uu);
+      }
+      store_f32<VN>(a.s0 + idx, b);
+      store_f32<VN>(k.r + idx, g);
+    }
+    const float s = block_sum_fixed(uu);
+    __syncthreads();  // the next chunk's sum reuses the block sum's shared memory
+    if (threadIdx.x == 0) {
+      k.part[2 * ch] = s;
+      k.part[2 * ch + 1] = 0.0f;
+    }
+  }
+  // as K10: zero exactly the vectors this thread read, after every peer's CTA of this index has read them too
+  rank_barrier(c, a.channel);
+  if (a.zero_input) {
+    uint4* mine = reinterpret_cast<uint4*>(const_cast<void*>(a.in[c.rank]));
+    for (int ch = blockIdx.x; ch < k.nchunks; ch += gridDim.x) {
+      const LwChunk q = k.chunks[ch];
+      for (int v = q.first_vec + (int)threadIdx.x; v < q.first_vec + q.nvec; v += blockDim.x)
+        mine[v] = make_uint4(0, 0, 0, 0);
+    }
+  }
+}
+
+// max(norm, eps) of the matrix whose partials are chunks [first, first + count), folded in double in a fixed order
+// as lw_trust does, rounded to fp32 once.
+__device__ float muon_norm(const MuonArgs& k, int first, int count) {
+  __shared__ float s_norm;
+  DoublePair acc = {0.0, 0.0};
+  for (int i = threadIdx.x; i < count; i += blockDim.x) acc.x += (double)k.part[2 * (first + i)];
+  acc = block_sum_fixed(acc);
+  if (threadIdx.x == 0) {
+    const float n = (float)sqrt(acc.x);
+    s_norm = n > k.eps ? n : k.eps;
+  }
+  __syncthreads();
+  return s_norm;
+}
+
+// Position of element e (row-major in the [rows, cols] parameter) in its NS operand: the same place, or for a tall
+// matrix (rows > cols) the transposed one.
+__device__ __forceinline__ int muon_pos(const MuonMat& m, int e) {
+  return m.rows > m.cols ? (e % m.cols) * m.rows + e / m.cols : e;
+}
+
+// K13: purely local.  X0 = bf16(u / max(norm, eps)) for every element of every matrix of the bucket.  Elements past
+// a matrix's end (the padding of its last vector) are skipped.
+template <typename T>
+__global__ void __launch_bounds__(512) muon_normalize_kernel(MuonArgs k) {
+  constexpr int VN = Vec<T>::N;
+  int tensor = -1;
+  float nrm = 1.0f;
+  for (int ch = blockIdx.x; ch < k.nchunks; ch += gridDim.x) {
+    const LwChunk q = k.chunks[ch];
+    const MuonMat m = k.mats[ch];
+    if (q.tfirst != tensor) {
+      tensor = q.tfirst;
+      nrm = muon_norm(k, q.tfirst, q.tcount);
+    }
+    const int numel = m.rows * m.cols;
+    for (int v = q.first_vec + (int)threadIdx.x; v < q.first_vec + q.nvec; v += blockDim.x) {
+      float u[VN];
+      load_f32<VN>(k.r + (size_t)v * VN, u);
+#pragma unroll
+      for (int i = 0; i < VN; ++i) {
+        const int e = v * VN + i - m.elem0;
+        if (e < numel) k.x0[m.x0 + muon_pos(m, e)] = __float2bfloat16_rn(__fdiv_rn(u[i], nrm));
+      }
+    }
+  }
+}
+
+// K14: purely local.  w = w (1 - lr wd) - (lr f) O on the fp32 master, with lr = h.lr * lr_scale and O read back in
+// the parameter's orientation; writes master and output, then bumps the step counter.
+template <typename T>
+__global__ void __launch_bounds__(512) muon_apply_kernel(CommCtx c, ARArgs a, MuonArgs k) {
+  constexpr int VN = Vec<T>::N;
+  const float lr = a.h.lr * (a.lr_scale ? *a.lr_scale : 1.0f);
+  const float decay = 1.0f - lr * a.h.weight_decay;
+  T* out = reinterpret_cast<T*>(a.out[c.rank]);
+  for (int ch = blockIdx.x; ch < k.nchunks; ch += gridDim.x) {
+    const LwChunk q = k.chunks[ch];
+    const MuonMat m = k.mats[ch];
+    const double f = k.lr_mode ? 0.2 * sqrt((double)max(m.rows, m.cols))
+                               : sqrt(fmax(1.0, (double)m.rows / (double)m.cols));
+    const float step = (float)((double)lr * f);
+    const int numel = m.rows * m.cols;
+    for (int v = q.first_vec + (int)threadIdx.x; v < q.first_vec + q.nvec; v += blockDim.x) {
+      const size_t idx = (size_t)v * VN;
+      float p[VN];
+      load_master<T, VN>(a, out, idx, p);
+#pragma unroll
+      for (int i = 0; i < VN; ++i) {
+        const int e = (int)idx + i - m.elem0;
+        if (e < numel) p[i] = fmaf(-step, __bfloat162float(k.o[m.x0 + muon_pos(m, e)]), p[i] * decay);
+      }
+      if (a.master) store_f32<VN>(a.master + idx, p);
+      reinterpret_cast<uint4*>(out)[v] = Vec<T>::pack(p);
+    }
+  }
+  finish_step(a);
+}
+
 // ------------------------------------------------------------------ K2: two-shot (P2P) and K3: NVLS
 template <typename T, bool kNVLS>
 __global__ void __launch_bounds__(512) allreduce_sliced_kernel(CommCtx c, ARArgs a) {
@@ -1159,6 +1329,27 @@ int b200dp_comm_lw_bucket(const CommCtx* ctx, const ARArgs* args, const LwArgs* 
     using T = typename decltype(tag)::type;
     if (phase == 1) lw_apply_kernel<T><<<blocks, threads, 0, st>>>(*ctx, *args, *lw);
     else allreduce_oneshot_lw_kernel<T><<<blocks, threads, 0, st>>>(*ctx, *args, *lw);
+    return cudaGetLastError();
+  }));
+}
+
+int b200dp_comm_muon_bytes() { return (int)sizeof(MuonArgs); }
+
+// phase: 0 reduce + momentum + u + chunk partials (K12), 1 norms + X0 (K13), 2 decay + NS result + step counter
+// (K14).  args->h.kind must be OPT_MUON; dtype as in b200dp_comm_allreduce.
+int b200dp_comm_muon_bucket(const CommCtx* ctx, const ARArgs* args, const MuonArgs* mu, int phase, int dtype,
+                            int blocks, int threads, unsigned long long stream) {
+  if (!launch_ok("muon", ctx, args->channel, "phase", phase, 3, dtype, blocks, threads)) return -1;
+  if (args->h.kind != OPT_MUON || mu->nchunks < 0) {
+    snprintf(g_comm_err, sizeof(g_comm_err), "bad muon launch: kind=%d chunks=%d", args->h.kind, mu->nchunks);
+    return -1;
+  }
+  cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
+  return launched("muon", with_dtype(dtype, [&](auto tag) {
+    using T = typename decltype(tag)::type;
+    if (phase == 0) allreduce_oneshot_muon_kernel<T><<<blocks, threads, 0, st>>>(*ctx, *args, *mu);
+    else if (phase == 1) muon_normalize_kernel<T><<<blocks, threads, 0, st>>>(*mu);
+    else muon_apply_kernel<T><<<blocks, threads, 0, st>>>(*ctx, *args, *mu);
     return cudaGetLastError();
   }));
 }

@@ -260,6 +260,7 @@ ConvParams conv_params() {
   p.g.M = INT_MAX;
   p.g.splits = 1;
   p.g.alpha = 1.0f;
+  p.g.res_scale = 1.0f;
   return p;
 }
 

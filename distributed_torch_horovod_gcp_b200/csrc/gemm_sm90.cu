@@ -114,10 +114,10 @@ const char* b200dp_gemm_last_error() { return g_err; }
 // split to finish a tile sums the partials of all splits in split order.
 // Requirements: K % 8 == 0 for K-major operands, M % 8 (A) / N % 8 (B) == 0 for MN-major, N % 8 == 0,
 // 16-byte aligned base pointers and leading dimensions, residual included; preact 4-byte aligned.
-int b200dp_gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, int lda, int ldb, int ldc,
+static int gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, int lda, int ldb, int ldc,
                      int a_mn, int b_mn, const void* bias_bf16, const void* bias_f32, const void* residual,
-                     void* preact, int act, int out_mode, int out_bf16, float alpha, int splits, int block_n,
-                     int max_ctas, float* stats, const void* res_mask, unsigned long long stream) {
+                     void* preact, int act, int out_mode, int out_bf16, float alpha, float beta, int splits,
+                     int block_n, int max_ctas, float* stats, const void* res_mask, unsigned long long stream) {
   if (ensure_init()) return -1;
   if (M <= 0 || N <= 0 || K <= 0) return fail("bad shape");
   if ((N % 8) || (lda % 8) || (ldb % 8) || (ldc % 4) || ((out_mode == 0 || out_bf16) && (ldc % 8)))
@@ -138,7 +138,9 @@ int b200dp_gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K,
   if (p.splits > 1 && (out_mode == 0 || bias_bf16 || bias_f32 || residual || preact || act))
     return fail("split-K requires out_mode 1/2 without bias, residual or activation");
   p.act = act; p.out_mode = out_mode; p.c_bf16 = out_bf16 ? 1 : 0; p.C = C; p.bias = bias_bf16; p.bias_f32 = bias_f32;
-  p.residual = residual; p.preact = preact; p.alpha = alpha;
+  p.residual = residual; p.preact = preact; p.alpha = alpha; p.res_scale = beta;
+  if (beta != 1.0f && (residual == nullptr || act > 2 || res_mask != nullptr))
+    return fail("beta: a plain residual (act 0..2, no res_mask) required");
   p.stats = stats;
   p.res_mask = reinterpret_cast<const unsigned char*>(res_mask);
   if (res_mask != nullptr && (residual == nullptr || preact != nullptr || act > 2 || out_mode != 0 || (N % 64) ||
@@ -159,6 +161,26 @@ int b200dp_gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K,
   if (p.splits > 1) p.splitk_slice = (long long)M * ldc;
   return run_splitk(p, p.num_m_blocks * p.num_n_blocks, st,
                     [&] { return launch_bn(BN, a_mn, b_mn, ma, mb, mc, p, max_ctas, st); });
+}
+
+int b200dp_gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, int lda, int ldb, int ldc,
+                     int a_mn, int b_mn, const void* bias_bf16, const void* bias_f32, const void* residual,
+                     void* preact, int act, int out_mode, int out_bf16, float alpha, int splits, int block_n,
+                     int max_ctas, float* stats, const void* res_mask, unsigned long long stream) {
+  return gemm_bf16(A, B, C, M, N, K, lda, ldb, ldc, a_mn, b_mn, bias_bf16, bias_f32, residual, preact, act, out_mode,
+                   out_bf16, alpha, 1.0f, splits, block_n, max_ctas, stats, res_mask, stream);
+}
+
+// b200dp_gemm_bf16 with the residual scaled: out_mode 0 / 2 compute act(alpha*AB + bias) + beta*residual, the
+// residual term added by one fma and the sum rounded once to C's dtype.  beta != 1 needs a plain residual (act
+// 0..2, no res_mask).
+int b200dp_gemm_bf16_scaled(const void* A, const void* B, void* C, int M, int N, int K, int lda, int ldb, int ldc,
+                            int a_mn, int b_mn, const void* bias_bf16, const void* bias_f32, const void* residual,
+                            void* preact, int act, int out_mode, int out_bf16, float alpha, float beta, int splits,
+                            int block_n, int max_ctas, float* stats, const void* res_mask,
+                            unsigned long long stream) {
+  return gemm_bf16(A, B, C, M, N, K, lda, ldb, ldc, a_mn, b_mn, bias_bf16, bias_f32, residual, preact, act, out_mode,
+                   out_bf16, alpha, beta, splits, block_n, max_ctas, stats, res_mask, stream);
 }
 
 }  // extern "C"

@@ -43,6 +43,7 @@ struct GemmParams {
   int n_fastest;           // tile order: consecutive CTAs walk the N blocks of one M block first (A tile is
                            // fetched from HBM once and re-used from L2 while the whole B matrix stays in L2)
   float alpha;
+  float res_scale;         // multiplies the residual of the fused epilogue (act 0..2): alpha acc + res_scale residual
   const unsigned char* res_mask;   // optional, with a plain residual (act 0..2): bit j of byte [row][col/8] keeps
                            // residual element (row, 8*(col/8)+j) — the ReLU sign bits of the block output whose
                            // skip-branch gradient the residual is (N % 64 == 0 required)
@@ -406,8 +407,8 @@ __device__ __forceinline__ void res_stage(const uint4* rv, uint32_t stg, int r0,
 
 // Epilogue of this thread's part of a finished 128 x BN tile, straight from the wgmma fragment d of
 // warpgroup wg — tile rows r and r + 8 (r = 64 wg + 16 warp + lane / 4), columns 8j + 2 (lane % 4) + {0, 1}:
-// alpha, bias, pre-activation, activation, residual; then bf16 pairs into the staging tile (out_mode 0: the 8
-// rows of a warp store hit 8 different swizzle positions, so the 4-byte stores are conflict-free), or pairs
+// alpha, bias, pre-activation, activation, residual (times res_scale); then bf16 pairs into the staging tile
+// (out_mode 0: the 8 rows of a warp store hit 8 different swizzle positions, so the 4-byte stores are conflict-free), or pairs
 // added into C (out_mode 1) or stored (out_mode 2) at column offset c_off, in C's dtype; with split-K, fp32
 // pairs stored into the workspace slice of the item's split.  m0: first row of the tile in the [M, ldc]
 // matrix.  A residual (out_mode != 1) has been staged at the output's place; every element is read and then
@@ -427,7 +428,7 @@ __device__ __forceinline__ void epilogue_frag(const GemmParams& p, const float* 
   const bool plain = p.out_mode == 0 && p.alpha == 1.0f && p.bias == nullptr && p.bias_f32 == nullptr &&
                      p.preact == nullptr && p.act == 0 && p.residual == nullptr;
   const bool res_only = p.out_mode == 0 && p.residual != nullptr && p.preact == nullptr && p.alpha == 1.0f &&
-                        p.bias == nullptr && p.bias_f32 == nullptr && p.act == 0;
+                        p.res_scale == 1.0f && p.bias == nullptr && p.bias_f32 == nullptr && p.act == 0;
   if (plain) {
     // the common case (plain bf16 output, optionally with BN statistics)
 #pragma unroll
@@ -501,9 +502,9 @@ __device__ __forceinline__ void epilogue_frag(const GemmParams& p, const float* 
           } else if (p.act == 4) {
             v0 = a0 > 0.0f ? v0 : 0.0f;
             v1 = a1 > 0.0f ? v1 : 0.0f;
-          } else {
-            v0 += a0;
-            v1 += a1;
+          } else {  // one rounding: with res_scale == 1 these are the bits of v + a
+            v0 = fmaf(p.res_scale, a0, v0);
+            v1 = fmaf(p.res_scale, a1, v1);
           }
         }
       }

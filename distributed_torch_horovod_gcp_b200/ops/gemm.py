@@ -32,6 +32,11 @@ def register(lib, have):
     lib.b200dp_gemm_bf16.argtypes = [vp, vp, vp, i, i, i, i, i, i, i, i, vp, vp, vp, vp, i, i, i, f, i,
                                      i, i, vp, vp, ctypes.c_uint64]
     lib.b200dp_gemm_bf16.restype = i
+    if hasattr(lib, "b200dp_gemm_bf16_scaled"):
+        lib.b200dp_gemm_bf16_scaled.argtypes = [vp, vp, vp, i, i, i, i, i, i, i, i, vp, vp, vp, vp, i, i, i, f, f,
+                                                i, i, i, vp, vp, ctypes.c_uint64]
+        lib.b200dp_gemm_bf16_scaled.restype = i
+        have["gemm_scaled"] = True
     lib.b200dp_gemm_last_error.restype = ctypes.c_char_p
     have["gemm"] = True
     have["linear"] = True
@@ -42,28 +47,33 @@ def gemm(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor, M: int, N: int, K:
          residual: Optional[torch.Tensor] = None, preact: Optional[torch.Tensor] = None,
          act: int = 0, out_mode: int = 0, alpha: float = 1.0, splits: int = 1, block_n: int = 0,
          max_ctas: int = 0, stats: Optional[torch.Tensor] = None,
-         res_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+         res_mask: Optional[torch.Tensor] = None, beta: float = 1.0) -> torch.Tensor:
     """Raw kernel call.  ``a``: [M,K] (K-major) or [K,M] (MN-major) bf16 with contiguous rows;
     ``b``: [N,K] or [K,N]; ``out``: [M,N] bf16 (out_mode 0), or bf16 / fp32 (1: add, 2: store; rounded once
     from the fp32 result).  Split-K (out_mode 1/2, splits > 1) sums in split order through an fp32 workspace
     allocated per launch on the current stream, so it may run on any stream.  ``stats`` accumulates through one per-library set of
     per-CTA slots: calls with ``stats`` (and the BatchNorm reductions of ``ops.bn``) must not run
-    concurrently on different streams."""
+    concurrently on different streams.  ``beta`` multiplies the residual (``act(alpha AB + bias) + beta residual``,
+    rounded once); ``beta != 1`` needs a plain residual (act 0..2, no ``res_mask``)."""
     assert _lib is not None, "libb200dp_kernels.so not loaded"
     assert a.dtype == torch.bfloat16 and b.dtype == torch.bfloat16
     assert a.stride(-1) == 1 and b.stride(-1) == 1 and out.stride(-1) == 1
     assert out.dtype == torch.bfloat16 or (out_mode != 0 and out.dtype == torch.float32)
     bias_bf = bias.data_ptr() if bias is not None and bias.dtype == torch.bfloat16 else None
     bias_f32 = bias.data_ptr() if bias is not None and bias.dtype == torch.float32 else None
-    rc = _lib.b200dp_gemm_bf16(
-        a.data_ptr(), b.data_ptr(), out.data_ptr(), M, N, K, a.stride(0), b.stride(0), out.stride(0),
-        int(a_mn), int(b_mn), bias_bf, bias_f32,
-        residual.data_ptr() if residual is not None else None,
-        preact.data_ptr() if preact is not None else None,
-        act, out_mode, int(out.dtype == torch.bfloat16), float(alpha), splits, block_n, max_ctas,
-        stats.data_ptr() if stats is not None else None,
-        res_mask.data_ptr() if res_mask is not None else None,
-        torch.cuda.current_stream(a.device).cuda_stream)
+    head = (a.data_ptr(), b.data_ptr(), out.data_ptr(), M, N, K, a.stride(0), b.stride(0), out.stride(0),
+            int(a_mn), int(b_mn), bias_bf, bias_f32,
+            residual.data_ptr() if residual is not None else None,
+            preact.data_ptr() if preact is not None else None,
+            act, out_mode, int(out.dtype == torch.bfloat16), float(alpha))
+    tail = (splits, block_n, max_ctas,
+            stats.data_ptr() if stats is not None else None,
+            res_mask.data_ptr() if res_mask is not None else None,
+            torch.cuda.current_stream(a.device).cuda_stream)
+    if beta == 1.0:
+        rc = _lib.b200dp_gemm_bf16(*head, *tail)
+    else:
+        rc = _lib.b200dp_gemm_bf16_scaled(*head, float(beta), *tail)
     if rc != 0:
         raise RuntimeError("b200dp_gemm_bf16: " + (_lib.b200dp_gemm_last_error() or b"").decode())
     counters.bump("gemm_sm90")

@@ -31,10 +31,19 @@ and still overlap backward: a one-shot reduction that writes the update directio
 sum of squares of the master weights and of the direction per chunk (K10), then a local update that folds
 each tensor's partials into its ratio in fp64 and applies it (K11).  A chunk is a fixed-size slice of one
 tensor; the per-bucket chunk table is built once here and kept on the device, so graph replays reuse it.
+
+Muon (``hvd.Muon``) follows each bucket's param group.  AdamW groups run the K7 launch with ``adamw=1``.  A Muon
+bucket runs, from its own hook: a one-shot reduction that updates the momentum buffer (S0), writes u to R and one
+fp32 sum of squares of u per chunk (K12); a local pass that folds each matrix's partials in fp64 and writes
+X0 = bf16(u / max(‖u‖, eps)) into engine-owned scratch, transposed for tall matrices (K13); ``ns_steps``
+Newton–Schulz iterations of three wgmma GEMMs per matrix (``ops.gemm.gemm``); and the update
+w = w (1 - lr wd) - lr f O on the master weights (K14).  Every rank reduces the whole bucket and runs the same
+deterministic GEMMs on the same bits of u, so the replicas stay bit-identical without exchanging O.
 """
 from __future__ import annotations
 
 import contextlib
+import ctypes
 import weakref
 from typing import Dict, List, Optional
 
@@ -48,7 +57,9 @@ from .buckets import Bucket, arena_sizes
 _ENGINES: "weakref.WeakSet[FusedEngine]" = weakref.WeakSet()
 LW_CHUNK_ELEMS = 16384          # elements per chunk of the LARS / LAMB partial norms
 _LAYERWISE_KINDS = ("lars", "lamb")
+_ONE_SHOT_ONLY_KINDS = ("lars", "lamb", "muon")    # kinds the engine does not combine with clipping or compression
 _logged_layerwise_fallback = False
+_logged_muon_fallback = False
 
 
 def _elem_size(dtype: torch.dtype) -> int:
@@ -71,10 +82,28 @@ def arena_view(flat: torch.Tensor, lo: int, param: torch.Tensor) -> torch.Tensor
     return seg.view(param.shape)
 
 
+def _muon_unsupported(opt, buckets: List[Bucket]) -> Optional[str]:
+    """Why the fused engine cannot run ``hvd.Muon`` ``opt`` on ``buckets``, or None: it needs the wgmma GEMM,
+    fp32 / bf16 parameters and Muon matrices with both dimensions multiples of 8 (the GEMM's operand layouts)."""
+    from ..ops import kernels
+    if not (kernels.has("gemm") and kernels.has("gemm_scaled")):
+        return "the kernels library with the wgmma GEMM and its scaled-residual entry point is not loaded"
+    if any(b.dtype not in (torch.float32, torch.bfloat16) for b in buckets):
+        return "parameters must be fp32 or bf16"
+    for g in opt.param_groups:
+        if g["use_muon"]:
+            for p in g["params"]:
+                if p.dim() != 2 or p.shape[0] % 8 or p.shape[1] % 8:
+                    return f"a Muon matrix of shape {tuple(p.shape)} is not a multiple of 8 in both dimensions"
+    return None
+
+
 def _classify(opt) -> Optional[str]:
-    """Return 'sgd' | 'adam' | 'adamw' | 'lars' | 'lamb' if the wrapped optimizer's update rule is one the
-    fused kernels implement exactly, else None."""
-    from ..torch.optim import LARS, LAMB
+    """Return 'sgd' | 'adam' | 'adamw' | 'lars' | 'lamb' | 'muon' if the wrapped optimizer's update rule is one
+    the fused kernels implement, else None."""
+    from ..torch.optim import LARS, LAMB, Muon
+    if isinstance(opt, Muon):
+        return "muon"
     if isinstance(opt, torch.optim.SGD):
         return "sgd"
     if isinstance(opt, LARS):
@@ -99,16 +128,24 @@ class FusedEngine:
     @staticmethod
     def try_create(opt, buckets: List[Bucket], wire_dtype,
                    max_grad_norm: Optional[float] = None) -> Optional["FusedEngine"]:
-        global _logged_layerwise_fallback
+        global _logged_layerwise_fallback, _logged_muon_fallback
         rt = _state.runtime()
         kind = _classify(opt)
-        if kind in _LAYERWISE_KINDS and (wire_dtype is not None or max_grad_norm is not None):
+        if kind in _ONE_SHOT_ONLY_KINDS and (wire_dtype is not None or max_grad_norm is not None):
             if not _logged_layerwise_fallback:
                 _state.log.warning("%s with %s runs on the generic path (all-reduce, then the optimizer's own "
                                    "step): the fused engine does not combine them", type(opt).__name__,
                                    "max_grad_norm" if max_grad_norm is not None else "wire compression")
                 _logged_layerwise_fallback = True
             kind = None
+        if kind == "muon":
+            why = _muon_unsupported(opt, buckets)
+            if why is not None:
+                if not _logged_muon_fallback:
+                    _state.log.warning("Muon runs on the generic path (all-reduce, then the optimizer's own step): %s",
+                                       why)
+                    _logged_muon_fallback = True
+                kind = None
         ok_dtypes = all(b.dtype in (torch.float32, torch.bfloat16, torch.float16) for b in buckets)
         devs = {b.device for b in buckets}
         wire_ok = wire_dtype is None or (wire_dtype in (torch.bfloat16, torch.float16) and
@@ -154,7 +191,8 @@ class FusedEngine:
         self.max_grad_norm = None if max_grad_norm is None else float(max_grad_norm)
         self.clip = self.max_grad_norm is not None
         self.layerwise = kind in _LAYERWISE_KINDS
-        second_moment = kind in ("adam", "adamw", "lamb")
+        self.muon = kind == "muon"
+        second_moment = kind in ("adam", "adamw", "lamb", "muon")
         self.arenas: Dict[torch.dtype, dict] = {}
         for (dtype, device), n in arena_sizes(buckets).items():
             def f32(on: bool = True):
@@ -166,7 +204,7 @@ class FusedEngine:
             g.zero_()
             p.zero_()
             ar = {"G": G, "P": P, "g": g, "p": p, "M": f32(dtype != torch.float32), "S0": f32(),
-                  "S1": f32(second_moment), "R": f32(self.clip or self.layerwise)}
+                  "S1": f32(second_moment), "R": f32(self.clip or self.layerwise or self.muon)}
             if self.wire is not None:       # local fp32 gradients (autograd) and the model's fp32 parameters
                 ar["gw"], ar["g"], ar["p"] = g, f32(), f32()
             self.arenas[dtype] = ar
@@ -204,8 +242,10 @@ class FusedEngine:
             fin.slots, fin.nslots = self.slots.data_ptr(), self.slots.numel()
             fin.norm, fin.coef, fin.max_norm = self.grad_norm.data_ptr(), self.coef.data_ptr(), self.max_grad_norm
             self._fin_args = fin
-        if self.layerwise:
+        if self.layerwise or self.muon:
             self._build_chunks()
+        if self.muon:
+            self._build_muon()
         self._done = torch.cuda.Event()
         self.steps = 0
         self.rehomed = 0
@@ -270,7 +310,7 @@ class FusedEngine:
             a.inp[r], a.out[r] = gp[r], pp[r]
         both_mc = ar["G"].mc_ptr != 0 and ar["P"].mc_ptr != 0
         algo = symm.pick_algo(nbytes, need_mc=both_mc)
-        if self.wire is not None or self.clip or self.layerwise:
+        if self.wire is not None or self.clip or self.layerwise or self.muon:
             algo = S.ALGO_ONESHOT            # every rank must hold the full fp32 update / gradient (see __init__)
         if algo == S.ALGO_NVLS and not both_mc:
             algo = S.ALGO_TWOSHOT
@@ -341,6 +381,70 @@ class FusedEngine:
             k.nchunks = n
             self._lw_args[b.index] = k
 
+    def _build_muon(self):
+        """Muon: per chunk of ``_build_chunks``'s table, the matrix it belongs to (``MuonMat``, zero in AdamW
+        buckets), each Muon bucket's argument block and matrices, and the NS scratch: X0 / X1 (ping-pong operands,
+        one region per matrix of the largest bucket) and the Gram G and its update H of the largest matrix."""
+        S = self.S
+        mats, self._mu_args, self._mu_mats = [], {}, {}
+        x_elems, g_elems = 1, 1
+        for b in self.buckets:
+            vn = 16 // torch.empty((), dtype=b.dtype).element_size()
+            per = LW_CHUNK_ELEMS // vn
+            use = self._use_muon(b)
+            x0, mm = 0, []
+            for s in b.slots:
+                cnt = ((s.numel + vn - 1) // vn + per - 1) // per
+                rows, cols = s.param.shape if use else (0, 0)
+                mats += [(rows, cols, s.offset, x0)] * cnt
+                if use:
+                    mm.append((rows, cols, x0))
+                    g_elems = max(g_elems, min(rows, cols) ** 2)
+                    x0 += s.numel
+            x_elems = max(x_elems, x0)
+            self._mu_mats[b.index] = mm
+        self.mu_mats = torch.tensor(mats or [(0, 0, 0, 0)], dtype=torch.int32).to(self.device)
+        bf = dict(dtype=torch.bfloat16, device=self.device)
+        self.ns_x = [torch.zeros(x_elems, **bf), torch.zeros(x_elems, **bf)]
+        self.ns_g, self.ns_h = torch.zeros(g_elems, **bf), torch.zeros(g_elems, **bf)
+        for b in self.buckets:
+            if not self._use_muon(b):
+                continue
+            lw = self._lw_args[b.index]
+            k = S.MuonArgs()
+            k.r, k.part, k.chunks, k.nchunks = lw.r, lw.part, lw.chunks, lw.nchunks
+            # mu_mats has one row per chunk row, and both rows are four int32, so a chunk's byte offset in
+            # lw_chunks is its offset in mu_mats as well
+            assert ctypes.sizeof(S.MuonMat) == ctypes.sizeof(S.LwChunk) == 16
+            k.mats = self.mu_mats.data_ptr() + (lw.chunks - self.lw_chunks.data_ptr())
+            k.x0 = self.ns_x[0].data_ptr()
+            self._mu_args[b.index] = k
+
+    def _use_muon(self, b: Bucket) -> bool:
+        return self.muon and bool(self.opt.param_groups[b.group_index]["use_muon"])
+
+    def _newton_schulz(self, b: Bucket, group: dict) -> torch.Tensor:
+        """``ns_steps`` iterations on every matrix of Muon bucket ``b``, from X0 in ``ns_x[0]``, on the current
+        (side) stream: G = X Xᵀ, H = c G·G + b G, X ← a X + H·X.  Returns the scratch that holds O."""
+        from ..ops import gemm as G
+        a, bb, c = (float(v) for v in group["ns_coefficients"])
+        steps = int(group["ns_steps"])
+        for rows, cols, x0 in self._mu_mats[b.index]:
+            p, q = min(rows, cols), max(rows, cols)
+            gm, hm = self.ns_g[:p * p].view(p, p), self.ns_h[:p * p].view(p, p)
+            splits = G._splits_for(p, p, q)
+            for i in range(steps):
+                x = self.ns_x[i % 2][x0: x0 + p * q].view(p, q)
+                y = self.ns_x[(i + 1) % 2][x0: x0 + p * q].view(p, q)
+                if splits > 1:
+                    G.gemm(x, x, gm, p, p, q, out_mode=2, splits=splits)
+                else:
+                    G.gemm(x, x, gm, p, p, q)
+                G.gemm(gm, gm, hm, p, p, p, b_mn=True, residual=gm, alpha=c, beta=bb)
+                G.gemm(hm, x, y, p, q, p, b_mn=True, residual=x, beta=a)
+                self.kernel_launches += 3
+        return self.ns_x[steps % 2]
+
     def trust_ratios(self) -> Dict[str, torch.Tensor]:
         """LARS / LAMB: each parameter's trust ratio of the latest update, by name (0-dim fp32 views of a
         device buffer that every step, graph replays included, rewrites)."""
@@ -357,7 +461,16 @@ class FusedEngine:
         h.lr = float(lr)
         h.weight_decay = float(group.get("weight_decay", 0.0))
         h.maximize = int(bool(group.get("maximize", False)))
-        if self.kind == "sgd":
+        if self.kind == "muon" and group["use_muon"]:
+            h.kind = S.OPT_MUON
+            h.momentum = float(group["momentum"])
+            h.dampening = float(1 - group["momentum"])     # the lerp weight, formed in double as torch does
+            h.nesterov = int(bool(group["nesterov"]))
+        elif self.kind == "muon":
+            h.kind, h.adamw = S.OPT_ADAM, 1
+            b1, b2 = group["betas"]
+            h.beta1, h.beta2, h.eps = float(b1), float(b2), float(group["adam_eps"])
+        elif self.kind == "sgd":
             h.kind = S.OPT_SGD
             h.momentum = float(group.get("momentum", 0.0))
             h.dampening = float(group.get("dampening", 0.0))
@@ -397,6 +510,8 @@ class FusedEngine:
         with self._span(f"bucket.{b.index}", op, b.nbytes, f"bucket.{b.index} {op} {b.nbytes / 2**20:.1f}MB"):
             if self.clip:
                 self.symm.launch_clip_bucket(a, self._clip_args[b.index], self.S.CLIP_REDUCE, kdtype, kbytes, self.side)
+            elif self.muon and b.index in self._mu_args:
+                self._launch_muon(b, a, kdtype, kbytes)
             elif self.layerwise:
                 group = self.opt.param_groups[b.group_index]
                 k = self._lw_args[b.index]
@@ -409,6 +524,20 @@ class FusedEngine:
                 self.symm.launch_allreduce(a, self._algo[b.index], kdtype, kbytes, self.side)
             self.kernel_launches += 1
         return True
+
+    def _launch_muon(self, b: Bucket, a, kdtype, kbytes):
+        """The four phases of a Muon bucket on the side stream: K12, K13, the NS GEMMs, K14."""
+        S, group = self.S, self.opt.param_groups[b.group_index]
+        k = self._mu_args[b.index]
+        k.nesterov = int(bool(group["nesterov"]))
+        k.lr_mode = 1 if group["adjust_lr_fn"] == "match_rms_adamw" else 0
+        k.eps = float(group["eps"])
+        self.symm.launch_muon_bucket(a, k, S.MUON_REDUCE, kdtype, kbytes, self.side)
+        self.symm.launch_muon_bucket(a, k, S.MUON_NORMALIZE, kdtype, kbytes, self.side)
+        with torch.cuda.stream(self.side):
+            k.o = self._newton_schulz(b, group).data_ptr()
+        self.symm.launch_muon_bucket(a, k, S.MUON_APPLY, kdtype, kbytes, self.side)
+        self.kernel_launches += 2
 
     @contextlib.contextmanager
     def _span(self, name: str, op: str, nbytes: int, label: str):
@@ -494,7 +623,7 @@ class FusedEngine:
                 if self.kind == "sgd":
                     if opt.param_groups[b.group_index].get("momentum", 0.0) != 0.0:
                         st["momentum_buffer"] = v0
-                elif self.kind == "lars":
+                elif self.kind == "lars" or self._use_muon(b):
                     st["momentum_buffer"] = v0
                 else:
                     st["step"] = torch.tensor(float(steps_dev))
@@ -511,7 +640,7 @@ class FusedEngine:
             for s in b.slots:
                 st = opt.state.get(s.param, {})
                 lo = b.flat_offset + s.offset
-                if self.kind in ("sgd", "lars"):
+                if self.kind in ("sgd", "lars") or self._use_muon(b):
                     mb = st.get("momentum_buffer")
                     if mb is not None:
                         arena_view(ar["S0"], lo, s.param).copy_(mb)

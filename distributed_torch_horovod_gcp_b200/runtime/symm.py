@@ -27,7 +27,7 @@ CH_ENGINE, CH_USER, CH_BCAST, CH_OPT = 0, 1, 2, 3
 ALGO_ONESHOT, ALGO_TWOSHOT, ALGO_NVLS = 0, 1, 2
 ALGO_NAMES = {0: "oneshot", 1: "twoshot", 2: "nvls"}
 _DTYPE_CODE = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}
-OPT_NONE, OPT_SGD, OPT_ADAM, OPT_LARS, OPT_LAMB = 0, 1, 2, 3, 4
+OPT_NONE, OPT_SGD, OPT_ADAM, OPT_LARS, OPT_LAMB, OPT_MUON = 0, 1, 2, 3, 4, 5
 
 
 class CommCtx(ctypes.Structure):
@@ -74,6 +74,20 @@ class LwArgs(ctypes.Structure):
 
 
 LW_REDUCE, LW_APPLY = 0, 1
+
+
+class MuonMat(ctypes.Structure):
+    _fields_ = [("rows", ctypes.c_int), ("cols", ctypes.c_int), ("elem0", ctypes.c_int), ("x0", ctypes.c_int)]
+
+
+class MuonArgs(ctypes.Structure):
+    _fields_ = [("r", ctypes.c_uint64), ("part", ctypes.c_uint64), ("chunks", ctypes.c_uint64),
+                ("mats", ctypes.c_uint64), ("x0", ctypes.c_uint64), ("o", ctypes.c_uint64),
+                ("nchunks", ctypes.c_int), ("nesterov", ctypes.c_int), ("lr_mode", ctypes.c_int),
+                ("eps", ctypes.c_float)]
+
+
+MUON_REDUCE, MUON_NORMALIZE, MUON_APPLY = 0, 1, 2
 
 
 class BcastArgs(ctypes.Structure):
@@ -202,6 +216,15 @@ class KernelLauncher:
         self._launched(self.lib.b200dp_comm_lw_bucket(ctypes.byref(self.ctx), ctypes.byref(args), ctypes.byref(lw),
                                                       phase, _DTYPE_CODE[dtype], blocks, 512, stream.cuda_stream))
 
+    def launch_muon_bucket(self, args: ARArgs, mu: MuonArgs, phase: int, dtype: torch.dtype, nbytes: int,
+                           stream: torch.cuda.Stream):
+        """One phase of a Muon bucket: ``MUON_REDUCE`` (one-shot reduction, momentum, u into ``mu.r``, per-chunk
+        sums of squares), ``MUON_NORMALIZE`` (per-matrix norms, bf16 NS inputs into ``mu.x0``) or ``MUON_APPLY``
+        (decay and NS result ``mu.o`` applied, step counter)."""
+        blocks = self.pick_blocks(ALGO_ONESHOT, nbytes)
+        self._launched(self.lib.b200dp_comm_muon_bucket(ctypes.byref(self.ctx), ctypes.byref(args), ctypes.byref(mu),
+                                                        phase, _DTYPE_CODE[dtype], blocks, 512, stream.cuda_stream))
+
 
 class SymmRuntime(KernelLauncher):
     def __init__(self):
@@ -312,6 +335,10 @@ class SymmRuntime(KernelLauncher):
         L.b200dp_comm_clip_bucket.argtypes = [P(CommCtx), P(ARArgs), P(ClipArgs), i, i, i, i, u64]
         L.b200dp_comm_clip_finalize.argtypes = [P(ClipArgs), u64]
         L.b200dp_comm_lw_bucket.argtypes = [P(CommCtx), P(ARArgs), P(LwArgs), i, i, i, i, u64]
+        if hasattr(L, "b200dp_comm_muon_bucket"):
+            L.b200dp_comm_muon_bucket.argtypes = [P(CommCtx), P(ARArgs), P(MuonArgs), i, i, i, i, u64]
+            if L.b200dp_comm_muon_bytes() != ctypes.sizeof(MuonArgs):
+                raise RuntimeError("ctypes/C struct layout mismatch: MuonArgs")
         if hasattr(L, "b200dp_comm_collective"):
             L.b200dp_comm_collective.argtypes = [P(CommCtx), P(CollArgs), i, i, i, i, u64]
             if L.b200dp_comm_coll_bytes() != ctypes.sizeof(CollArgs):

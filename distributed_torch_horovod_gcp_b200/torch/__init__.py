@@ -25,7 +25,7 @@ from .mpi_ops import (Average, Sum, Adasum, Min, Max, Product, HorovodInternalEr
 from .functions import (broadcast_parameters, broadcast_optimizer_state, broadcast_object,
                         allgather_object)
 from .optimizer import DistributedOptimizer
-from .optim import LARS, LAMB
+from .optim import LARS, LAMB, Muon
 from .sync_batch_norm import SyncBatchNorm
 from .process_sets import ProcessSet, global_process_set, add_process_set, remove_process_set
 from . import elastic
