@@ -105,7 +105,7 @@ def time_kernels(arm, iters):
                     if ph is None:
                         symm.launch_allreduce(a, eng._algo[b.index], b.dtype, nbytes, eng.side)
                     else:
-                        symm.launch_lw_bucket(a, eng._lw_args[b.index], ph, b.dtype, nbytes, eng.side)
+                        symm.launch_bucket("lw", a, eng._lw_args[b.index], ph, b.dtype, nbytes, eng.side)
         e1.record(eng.side)
         torch.cuda.synchronize()
         return round(e0.elapsed_time(e1) / iters, 4)

@@ -101,8 +101,8 @@ def time_muon_kernels(arm, iters):
         for _ in range(iters):
             for b in eng.buckets:
                 if b.index in eng._mu_args:
-                    eng.symm.launch_muon_bucket(eng._args[b.index], eng._mu_args[b.index], phase, eng._kdtype[b.index],
-                                                eng._kbytes[b.index], eng.side)
+                    eng.symm.launch_bucket("muon", eng._args[b.index], eng._mu_args[b.index], phase,
+                                           eng._kdtype[b.index], eng._kbytes[b.index], eng.side)
         e1.record(eng.side)
         torch.cuda.synchronize()
         out[name] = round(e0.elapsed_time(e1) / iters, 4)

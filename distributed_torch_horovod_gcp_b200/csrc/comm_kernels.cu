@@ -118,15 +118,20 @@ struct LwChunk {
   int tcount;     // chunks of that tensor
 };
 
-struct LwArgs {
-  float* r;                // fp32 update direction of this bucket (LARS g + wd w, LAMB m^/(sqrt(v^)+eps) + wd w)
-  float* part;             // per chunk: {sum of w^2, sum of dir^2} (K10 writes, K11 reads)
-  float* ratio;            // per chunk: the tensor's trust ratio, written at the tensor's first chunk (K11)
+// A bucket's slice of the chunk table and of the arrays indexed by it, shared by LARS / LAMB and Muon.
+struct ChunkArgs {
+  float* r;                // fp32 arena of this bucket: the update direction (K10) or Muon's u (K12)
+  float* part;             // per chunk: two fp32 partial sums of squares (K10 / K12 write, K11 / K13 read)
   const LwChunk* chunks;   // this bucket's chunk table
   int nchunks;
+  int pad_;
+};
+
+struct LwArgs {
+  ChunkArgs tab;           // r: LARS g + wd w, LAMB m^/(sqrt(v^)+eps) + wd w; part: {sum of w^2, sum of r^2}
+  float* ratio;            // per chunk: the tensor's trust ratio, written at the tensor's first chunk (K11)
   int adaptive;            // 0: trust ratio 1 (biases, norm layers)
   float trust_coef;        // LARS eta; 1 for LAMB
-  int pad_;
 };
 
 // Muon (h.kind OPT_MUON) on the one-shot path.  A bucket of matrices runs in three phases here, all launched from
@@ -134,7 +139,7 @@ struct LwArgs {
 // and 2: phase 0 (K12) reduces, updates the momentum buffer in s0, writes u to `r` and per-chunk sums of squares of
 // u; phase 1 (K13) folds each matrix's partials into its norm and writes X0 = bf16(u / max(norm, eps)), transposed
 // for tall matrices so that every NS operand has rows <= cols; phase 2 (K14) applies the decay and the NS result O.
-// The chunk table is LARS / LAMB's (LwChunk); `mats` gives the matrix of each chunk.
+// `tab` is LARS / LAMB's chunk table (ChunkArgs); `mats` gives the matrix of each chunk.
 struct MuonMat {
   int rows;       // the parameter's shape
   int cols;
@@ -143,16 +148,14 @@ struct MuonMat {
 };
 
 struct MuonArgs {
-  float* r;                  // fp32 u of this bucket (nesterov: g.lerp(buf, momentum), else buf)
-  float* part;               // per chunk: {sum of u^2, 0} (K12 writes, K13 reads)
-  const LwChunk* chunks;     // this bucket's chunk table
+  ChunkArgs tab;             // r: u (nesterov: g.lerp(buf, momentum), else buf); part: {sum of u^2, 0}
   const MuonMat* mats;       // per chunk: the matrix the chunk belongs to
   __nv_bfloat16* x0;         // K13: the bucket's NS inputs
   const __nv_bfloat16* o;    // K14: the bucket's NS results, laid out as x0
-  int nchunks;
   int nesterov;
   int lr_mode;               // learning-rate factor f: 0 sqrt(max(1, rows / cols)), 1 0.2 sqrt(max(rows, cols))
   float eps;                 // clamp of the norm
+  int pad_;
 };
 
 // reduce-scatter / all-gather among a group of ranks: `coll`'s pointers are indexed by group rank (the index in
@@ -709,6 +712,30 @@ __global__ void __launch_bounds__(512) clip_apply_kernel(CommCtx c, ARArgs a, Cl
 }
 
 // ------------------------------------------------------------------ K10 / K11: LARS / LAMB
+// The zero-on-consume tail of K10 and K12, after their closing barrier: zero exactly the vectors this thread read
+// in the chunk walk.  The CTA of the same index on every peer has read them too, while other CTAs may still be
+// reading theirs.  Vectors outside every chunk (bucket padding) are never written, so they stay zero.
+__device__ __forceinline__ void zero_chunks(const ChunkArgs& t, const void* in) {
+  uint4* mine = reinterpret_cast<uint4*>(const_cast<void*>(in));
+  for (int ch = blockIdx.x; ch < t.nchunks; ch += gridDim.x) {
+    const LwChunk q = t.chunks[ch];
+    for (int v = q.first_vec + (int)threadIdx.x; v < q.first_vec + q.nvec; v += blockDim.x)
+      mine[v] = make_uint4(0, 0, 0, 0);
+  }
+}
+
+// The fold of K11 and K13: the sums of a tensor's partials over chunks [first, first + count) in double (the
+// second only if `both`), thread t adding partials t, t + blockDim, ... then a fixed shuffle / warp tree, so every
+// CTA that needs them computes the same bits without waiting for another.  Valid in thread 0.
+__device__ __forceinline__ DoublePair fold_partials(const float* part, int first, int count, bool both) {
+  DoublePair acc = {0.0, 0.0};
+  for (int i = threadIdx.x; i < count; i += blockDim.x) {
+    acc.x += (double)part[2 * (first + i)];
+    if (both) acc.y += (double)part[2 * (first + i) + 1];
+  }
+  return block_sum_fixed(acc);
+}
+
 // K10: K1's reduction (same fixed rank order, same `scale * sum`), then the update direction into `k.r`
 // (LAMB also updates exp_avg / exp_avg_sq in s0 / s1) and, per chunk, the fp32 sums of squares of the master
 // weights and of the direction.  CTAs walk whole chunks, so every partial covers one tensor only and is added
@@ -723,8 +750,8 @@ __global__ void __launch_bounds__(512) allreduce_oneshot_lw_kernel(CommCtx c, AR
   if (lamb) bias_corrections(a.h.beta1, a.h.beta2, (a.step_ctr ? *a.step_ctr : 0) + 1, &bc1, &bc2_sqrt);
 
   if (!rank_barrier(c, a.channel)) return;
-  for (int ch = blockIdx.x; ch < k.nchunks; ch += gridDim.x) {
-    const LwChunk q = k.chunks[ch];
+  for (int ch = blockIdx.x; ch < k.tab.nchunks; ch += gridDim.x) {
+    const LwChunk q = k.tab.chunks[ch];
     float ww = 0.0f, dd = 0.0f;
     for (int v = q.first_vec + (int)threadIdx.x; v < q.first_vec + q.nvec; v += blockDim.x) {
       uint4 raw[B200DP_MAX_RANKS];
@@ -769,40 +796,24 @@ __global__ void __launch_bounds__(512) allreduce_oneshot_lw_kernel(CommCtx c, AR
         ww = fmaf(p[i], p[i], ww);
         dd = fmaf(g[i], g[i], dd);
       }
-      store_f32<VN>(k.r + idx, g);
+      store_f32<VN>(k.tab.r + idx, g);
     }
     const float2 s = block_sum_fixed(make_float2(ww, dd));
     __syncthreads();  // the next chunk's sum reuses the block sum's shared memory
     if (threadIdx.x == 0) {
-      k.part[2 * ch] = s.x;
-      k.part[2 * ch + 1] = s.y;
+      k.tab.part[2 * ch] = s.x;
+      k.tab.part[2 * ch + 1] = s.y;
     }
   }
-  // Zero exactly the vectors this thread read: after the barrier, the CTA of the same index on every peer has
-  // read them too, while other CTAs may still be reading theirs.  Vectors outside every chunk (bucket padding)
-  // are never written, so they stay zero.
   rank_barrier(c, a.channel);
-  if (a.zero_input) {
-    uint4* mine = reinterpret_cast<uint4*>(const_cast<void*>(a.in[c.rank]));
-    for (int ch = blockIdx.x; ch < k.nchunks; ch += gridDim.x) {
-      const LwChunk q = k.chunks[ch];
-      for (int v = q.first_vec + (int)threadIdx.x; v < q.first_vec + q.nvec; v += blockDim.x)
-        mine[v] = make_uint4(0, 0, 0, 0);
-    }
-  }
+  if (a.zero_input) zero_chunks(k.tab, a.in[c.rank]);
 }
 
-// Trust ratio of the tensor whose partials are chunks [first, first + count): thread t adds partials t,
-// t + blockDim, ... in double, then a fixed shuffle / warp tree, so every CTA that needs the ratio computes the
-// same bits without waiting for another.  1 when the group is not adaptive or either norm is not > 0.
+// Trust ratio of the tensor whose partials are chunks [first, first + count), computed by thread 0 from
+// fold_partials and broadcast to the CTA.  1 when the group is not adaptive or either norm is not > 0.
 __device__ float lw_trust(const LwArgs& k, int first, int count) {
   __shared__ float s_ratio;
-  DoublePair wd = {0.0, 0.0};
-  for (int i = threadIdx.x; i < count; i += blockDim.x) {
-    wd.x += (double)k.part[2 * (first + i)];
-    wd.y += (double)k.part[2 * (first + i) + 1];
-  }
-  wd = block_sum_fixed(wd);
+  const DoublePair wd = fold_partials(k.tab.part, first, count, true);
   if (threadIdx.x == 0) {
     const double wn = sqrt(wd.x), dn = sqrt(wd.y);
     s_ratio = (k.adaptive && wn > 0.0 && dn > 0.0) ? (float)((double)k.trust_coef * wn / dn) : 1.0f;
@@ -822,8 +833,8 @@ __global__ void __launch_bounds__(512) lw_apply_kernel(CommCtx c, ARArgs a, LwAr
   T* out = reinterpret_cast<T*>(a.out[c.rank]);
   int tensor = -1;
   float trust = 1.0f;
-  for (int ch = blockIdx.x; ch < k.nchunks; ch += gridDim.x) {
-    const LwChunk q = k.chunks[ch];
+  for (int ch = blockIdx.x; ch < k.tab.nchunks; ch += gridDim.x) {
+    const LwChunk q = k.tab.chunks[ch];
     if (q.tfirst != tensor) {
       tensor = q.tfirst;
       trust = lw_trust(k, q.tfirst, q.tcount);
@@ -833,7 +844,7 @@ __global__ void __launch_bounds__(512) lw_apply_kernel(CommCtx c, ARArgs a, LwAr
     for (int v = q.first_vec + (int)threadIdx.x; v < q.first_vec + q.nvec; v += blockDim.x) {
       const size_t idx = (size_t)v * VN;
       float d[VN], p[VN];
-      load_f32<VN>(k.r + idx, d);
+      load_f32<VN>(k.tab.r + idx, d);
       load_master<T, VN>(a, out, idx, p);
       if (lamb) {
 #pragma unroll
@@ -870,8 +881,8 @@ __global__ void __launch_bounds__(512) allreduce_oneshot_muon_kernel(CommCtx c, 
   const float mu = a.h.momentum, w = a.h.dampening;  // dampening carries Muon's lerp weight 1 - momentum
 
   if (!rank_barrier(c, a.channel)) return;
-  for (int ch = blockIdx.x; ch < k.nchunks; ch += gridDim.x) {
-    const LwChunk q = k.chunks[ch];
+  for (int ch = blockIdx.x; ch < k.tab.nchunks; ch += gridDim.x) {
+    const LwChunk q = k.tab.chunks[ch];
     float uu = 0.0f;
     for (int v = q.first_vec + (int)threadIdx.x; v < q.first_vec + q.nvec; v += blockDim.x) {
       uint4 raw[B200DP_MAX_RANKS];
@@ -899,34 +910,24 @@ __global__ void __launch_bounds__(512) allreduce_oneshot_muon_kernel(CommCtx c, 
         uu = fmaf(g[i], g[i], uu);
       }
       store_f32<VN>(a.s0 + idx, b);
-      store_f32<VN>(k.r + idx, g);
+      store_f32<VN>(k.tab.r + idx, g);
     }
     const float s = block_sum_fixed(uu);
     __syncthreads();  // the next chunk's sum reuses the block sum's shared memory
     if (threadIdx.x == 0) {
-      k.part[2 * ch] = s;
-      k.part[2 * ch + 1] = 0.0f;
+      k.tab.part[2 * ch] = s;
+      k.tab.part[2 * ch + 1] = 0.0f;
     }
   }
-  // as K10: zero exactly the vectors this thread read, after every peer's CTA of this index has read them too
   rank_barrier(c, a.channel);
-  if (a.zero_input) {
-    uint4* mine = reinterpret_cast<uint4*>(const_cast<void*>(a.in[c.rank]));
-    for (int ch = blockIdx.x; ch < k.nchunks; ch += gridDim.x) {
-      const LwChunk q = k.chunks[ch];
-      for (int v = q.first_vec + (int)threadIdx.x; v < q.first_vec + q.nvec; v += blockDim.x)
-        mine[v] = make_uint4(0, 0, 0, 0);
-    }
-  }
+  if (a.zero_input) zero_chunks(k.tab, a.in[c.rank]);
 }
 
-// max(norm, eps) of the matrix whose partials are chunks [first, first + count), folded in double in a fixed order
-// as lw_trust does, rounded to fp32 once.
+// max(norm, eps) of the matrix whose partials are chunks [first, first + count), from fold_partials (the first
+// sums only: K12 writes 0 to the second), rounded to fp32 once by thread 0 and broadcast to the CTA.
 __device__ float muon_norm(const MuonArgs& k, int first, int count) {
   __shared__ float s_norm;
-  DoublePair acc = {0.0, 0.0};
-  for (int i = threadIdx.x; i < count; i += blockDim.x) acc.x += (double)k.part[2 * (first + i)];
-  acc = block_sum_fixed(acc);
+  const DoublePair acc = fold_partials(k.tab.part, first, count, false);
   if (threadIdx.x == 0) {
     const float n = (float)sqrt(acc.x);
     s_norm = n > k.eps ? n : k.eps;
@@ -948,8 +949,8 @@ __global__ void __launch_bounds__(512) muon_normalize_kernel(MuonArgs k) {
   constexpr int VN = Vec<T>::N;
   int tensor = -1;
   float nrm = 1.0f;
-  for (int ch = blockIdx.x; ch < k.nchunks; ch += gridDim.x) {
-    const LwChunk q = k.chunks[ch];
+  for (int ch = blockIdx.x; ch < k.tab.nchunks; ch += gridDim.x) {
+    const LwChunk q = k.tab.chunks[ch];
     const MuonMat m = k.mats[ch];
     if (q.tfirst != tensor) {
       tensor = q.tfirst;
@@ -958,7 +959,7 @@ __global__ void __launch_bounds__(512) muon_normalize_kernel(MuonArgs k) {
     const int numel = m.rows * m.cols;
     for (int v = q.first_vec + (int)threadIdx.x; v < q.first_vec + q.nvec; v += blockDim.x) {
       float u[VN];
-      load_f32<VN>(k.r + (size_t)v * VN, u);
+      load_f32<VN>(k.tab.r + (size_t)v * VN, u);
 #pragma unroll
       for (int i = 0; i < VN; ++i) {
         const int e = v * VN + i - m.elem0;
@@ -976,8 +977,8 @@ __global__ void __launch_bounds__(512) muon_apply_kernel(CommCtx c, ARArgs a, Mu
   const float lr = a.h.lr * (a.lr_scale ? *a.lr_scale : 1.0f);
   const float decay = 1.0f - lr * a.h.weight_decay;
   T* out = reinterpret_cast<T*>(a.out[c.rank]);
-  for (int ch = blockIdx.x; ch < k.nchunks; ch += gridDim.x) {
-    const LwChunk q = k.chunks[ch];
+  for (int ch = blockIdx.x; ch < k.tab.nchunks; ch += gridDim.x) {
+    const LwChunk q = k.tab.chunks[ch];
     const MuonMat m = k.mats[ch];
     const double f = k.lr_mode ? 0.2 * sqrt((double)max(m.rows, m.cols))
                                : sqrt(fmax(1.0, (double)m.rows / (double)m.cols));
@@ -1280,6 +1281,14 @@ static bool size_ok(const char* what, const char* size_name, unsigned long long 
   return false;
 }
 
+// The chunked entry points (LARS / LAMB, Muon) walk the chunk table, not `n`: the optimizer kind must be one of
+// the entry point's (`kind_ok`) and the chunk count not negative.  Sets the error message and returns false otherwise.
+static bool chunks_ok(const char* what, bool kind_ok, int kind, const ChunkArgs& t) {
+  if (kind_ok && t.nchunks >= 0) return true;
+  snprintf(g_comm_err, sizeof(g_comm_err), "bad %s launch: kind=%d chunks=%d", what, kind, t.nchunks);
+  return false;
+}
+
 // Elements of a dtype code per 16-byte vector.
 static unsigned long long vec_elems(int dtype) { return dtype == 0 ? 4 : 8; }
 
@@ -1319,11 +1328,9 @@ int b200dp_comm_lw_bytes() { return (int)sizeof(LwArgs); }
 // args->h.kind selects LARS or LAMB.  dtype as in b200dp_comm_allreduce.
 int b200dp_comm_lw_bucket(const CommCtx* ctx, const ARArgs* args, const LwArgs* lw, int phase, int dtype,
                           int blocks, int threads, unsigned long long stream) {
-  if (!launch_ok("layer-wise", ctx, args->channel, "phase", phase, 2, dtype, blocks, threads)) return -1;
-  if ((args->h.kind != OPT_LARS && args->h.kind != OPT_LAMB) || lw->nchunks < 0) {
-    snprintf(g_comm_err, sizeof(g_comm_err), "bad layer-wise launch: kind=%d chunks=%d", args->h.kind, lw->nchunks);
+  if (!launch_ok("layer-wise", ctx, args->channel, "phase", phase, 2, dtype, blocks, threads) ||
+      !chunks_ok("layer-wise", args->h.kind == OPT_LARS || args->h.kind == OPT_LAMB, args->h.kind, lw->tab))
     return -1;
-  }
   cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
   return launched("layer-wise", with_dtype(dtype, [&](auto tag) {
     using T = typename decltype(tag)::type;
@@ -1339,11 +1346,9 @@ int b200dp_comm_muon_bytes() { return (int)sizeof(MuonArgs); }
 // (K14).  args->h.kind must be OPT_MUON; dtype as in b200dp_comm_allreduce.
 int b200dp_comm_muon_bucket(const CommCtx* ctx, const ARArgs* args, const MuonArgs* mu, int phase, int dtype,
                             int blocks, int threads, unsigned long long stream) {
-  if (!launch_ok("muon", ctx, args->channel, "phase", phase, 3, dtype, blocks, threads)) return -1;
-  if (args->h.kind != OPT_MUON || mu->nchunks < 0) {
-    snprintf(g_comm_err, sizeof(g_comm_err), "bad muon launch: kind=%d chunks=%d", args->h.kind, mu->nchunks);
+  if (!launch_ok("muon", ctx, args->channel, "phase", phase, 3, dtype, blocks, threads) ||
+      !chunks_ok("muon", args->h.kind == OPT_MUON, args->h.kind, mu->tab))
     return -1;
-  }
   cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
   return launched("muon", with_dtype(dtype, [&](auto tag) {
     using T = typename decltype(tag)::type;

@@ -43,7 +43,6 @@ deterministic GEMMs on the same bits of u, so the replicas stay bit-identical wi
 from __future__ import annotations
 
 import contextlib
-import ctypes
 import weakref
 from typing import Dict, List, Optional
 
@@ -347,78 +346,61 @@ class FusedEngine:
         return k, ap
 
     def _build_chunks(self):
-        """LARS / LAMB: the chunk table of every bucket (one device tensor, a slice per bucket), the per-chunk
-        partial sums and the per-chunk ratio slots.  Tensors start on a 16-byte boundary, so a vector never
-        straddles two tensors; a tensor's last vector may end in padding, which is zero in every arena and adds
-        nothing to either norm."""
+        """LARS / LAMB and Muon: in one pass over every bucket's slots, the chunk table (one device tensor, a slice
+        per bucket) and, with Muon, the matrix of each chunk (``MuonMat`` rows, zero in AdamW buckets); then each
+        bucket's ``ChunkArgs`` over its slices of the table, of the per-chunk partial sums and of R, embedded in its
+        ``LwArgs`` (with its per-chunk ratio slots) or, in a Muon bucket, its ``MuonArgs``.  Tensors start on a
+        16-byte boundary, so a vector never straddles two tensors; a tensor's last vector may end in padding, which
+        is zero in every arena and adds nothing to either norm."""
         S = self.S
-        rows, first = [], {}
-        span = {}
+        rows, mats, first, span = [], [], {}, {}
+        self._mu_mats = {}
         for b in self.buckets:
-            vn = 16 // torch.empty((), dtype=b.dtype).element_size()
+            vn = 16 // _elem_size(b.dtype)
             per = LW_CHUNK_ELEMS // vn
-            base = len(rows)
+            base, use, x0, mm = len(rows), self._use_muon(b), 0, []
             for s in b.slots:
                 v0, nv = s.offset // vn, (s.numel + vn - 1) // vn
                 t0, cnt = len(rows) - base, (nv + per - 1) // per
                 if cnt:
                     first[s.name] = len(rows)
                 rows += [(v0 + c * per, min(per, nv - c * per), t0, cnt) for c in range(cnt)]
+                shape = tuple(s.param.shape) if use else (0, 0)
+                mats += [(*shape, s.offset, x0)] * cnt
+                if use:
+                    mm.append((*shape, x0))
+                    x0 += s.numel
+            self._mu_mats[b.index] = mm
             span[b.index] = (base, len(rows) - base)
         total = max(len(rows), 1)
         self.lw_chunks = torch.tensor(rows or [(0, 0, 0, 0)], dtype=torch.int32).to(self.device)
         self.lw_part = torch.zeros(2 * total, dtype=torch.float32, device=self.device)
         self.lw_ratio = torch.ones(total, dtype=torch.float32, device=self.device)
+        if self.muon:
+            self.mu_mats = torch.tensor(mats or [(0, 0, 0, 0)], dtype=torch.int32).to(self.device)
         self._lw_first = first
         self._lw_args: Dict[int, object] = {}
+        self._mu_args: Dict[int, object] = {}
         for b in self.buckets:
             base, n = span[b.index]
-            k = S.LwArgs()
-            k.r = self.arenas[b.dtype]["R"].data_ptr() + 4 * b.flat_offset
-            k.part = self.lw_part.data_ptr() + 8 * base
-            k.ratio = self.lw_ratio.data_ptr() + 4 * base
-            k.chunks = self.lw_chunks.data_ptr() + 16 * base
-            k.nchunks = n
-            self._lw_args[b.index] = k
+            tab = S.ChunkArgs(r=self.arenas[b.dtype]["R"].data_ptr() + 4 * b.flat_offset,
+                              part=self.lw_part.data_ptr() + 8 * base, chunks=self.lw_chunks.data_ptr() + 16 * base,
+                              nchunks=n)
+            if self.layerwise:
+                self._lw_args[b.index] = S.LwArgs(tab=tab, ratio=self.lw_ratio.data_ptr() + 4 * base)
+            elif self._use_muon(b):
+                self._mu_args[b.index] = S.MuonArgs(tab=tab, mats=self.mu_mats.data_ptr() + 16 * base)
 
     def _build_muon(self):
-        """Muon: per chunk of ``_build_chunks``'s table, the matrix it belongs to (``MuonMat``, zero in AdamW
-        buckets), each Muon bucket's argument block and matrices, and the NS scratch: X0 / X1 (ping-pong operands,
-        one region per matrix of the largest bucket) and the Gram G and its update H of the largest matrix."""
-        S = self.S
-        mats, self._mu_args, self._mu_mats = [], {}, {}
-        x_elems, g_elems = 1, 1
-        for b in self.buckets:
-            vn = 16 // torch.empty((), dtype=b.dtype).element_size()
-            per = LW_CHUNK_ELEMS // vn
-            use = self._use_muon(b)
-            x0, mm = 0, []
-            for s in b.slots:
-                cnt = ((s.numel + vn - 1) // vn + per - 1) // per
-                rows, cols = s.param.shape if use else (0, 0)
-                mats += [(rows, cols, s.offset, x0)] * cnt
-                if use:
-                    mm.append((rows, cols, x0))
-                    g_elems = max(g_elems, min(rows, cols) ** 2)
-                    x0 += s.numel
-            x_elems = max(x_elems, x0)
-            self._mu_mats[b.index] = mm
-        self.mu_mats = torch.tensor(mats or [(0, 0, 0, 0)], dtype=torch.int32).to(self.device)
+        """Muon: the NS scratch, X0 / X1 (ping-pong operands, one region per matrix of the largest bucket) and the
+        Gram G and its update H of the largest matrix, and each Muon bucket's NS input pointer."""
+        x_elems = max([1] + [sum(r * c for r, c, _ in mm) for mm in self._mu_mats.values()])
+        g_elems = max([1] + [min(r, c) ** 2 for mm in self._mu_mats.values() for r, c, _ in mm])
         bf = dict(dtype=torch.bfloat16, device=self.device)
         self.ns_x = [torch.zeros(x_elems, **bf), torch.zeros(x_elems, **bf)]
         self.ns_g, self.ns_h = torch.zeros(g_elems, **bf), torch.zeros(g_elems, **bf)
-        for b in self.buckets:
-            if not self._use_muon(b):
-                continue
-            lw = self._lw_args[b.index]
-            k = S.MuonArgs()
-            k.r, k.part, k.chunks, k.nchunks = lw.r, lw.part, lw.chunks, lw.nchunks
-            # mu_mats has one row per chunk row, and both rows are four int32, so a chunk's byte offset in
-            # lw_chunks is its offset in mu_mats as well
-            assert ctypes.sizeof(S.MuonMat) == ctypes.sizeof(S.LwChunk) == 16
-            k.mats = self.mu_mats.data_ptr() + (lw.chunks - self.lw_chunks.data_ptr())
+        for k in self._mu_args.values():
             k.x0 = self.ns_x[0].data_ptr()
-            self._mu_args[b.index] = k
 
     def _use_muon(self, b: Bucket) -> bool:
         return self.muon and bool(self.opt.param_groups[b.group_index]["use_muon"])
@@ -509,7 +491,8 @@ class FusedEngine:
         kdtype, kbytes = self._kdtype[b.index], self._kbytes[b.index]
         with self._span(f"bucket.{b.index}", op, b.nbytes, f"bucket.{b.index} {op} {b.nbytes / 2**20:.1f}MB"):
             if self.clip:
-                self.symm.launch_clip_bucket(a, self._clip_args[b.index], self.S.CLIP_REDUCE, kdtype, kbytes, self.side)
+                self.symm.launch_bucket("clip", a, self._clip_args[b.index], self.S.CLIP_REDUCE, kdtype, kbytes,
+                                        self.side)
             elif self.muon and b.index in self._mu_args:
                 self._launch_muon(b, a, kdtype, kbytes)
             elif self.layerwise:
@@ -517,8 +500,8 @@ class FusedEngine:
                 k = self._lw_args[b.index]
                 k.adaptive = int(bool(group["adaptive"]))
                 k.trust_coef = float(group["trust_coefficient"]) if self.kind == "lars" else 1.0
-                self.symm.launch_lw_bucket(a, k, self.S.LW_REDUCE, kdtype, kbytes, self.side)
-                self.symm.launch_lw_bucket(a, k, self.S.LW_APPLY, kdtype, kbytes, self.side)
+                self.symm.launch_bucket("lw", a, k, self.S.LW_REDUCE, kdtype, kbytes, self.side)
+                self.symm.launch_bucket("lw", a, k, self.S.LW_APPLY, kdtype, kbytes, self.side)
                 self.kernel_launches += 1
             else:
                 self.symm.launch_allreduce(a, self._algo[b.index], kdtype, kbytes, self.side)
@@ -532,11 +515,11 @@ class FusedEngine:
         k.nesterov = int(bool(group["nesterov"]))
         k.lr_mode = 1 if group["adjust_lr_fn"] == "match_rms_adamw" else 0
         k.eps = float(group["eps"])
-        self.symm.launch_muon_bucket(a, k, S.MUON_REDUCE, kdtype, kbytes, self.side)
-        self.symm.launch_muon_bucket(a, k, S.MUON_NORMALIZE, kdtype, kbytes, self.side)
+        self.symm.launch_bucket("muon", a, k, S.MUON_REDUCE, kdtype, kbytes, self.side)
+        self.symm.launch_bucket("muon", a, k, S.MUON_NORMALIZE, kdtype, kbytes, self.side)
         with torch.cuda.stream(self.side):
             k.o = self._newton_schulz(b, group).data_ptr()
-        self.symm.launch_muon_bucket(a, k, S.MUON_APPLY, kdtype, kbytes, self.side)
+        self.symm.launch_bucket("muon", a, k, S.MUON_APPLY, kdtype, kbytes, self.side)
         self.kernel_launches += 2
 
     @contextlib.contextmanager
@@ -571,8 +554,8 @@ class FusedEngine:
             for b in self.buckets:
                 ap = self._apply_args[b.index]
                 self._fill_hyper(ap, self.opt.param_groups[b.group_index])
-                self.symm.launch_clip_bucket(ap, self._clip_args[b.index], self.S.CLIP_APPLY, self._kdtype[b.index],
-                                             self._kbytes[b.index], self.side)
+                self.symm.launch_bucket("clip", ap, self._clip_args[b.index], self.S.CLIP_APPLY,
+                                        self._kdtype[b.index], self._kbytes[b.index], self.side)
                 self.kernel_launches += 1
 
     def after_step(self):

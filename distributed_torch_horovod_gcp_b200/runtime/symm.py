@@ -67,10 +67,15 @@ class LwChunk(ctypes.Structure):
                 ("tcount", ctypes.c_int)]
 
 
+class ChunkArgs(ctypes.Structure):
+    _fields_ = [("r", ctypes.c_uint64), ("part", ctypes.c_uint64), ("chunks", ctypes.c_uint64),
+                ("nchunks", ctypes.c_int), ("pad_", ctypes.c_int)]
+
+
 class LwArgs(ctypes.Structure):
-    _fields_ = [("r", ctypes.c_uint64), ("part", ctypes.c_uint64), ("ratio", ctypes.c_uint64),
-                ("chunks", ctypes.c_uint64), ("nchunks", ctypes.c_int), ("adaptive", ctypes.c_int),
-                ("trust_coef", ctypes.c_float), ("pad_", ctypes.c_int)]
+    _anonymous_ = ("tab",)          # k.r, k.part, k.chunks, k.nchunks reach the embedded ChunkArgs
+    _fields_ = [("tab", ChunkArgs), ("ratio", ctypes.c_uint64), ("adaptive", ctypes.c_int),
+                ("trust_coef", ctypes.c_float)]
 
 
 LW_REDUCE, LW_APPLY = 0, 1
@@ -81,10 +86,9 @@ class MuonMat(ctypes.Structure):
 
 
 class MuonArgs(ctypes.Structure):
-    _fields_ = [("r", ctypes.c_uint64), ("part", ctypes.c_uint64), ("chunks", ctypes.c_uint64),
-                ("mats", ctypes.c_uint64), ("x0", ctypes.c_uint64), ("o", ctypes.c_uint64),
-                ("nchunks", ctypes.c_int), ("nesterov", ctypes.c_int), ("lr_mode", ctypes.c_int),
-                ("eps", ctypes.c_float)]
+    _anonymous_ = ("tab",)
+    _fields_ = [("tab", ChunkArgs), ("mats", ctypes.c_uint64), ("x0", ctypes.c_uint64), ("o", ctypes.c_uint64),
+                ("nesterov", ctypes.c_int), ("lr_mode", ctypes.c_int), ("eps", ctypes.c_float), ("pad_", ctypes.c_int)]
 
 
 MUON_REDUCE, MUON_NORMALIZE, MUON_APPLY = 0, 1, 2
@@ -195,35 +199,21 @@ class KernelLauncher:
         self._launched(self.lib.b200dp_comm_allreduce(ctypes.byref(self.ctx), ctypes.byref(args), algo,
                                                       _DTYPE_CODE[dtype], blocks, 512, stream.cuda_stream))
 
-    def launch_clip_bucket(self, args: ARArgs, clip: ClipArgs, phase: int, dtype: torch.dtype, nbytes: int,
-                           stream: torch.cuda.Stream):
-        """One bucket of the clip-mode engine: ``CLIP_REDUCE`` (one-shot reduction into ``clip.r`` plus the
-        per-CTA norm slots) or ``CLIP_APPLY`` (scale ``clip.r`` by the clip coefficient, optimizer update).
-        Both phases of a bucket use the same grid, so the reduce phase fills the same slots every step."""
+    def launch_bucket(self, mode: str, args: ARArgs, k, phase: int, dtype: torch.dtype, nbytes: int,
+                      stream: torch.cuda.Stream):
+        """One phase of a bucket of the engine modes that split the bucket kernel, through the C entry point
+        ``b200dp_comm_<mode>_bucket``: ``mode`` "clip" with ``ClipArgs`` ``k`` (``CLIP_REDUCE`` / ``CLIP_APPLY``),
+        "lw" with ``LwArgs`` (LARS / LAMB: ``LW_REDUCE`` / ``LW_APPLY``) or "muon" with ``MuonArgs``
+        (``MUON_REDUCE`` / ``MUON_NORMALIZE`` / ``MUON_APPLY``).  Every phase of a bucket runs on the same one-shot
+        grid, so the clip reduce phase fills the same norm slots every step."""
+        entry = getattr(self.lib, f"b200dp_comm_{mode}_bucket")
         blocks = self.pick_blocks(ALGO_ONESHOT, nbytes)
-        self._launched(self.lib.b200dp_comm_clip_bucket(ctypes.byref(self.ctx), ctypes.byref(args), ctypes.byref(clip),
-                                                        phase, _DTYPE_CODE[dtype], blocks, 512, stream.cuda_stream))
+        self._launched(entry(ctypes.byref(self.ctx), ctypes.byref(args), ctypes.byref(k), phase, _DTYPE_CODE[dtype],
+                             blocks, 512, stream.cuda_stream))
 
     def launch_clip_finalize(self, clip: ClipArgs, stream: torch.cuda.Stream):
         """Sum every bucket's norm slots (fixed order) into the global norm and the clip coefficient."""
         self._launched(self.lib.b200dp_comm_clip_finalize(ctypes.byref(clip), stream.cuda_stream))
-
-    def launch_lw_bucket(self, args: ARArgs, lw: LwArgs, phase: int, dtype: torch.dtype, nbytes: int,
-                         stream: torch.cuda.Stream):
-        """One bucket of a LARS / LAMB engine: ``LW_REDUCE`` (one-shot reduction, update direction into
-        ``lw.r``, per-chunk sums of squares) or ``LW_APPLY`` (per-tensor trust ratios, update, step counter)."""
-        blocks = self.pick_blocks(ALGO_ONESHOT, nbytes)
-        self._launched(self.lib.b200dp_comm_lw_bucket(ctypes.byref(self.ctx), ctypes.byref(args), ctypes.byref(lw),
-                                                      phase, _DTYPE_CODE[dtype], blocks, 512, stream.cuda_stream))
-
-    def launch_muon_bucket(self, args: ARArgs, mu: MuonArgs, phase: int, dtype: torch.dtype, nbytes: int,
-                           stream: torch.cuda.Stream):
-        """One phase of a Muon bucket: ``MUON_REDUCE`` (one-shot reduction, momentum, u into ``mu.r``, per-chunk
-        sums of squares), ``MUON_NORMALIZE`` (per-matrix norms, bf16 NS inputs into ``mu.x0``) or ``MUON_APPLY``
-        (decay and NS result ``mu.o`` applied, step counter)."""
-        blocks = self.pick_blocks(ALGO_ONESHOT, nbytes)
-        self._launched(self.lib.b200dp_comm_muon_bucket(ctypes.byref(self.ctx), ctypes.byref(args), ctypes.byref(mu),
-                                                        phase, _DTYPE_CODE[dtype], blocks, 512, stream.cuda_stream))
 
 
 class SymmRuntime(KernelLauncher):
@@ -335,10 +325,7 @@ class SymmRuntime(KernelLauncher):
         L.b200dp_comm_clip_bucket.argtypes = [P(CommCtx), P(ARArgs), P(ClipArgs), i, i, i, i, u64]
         L.b200dp_comm_clip_finalize.argtypes = [P(ClipArgs), u64]
         L.b200dp_comm_lw_bucket.argtypes = [P(CommCtx), P(ARArgs), P(LwArgs), i, i, i, i, u64]
-        if hasattr(L, "b200dp_comm_muon_bucket"):
-            L.b200dp_comm_muon_bucket.argtypes = [P(CommCtx), P(ARArgs), P(MuonArgs), i, i, i, i, u64]
-            if L.b200dp_comm_muon_bytes() != ctypes.sizeof(MuonArgs):
-                raise RuntimeError("ctypes/C struct layout mismatch: MuonArgs")
+        L.b200dp_comm_muon_bucket.argtypes = [P(CommCtx), P(ARArgs), P(MuonArgs), i, i, i, i, u64]
         if hasattr(L, "b200dp_comm_collective"):
             L.b200dp_comm_collective.argtypes = [P(CommCtx), P(CollArgs), i, i, i, i, u64]
             if L.b200dp_comm_coll_bytes() != ctypes.sizeof(CollArgs):
@@ -348,9 +335,10 @@ class SymmRuntime(KernelLauncher):
                 raise RuntimeError("ctypes/C struct layout mismatch: GroupCollArgs")
         lim = [ctypes.c_int() for _ in range(6)]
         L.b200dp_comm_limits(*[ctypes.byref(x) for x in lim])
-        got = tuple(x.value for x in lim) + (L.b200dp_comm_clip_bytes(), L.b200dp_comm_lw_bytes())
+        got = tuple(x.value for x in lim) + (L.b200dp_comm_clip_bytes(), L.b200dp_comm_lw_bytes(),
+                                             L.b200dp_comm_muon_bytes())
         want = (MAX_RANKS, MAX_BLOCKS, NUM_CHANNELS, ctypes.sizeof(CommCtx), ctypes.sizeof(ARArgs),
-                ctypes.sizeof(BcastArgs), ctypes.sizeof(ClipArgs), ctypes.sizeof(LwArgs))
+                ctypes.sizeof(BcastArgs), ctypes.sizeof(ClipArgs), ctypes.sizeof(LwArgs), ctypes.sizeof(MuonArgs))
         if got != want:
             raise RuntimeError(f"ctypes/C struct layout mismatch: C={got} python={want}")
 

@@ -46,12 +46,13 @@ def _call(lib, S, entry, cfg):
         a.channel, a.n = cfg["channel"], cfg["size"]
         return lib.b200dp_comm_clip_bucket(b(ctx), b(a), b(k), cfg["sel"], cfg["dtype"], cfg["blocks"],
                                            cfg["threads"], 0)
-    if entry == "lw_bucket":
-        a, k = S.ARArgs(), S.LwArgs()
-        a.channel, a.h.kind = cfg["channel"], cfg.get("kind", S.OPT_LARS)
+    if entry in ("lw_bucket", "muon_bucket"):
+        lw = entry == "lw_bucket"
+        a, k = S.ARArgs(), S.LwArgs() if lw else S.MuonArgs()
+        a.channel, a.h.kind = cfg["channel"], cfg.get("kind", S.OPT_LARS if lw else S.OPT_MUON)
         k.nchunks = cfg.get("nchunks", 1)
-        return lib.b200dp_comm_lw_bucket(b(ctx), b(a), b(k), cfg["sel"], cfg["dtype"], cfg["blocks"],
-                                         cfg["threads"], 0)
+        return getattr(lib, f"b200dp_comm_{entry}")(b(ctx), b(a), b(k), cfg["sel"], cfg["dtype"], cfg["blocks"],
+                                                    cfg["threads"], 0)
     if entry == "collective":
         a = S.CollArgs()
         a.channel, a.chunk = cfg["channel"], cfg["size"]
@@ -61,18 +62,19 @@ def _call(lib, S, entry, cfg):
     return lib.b200dp_comm_broadcast(b(ctx), b(a), cfg["blocks"], cfg["threads"], 0)
 
 
-# the selector's range: algo 0..2, phase 0..1, collective mode 0..2; broadcast has neither selector nor dtype
-SEL_LIMIT = {"allreduce": 3, "clip_bucket": 2, "lw_bucket": 2, "collective": 3}
+# the selector's range: algo 0..2, phase 0..1 (Muon 0..2), collective mode 0..2; broadcast has neither selector
+# nor dtype
+SEL_LIMIT = {"allreduce": 3, "clip_bucket": 2, "lw_bucket": 2, "muon_bucket": 3, "collective": 3}
 
 
-@pytest.mark.parametrize("entry", ["allreduce", "clip_bucket", "lw_bucket", "collective", "broadcast"])
+@pytest.mark.parametrize("entry", ["allreduce", "clip_bucket", "lw_bucket", "muon_bucket", "collective", "broadcast"])
 @pytest.mark.parametrize("field,value", BAD)
 def test_bad_launch_config_is_rejected(comm, entry, field, value):
     lib, S = comm
     if entry == "broadcast" and field in ("sel", "dtype"):
         pytest.skip("broadcast takes no selector or dtype")
-    if entry == "lw_bucket" and field == "size":
-        pytest.skip("the layer-wise kernels walk the chunk table, not n")
+    if entry in ("lw_bucket", "muon_bucket") and field == "size":
+        pytest.skip("the layer-wise and Muon kernels walk the chunk table, not n")
     if field == "sel" and value == 3:
         value = SEL_LIMIT[entry]
     cfg = dict(GOOD, **{field: value})
@@ -81,13 +83,16 @@ def test_bad_launch_config_is_rejected(comm, entry, field, value):
     assert msg.startswith("bad ") and "launch" in msg, msg
 
 
-@pytest.mark.parametrize("kind,nchunks", [("OPT_SGD", 1), ("OPT_ADAM", 1), ("OPT_LARS", -1)])
-def test_layerwise_rejects_other_optimizers_and_negative_chunks(comm, kind, nchunks):
+@pytest.mark.parametrize("entry,kind,nchunks", [
+    ("lw_bucket", "OPT_SGD", 1), ("lw_bucket", "OPT_ADAM", 1), ("lw_bucket", "OPT_LARS", -1),
+    ("muon_bucket", "OPT_LAMB", 1), ("muon_bucket", "OPT_MUON", -1)])
+def test_chunked_buckets_reject_other_optimizers_and_negative_chunks(comm, entry, kind, nchunks):
     lib, S = comm
     cfg = dict(GOOD, kind=getattr(S, kind), nchunks=nchunks)
-    assert _call(lib, S, "lw_bucket", cfg) == -1
+    assert _call(lib, S, entry, cfg) == -1
     msg = lib.b200dp_comm_last_error().decode()
-    assert msg.startswith("bad layer-wise launch") and f"kind={getattr(S, kind)}" in msg, msg
+    what = "layer-wise" if entry == "lw_bucket" else "muon"
+    assert msg.startswith(f"bad {what} launch") and f"kind={getattr(S, kind)}" in msg, msg
 
 
 @pytest.mark.parametrize("entry", ["allreduce", "clip_bucket", "collective"])
